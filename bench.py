@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py -- DRRs/sec fwd+bwd (512^3 CT -> 256^2 detector) and achieved algorithmic HBM GB/s vs the B200 peak.
+"""bench.py -- DRRs/sec fwd+bwd (512^3 CT -> 256^2 detector) and achieved algorithmic HBM GB/s vs the H100 peak.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--dump-outputs DIR]
 
 A "step" is one pass of the hot path over one batch of synthetic poses: Siddon forward (line integrals of
 `--batch` poses through a 512^3 fp32 volume onto a 256^2 detector) + Siddon backward (gradients w.r.t. the ray
@@ -13,7 +13,8 @@ Reported on ONE JSON line:
   value      whole-job DRRs/s with the rays already resident in HBM (kernels only, CUDA-event timed)
   e2e        the same metric through the public module call `DRR(rot, xyz)` + backward, with the pose parameters
              coming from pinned HOST memory every step and the images / loss / pose gradients copied back
-  roofline   algorithmic bytes of the dominant kernel / its CUDA-event duration vs the measured HBM peak
+  roofline   algorithmic bytes of the dominant kernel / its CUDA-event duration vs the HBM peak (MEASURED_PEAKS.json when
+             present, else the H100 SXM data sheet's 3.35 TB/s)
   cpu_baseline  the CPU oracle (C port of the reference algorithm, OpenMP) on a bounded sample, rank 0 only
 
 With N > 1 (torchrun, one rank per GPU, NCCL) the poses are sharded across ranks (weak scaling: `--batch` poses per
@@ -42,14 +43,7 @@ VOL = 512
 DET = 256
 METRIC = "DRRs/sec fwd+bwd (512^3 CT -> 256^2 det)"
 WORKLOAD = "siddon fwd+bwd(pose), 512^3 fp32 CT -> 256^2 detector"
-HBM_FALLBACK_GBS = 6650.0  # /opt/skills/guides/B200_PROFILING.md fallback
-# dram__bytes_read.sum + dram__bytes_write.sum per launch from `ncu --set full` captures of the default workload
-# (16 poses, 512^3 -> 256^2): profiles/r01_fwd_slab_B16_ncu_summary.txt and gpurun capture of the backward kernel.
-# Only quoted when the run uses that workload; otherwise null.
-NCU_TRAFFIC_SOURCE = ("not measured by this run: dram__bytes_read.sum + dram__bytes_write.sum of one `ncu --set full` capture of "
-                      "the same command (profiles/r02_siddon_sens_slab_ncu_summary.txt, captured 2026-09-24 on a B200 of this pool); null off the default workload")
-NCU_TRAFFIC_BYTES = {"siddon_fwd_slab_kernel": 1.05e9 + 0.02e9, "siddon_bwd_slab_kernel": 2.26e9 + 0.09e9,
-                     "siddon_sens_slab_kernel": 1.4126e9 + 0.1360e9}
+HBM_FALLBACK_GBS = 3350.0  # NVIDIA H100 SXM data sheet (HBM3)
 
 
 def parse():
@@ -66,7 +60,12 @@ def parse():
     ap.add_argument("--no-extra", action="store_true", help="skip the secondary BASELINE configs / reference-on-GPU legs")
     ap.add_argument("--workload", default="metric", choices=["metric", "config4"],
                     help="metric = BASELINE.json's metric workload (default); config4 = 512^3 -> 1024^2, 256 poses sharded over the GPUs")
-    return ap.parse_args()
+    ap.add_argument("--dump-outputs", metavar="DIR",
+                    help="after the timed steps, write what the timed path computed in its last step as DIR/<name>.npy")
+    args = ap.parse_args()
+    if args.dump_outputs and args.impl == "reference":
+        ap.error("--dump-outputs writes what the GPU path computed; --impl reference times the CPU port instead")
+    return args
 
 
 def hbm_peak():
@@ -76,7 +75,7 @@ def hbm_peak():
             return float(json.load(open(path))["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
         except Exception:
             pass
-    return HBM_FALLBACK_GBS, "fallback (B200_PROFILING.md)"
+    return HBM_FALLBACK_GBS, "data sheet (NVIDIA H100 SXM, HBM3)"
 
 
 class ClockSampler:
@@ -307,6 +306,24 @@ def run_reference(args, rank, world):
 # ---------------------------------------------------------------------------------------------------------------
 # GPU arm
 # ---------------------------------------------------------------------------------------------------------------
+DUMP_BYTES = 64 << 20
+
+
+def dump_outputs(directory, arrays):
+    """Writes each array as directory/<name>.npy in float32.  An array larger than its share of DUMP_BYTES is cut to a
+    seeded sample of its flattened elements (fixed seed: the same elements for the same arguments, so two builds of the
+    project can be compared output for output)."""
+    os.makedirs(directory, exist_ok=True)
+    share = DUMP_BYTES // len(arrays)
+    for name, t in arrays.items():
+        t = t.detach().float()
+        if t.numel() * 4 > share:
+            g = torch.Generator().manual_seed(0)
+            idx = torch.randint(0, t.numel(), (share // 4,), generator=g).unique()
+            t = t.reshape(-1)[idx.to(t.device)]
+        np.save(os.path.join(directory, name + ".npy"), t.cpu().numpy())
+
+
 def _time_events(fn, steps, warmup=2):
     """Per-launch CUDA-event times (ms) of fn on the current stream."""
     for _ in range(warmup):
@@ -568,7 +585,7 @@ def extra_configs(dev, lib, peak, main):
 
 
 def reference_on_gpu(vol_n, det_n):
-    """SURVEY 2b's bar: the reference's own PyTorch path (`Siddon.forward` + autograd) under .to("cuda") on this B200,
+    """SURVEY 2b's bar: the reference's own PyTorch path (`Siddon.forward` + autograd) under .to("cuda") on this GPU,
     512^3 -> 256^2, ONE pose, forward + backward (it materialises ~20 (1, 65536, 1539) tensors; B = 16 would not fit the
     comparison's spirit of a single call).  Wall clock around synchronised calls, 1 warm-up + 5 runs."""
     ref_mod = load_reference()
@@ -578,7 +595,7 @@ def reference_on_gpu(vol_n, det_n):
         run = ReferenceRun(ref_mod, vol_n, det_n, device="cuda")
         run.step(run.n_total)
         times = [run.step(run.n_total) for _ in range(5)]
-        return {"workload": f"reference Siddon.forward + backward on the same B200, {vol_n}^3 -> {det_n}^2, 1 pose per call",
+        return {"workload": f"reference Siddon.forward + backward on the same GPU, {vol_n}^3 -> {det_n}^2, 1 pose per call",
                 "drr_per_s": 1.0 / float(np.median(times)), "median_s": float(np.median(times)), "min_s": float(np.min(times)),
                 "peak_memory_gb": torch.cuda.max_memory_allocated() / 1e9}
     except Exception as exc:
@@ -613,7 +630,7 @@ def run_ours(args, rank, local_rank, world):
     rot_all, xyz_all = synthetic.make_poses(B * world, seed=0)
     mine = list(range(rank * B, (rank + 1) * B))
     balance = "contiguous slices"
-    if world > 1 and os.environ.get("B200DRR_BENCH_BALANCE", "0") == "1":  # opt-in: measured 1.3 % SLOWER at N = 8 (DESIGN.md 6)
+    if world > 1 and os.environ.get("B200DRR_BENCH_BALANCE", "0") == "1":  # opt-in (DESIGN.md 6)
         # every rank still renders exactly B poses (weak scaling), but WHICH poses is decided by their cost (voxels visited,
         # known from a closed-form count): the step ends when the slowest rank does
         from diffdrr_b200.parallel import balanced_pose_assignment
@@ -731,6 +748,9 @@ def run_ours(args, rank, local_rank, world):
         t_end.record(stream)
         barrier()
     ms_total = t_start.elapsed_time(t_end)
+    if args.dump_outputs and rank == 0:  # the legs below overwrite these buffers
+        dump_outputs(args.dump_outputs, {"image": outs[(state["k"] - 1) & 1] if world > 1 else outs[0],
+                                         "g_source": g_src, "g_target": g_tgt, "g_raylen": g_len})
     sens_list = [e[0].elapsed_time(e[1]) for e in events]
     sens_bwd_list = [e[1].elapsed_time(e[2]) for e in events]
     sens_ms = float(np.mean(sens_list))
@@ -873,7 +893,7 @@ def run_ours(args, rank, local_rank, world):
         "dtype": "f32", "data": "synthetic",
         "config": {"workload": WORKLOAD, "volume": [D] * 3, "detector": [args.det] * 2, "batch_per_gpu": B,
                    "global_batch": B * world, "renderer": "siddon", "parallelism": f"pose-sharded dp{world}", "gather": gather_kind, "pose_assignment": balance,
-                   "l2": f"inputs > L2 ({4 * D ** 3 / 1e6:.0f} MB volume vs 126 MB L2); no explicit flush",
+                   "l2": f"inputs > L2 ({4 * D ** 3 / 1e6:.0f} MB volume vs 50 MB L2); no explicit flush",
                    "mean_visits_per_ray": tot_visits / (B * N)},
         "e2e": {"value": e2e_value, "unit": "DRRs/s", "ms_per_step": e2e_ms_total / args.steps, "mode": e2e_mode,
                 "eager_value": total_drr / (e2e_eager_ms_total * 1e-3), "eager_ms_per_step": e2e_eager_ms_total / args.steps,
@@ -882,8 +902,7 @@ def run_ours(args, rank, local_rank, world):
                 "path": "DRR(rot, xyz) -> (img*w).sum().backward(); pinned host pose in; image stack + loss + pose grads out"},
         "gpu_launches": 2 * args.steps,
         "roofline": {"bound": "hbm", "kernel": dom[0], "achieved": dom[1], "peak": peak, "unit": "GB/s", "frac": dom[1] / peak,
-                     "traffic": NCU_TRAFFIC_BYTES.get(dom[0]) if (B, D, args.det) == (16, VOL, DET) else None,
-                     "traffic_source": NCU_TRAFFIC_SOURCE, "algorithmic_bytes_per_launch": dom[2], "ms_per_launch": dom[3], "peak_source": peak_src},
+                     "traffic": None, "algorithmic_bytes_per_launch": dom[2], "ms_per_launch": dom[3], "peak_source": peak_src},
         "step_breakdown_ms": {"siddon_sens_slab_kernel (image + sensitivities, one walk)": sens_ms,
                               "sens_bwd_kernel (elementwise backward)": sens_bwd_ms},
         "roofline_fwd": {"kernel": "siddon_fwd_slab_kernel (b200drr_siddon_fwd_grid's choice for this batch: rays cut into major-axis "
@@ -1035,6 +1054,8 @@ def run_config4(args, rank, local_rank, world):
         e1.record()
         barrier()
     ms_total = e0.elapsed_time(e1)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, {"image": out})
     t_brick = _time_events(brick, 3, warmup=1)
     t_slab = _time_events(slab, 3, warmup=1)
     stats = torch.tensor([ms_total, float(np.median(t_brick)), float(np.median(t_slab)), float(visits)], device=dev, dtype=torch.float64)

@@ -1,4 +1,4 @@
-"""diffdrr_b200 -- a Blackwell-native (sm_100a) differentiable DRR projector with DiffDRR's `DRR` module surface.
+"""diffdrr_b200 -- a Hopper-native (sm_90a) differentiable DRR projector with DiffDRR's `DRR` module surface.
 
 Hot path (Siddon + trilinear renderers, forward and backward) = hand-written CUDA kernels behind the C ABI of
 include/b200drr.h; host code (pose, detector geometry, module plumbing) = PyTorch.  No CPU fallback.

@@ -236,7 +236,7 @@ def load():
         if not os.path.exists(path):
             raise B200DRRError(
                 f"{path} is missing: build it with `python -c 'import __graft_entry__ as g; g.build()'` "
-                "(nvcc, sm_100a). diffdrr_b200 has no CPU or PyTorch fallback.")
+                "(nvcc, sm_90a). diffdrr_b200 has no CPU or PyTorch fallback.")
         handle = ctypes.CDLL(path)
         for name, (restype, argtypes) in _SIGNATURES.items():
             fn = getattr(handle, name)  # AttributeError if the ABI and the header drift apart

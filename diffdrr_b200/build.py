@@ -1,4 +1,4 @@
-"""Build recipe for libb200drr.so (hand-written sm_100a CUDA kernels + the C ABI of include/b200drr.h).
+"""Build recipe for libb200drr.so (hand-written sm_90a CUDA kernels + the C ABI of include/b200drr.h).
 
 The library is built IN-TREE (diffdrr_b200/libb200drr.so) with nvcc, so the artefact travels with a
 `gpurun` snapshot; nvcc cross-compiles without a GPU.  No torch headers are involved: the boundary is a
@@ -15,7 +15,7 @@ CSRC = os.path.join(_HERE, "csrc")
 LIB_PATH = os.path.join(_HERE, "libb200drr.so")
 SOURCES = ["siddon.cu", "siddon_brick.cu", "trilinear.cu", "literal.cu", "pose.cu", "ncc.cu", "capi.cu"]
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17", "-Xcompiler", "-fPIC", "-shared",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17", "-Xcompiler", "-fPIC", "-shared",
 ]
 
 
@@ -36,7 +36,7 @@ def _stale() -> bool:
 
 
 def build(force: bool = False, verbose: bool = False) -> str:
-    """Compile the CUDA extension for sm_100a if it is missing or older than its sources."""
+    """Compile the CUDA extension for sm_90a if it is missing or older than its sources."""
     if not force and not _stale():
         return LIB_PATH
     cmd = [_nvcc(), *NVCC_FLAGS, "-o", LIB_PATH + ".tmp", *[os.path.join(CSRC, s) for s in SOURCES]]

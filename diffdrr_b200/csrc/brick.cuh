@@ -319,7 +319,8 @@ B200_HD float acc_step(AccState& s, const AccConst& k)
     asm("{\n\t"
         ".reg .pred q, p0, p1, p2;\n\t"
         ".reg .f32 nx;\n\t"
-        "min.f32 nx, %0, %1, %2;\n\t"
+        "min.f32 nx, %0, %1;\n\t"
+        "min.f32 nx, nx, %2;\n\t"
         "sub.f32 %5, nx, %3;\n\t"
         "mov.f32 %3, nx;\n\t"
         "setp.lt.f32 q, nx, %6;\n\t"

@@ -1,4 +1,4 @@
-// common.cuh -- shared helpers for the sm_100a DRR kernels.
+// common.cuh -- shared helpers for the sm_90a DRR kernels.
 //
 // The per-ray math (ray_math.cuh) is written as host+device functions so that tests/hostemu can compile the very
 // same source with g++ and check it against the oracle in the CPU-only container.  That emulation is test
@@ -29,7 +29,7 @@ struct VolDims {
 B200_HD float ldg(const float* p)
 {
 #if defined(__CUDA_ARCH__)
-    return __ldg(p);  // (an L2::256B prefetch hint was measured: no effect, L2 already hits 80 %)
+    return __ldg(p);  // (an L2::256B prefetch hint was tried: no effect)
 #else
     return *p;
 #endif
@@ -64,6 +64,17 @@ B200_HD void red_add(float* addr, float v)
     *addr += v;
 #endif
 }
+
+#if defined(__CUDACC__)
+// SMs of the current device: the grid-stride launches size their grids from it
+inline int current_sm_count()
+{
+    int dev = 0, sms = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess)
+        return 1;
+    return sms;
+}
+#endif
 
 // One ray: d = (target - source) + eps (renderers.py:104-106), inv = 1/d.
 struct Ray {

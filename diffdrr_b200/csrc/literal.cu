@@ -1,4 +1,4 @@
-// literal.cu -- reference-literal Siddon / trilinear renderers for sm_100a, templated on the real type.
+// literal.cu -- reference-literal Siddon / trilinear renderers for sm_90a, templated on the real type.
 //
 // Two uses, both off the fast paths:
 //   * fp64: the reference reaches double precision through `drr.to(torch.float64)` (drr.py:75 comment, utils.py:110);

@@ -1,4 +1,4 @@
-// ncc.cu -- zero-normalised cross correlation of two image stacks and its gradient, three launches per training step (sm_100a).
+// ncc.cu -- zero-normalised cross correlation of two image stacks and its gradient, three launches per training step (sm_90a).
 //
 // Replaces reference diffdrr/metrics.py:21-44 (NormalizedCrossCorrelation2d, patch_size = None) on the registration loop
 // (registration.py:14-50 + the loss): ~40 ATen launches per step of a loop whose renderer takes 0.14 ms -- at one pose per

@@ -1,4 +1,4 @@
-// pose.cu -- the per-pose algebra either side of the pose-in kernels, one kernel each way (sm_100a).
+// pose.cu -- the per-pose algebra either side of the pose-in kernels, one kernel each way (sm_90a).
 //
 // DRR.forward turns pose parameters into the (src, G, Wd) triple of b200drr_siddon_fwd_pose through ~95 tiny ATen kernels per
 // training step (cos/sin/stack/bmm/cat and their autograd twins): 0.25 ms of a 1.6 ms step.  Here the same algebra is

@@ -2,8 +2,7 @@
 //
 // Why: with one lane per ray, the lanes of a warp that advance "one voxel per step" drift apart in depth (each
 // ray interleaves its minor-axis crossings differently), so a warp-wide gather touches ~one 32-byte sector PER
-// LANE and the L1 wavefront / miss-request pipes saturate (ncu: 22 sectors and 9.7 wavefronts per request,
-// profiles/).  Here every lane advances exactly one plane of its MAJOR axis (argmax |d|) per iteration, so the
+// LANE and the L1 wavefront / miss-request pipes saturate (many sectors and wavefronts per request).  Here every lane advances exactly one plane of its MAJOR axis (argmax |d|) per iteration, so the
 // 32 lanes of an 8x4 ray bundle always read from the same voxel plane and share sectors.
 //
 // Inside one major slab (between two consecutive major planes) a ray with minor slopes |d_u/d_m|, |d_v/d_m| <= 1

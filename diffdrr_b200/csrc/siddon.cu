@@ -1,4 +1,4 @@
-// siddon.cu -- Siddon exact-path DRR kernels for sm_100a (forward, backward, visit counter).
+// siddon.cu -- Siddon exact-path DRR kernels for sm_90a (forward, backward, visit counter).
 // One thread walks one ray (ray_math.cuh); blockIdx.y is the pose, blockIdx.x tiles the rays of that pose.
 #include <stdlib.h>
 
@@ -40,7 +40,7 @@ __global__ void __launch_bounds__(kThreads) siddon_fwd_fast_kernel(const float* 
     const int64_t r = (int64_t)b * N + n;
     const Ray ray = load_ray(src, tgt, b, r, eps);
     // arbitrary ray sets (sub-sampled / patched / user rays): no tiling is possible, the kernel is bound by DRAM/L2
-    // locality (measured: the lean walk is 10 % SLOWER here because it thrashes the caches faster), so keep the plain walk
+    // locality (the lean walk was slower here because it thrashes the caches faster), so keep the plain walk
     out[r] = __ldg(raylen + r) * siddon_ray_fast<false>(vol, dims, ray, shift, nullptr);
 }
 
@@ -141,7 +141,7 @@ __global__ void __launch_bounds__(TW* TH) siddon_fwd_grid_kernel(const float* __
 
 // ---------------------------------------------------------------------------------------------------
 // Slab-major detector-grid kernel.  The volume is cut into slabs of `slab` planes along axis 0 (the
-// slowest axis: a slab is one contiguous chunk of memory sized to stay resident in the 126 MB L2).
+// slowest axis: a slab is one contiguous chunk of memory sized to stay resident in the 50 MB L2).
 // blockIdx.x enumerates (slab, pose, tile) with the slab SLOWEST, so the CTAs in flight at any time --
 // across all poses of the batch -- gather from the same few slabs and the volume streams from HBM about
 // once per BATCH instead of once per pose.  Each CTA integrates its rays over its slab only (splitting a
@@ -222,7 +222,7 @@ cudaError_t launch_x_transpose_volume(const float* vol, VolDims dims, int axis, 
     const int64_t total = (int64_t)dims.d[0] * dims.d[1] * dims.d[2];
     cudaError_t e = cudaMemsetAsync(out + total, 0, sizeof(float) * 4, stream);  // the padding chunk
     if (e != cudaSuccess) return e;
-    transpose_volume_kernel<<<148 * 8, 256, 0, stream>>>(vol, dims, axis, out);
+    transpose_volume_kernel<<<current_sm_count() * 8, 256, 0, stream>>>(vol, dims, axis, out);
     return cudaGetLastError();
 }
 
@@ -498,7 +498,7 @@ cudaError_t launch_siddon_fwd_pose(const float* vol, VolDims dims, const float* 
     if (pieces > 0 && (int64_t)dims.d[0] * dims.d[1] * dims.d[2] < (int64_t)INT32_MAX)
         return launch_slab_variant<16, 16, 4, true>(vol, dims, src, nullptr, nullptr, out, B, H, W, pieces, shift, eps, stream,
                                                     PoseRays{G, Wd, rows, cols});
-    return launch_slab_variant<16, 16, 4>(vol, dims, src, nullptr, nullptr, out, B, H, W, 32, shift, eps, stream,
+    return launch_slab_variant<16, 16, 4>(vol, dims, src, nullptr, nullptr, out, B, H, W, 16, shift, eps, stream,
                                           PoseRays{G, Wd, rows, cols});
 }
 
@@ -732,14 +732,14 @@ cudaError_t launch_x_siddon_sens_chunk(const float* volT, VolDims dims, int axis
 #endif  // B200DRR_EXPERIMENTS
 
 // Major-axis pieces (MAJ kernels): every ray is cut into K pieces along its OWN major axis, a thread per (ray, piece).
-// Why: (1) the registration loop renders ONE pose per step -- 256^2 rays are 21 % of a B200's thread slots, each walking ~670
+// Why: (1) the registration loop renders ONE pose per step -- 256^2 rays are 24 % of an H100's thread slots, each walking ~670
 // voxels in series; (2) slabs along a FIXED axis give a ray that runs across them one to three pieces of very different length,
 // so the lanes of a warp finish at different times, while the major-axis pieces of a warp's rays carry equal shares of the visits.
-// Measured on B200, 512^3 -> 256^2 (profiles/r02_tune_small_batch.log; us per launch):
-//   forward   B = 1: 187 (32-plane slabs) -> 95 (K = 12);  2: 250 -> 152;  4: 365 -> 248;  8: 601 (brick 591) -> 504;
-//             16: 1142 (brick 1099) -> 1032 (K = 16)  -- the fastest forward kernel at every batch size measured (41 % of HBM roofline)
-//   sens      B = 1: 193 (thread per ray) -> 115 (K = 8..16);  2: 281 -> 192;  4: 394 (96-plane slabs) -> 312;  8: 637 (48-plane
-//             slabs) -> 639;  16: 1243 -> 1273  -- the slab-major kernel keeps batches >= 8 (its volume re-use through L2 pays there)
+// H100, 512^3 -> 256^2 (scripts/tune_thresholds.py; us per launch, pieces K = 16 / best slab height, 16 planes):
+//   forward          1 pose 124 / 157,  4: 538 / 777,  8: 1167 / 1331,  16: 2479 / 2479,  32: 5071 / 4571
+//   sensitivities    1 pose 139 / 180,  2: 388 / 504,  4: 625 / 701,  8: 1330 / 1265,  16: 2679 / 2402,  32: 5411 / 4484
+// so the forward takes pieces up to 16 poses (the module sends full grids of 2 poses and more to the brick kernel, which beats
+// both) and the sensitivities walk up to 6, both with K = 16; the slab-major kernels keep the bigger batches, with 16-plane slabs.
 // `load` = B * H * W in units of 256^2 rays.  Pieces thinner than ~24 planes only add set-up; volumes below 384^3 were not measured
 // at batch sizes > 4 (the slab-major tuning of BASELINE config 2 stands there), volumes below 96 voxels keep one thread per ray.
 // Returns K, 0 = not used.
@@ -757,7 +757,7 @@ int small_batch_pieces(const VolDims& dims, int B, int H, int W, bool sens)
     const double load = (double)B * H * W / 65536.0;
     const double max_load = dmax < 384 ? 4.0 : (sens ? 6.0 : 16.0);
     if (load > max_load) return 0;
-    int k = (!sens && load > 4.0) ? 16 : 12;
+    int k = (sens || load > 4.0) ? 16 : 12;
     if (k > dmax / 24) k = dmax / 24;
     return k < 2 ? 0 : k;
 }
@@ -789,8 +789,8 @@ cudaError_t launch_siddon_fwd_sens_grid(const float* vol, VolDims dims, const fl
         return launch_sens_slab_variant<8, 16, 8, 8>(vol, dims, src, tgt, raylen, out, sens, B, H, W, dims.d[0], shift, eps,
                                                      stream);
     switch (variant) {
-        SV(0, 8, 16, 8, 48, 8)  // tuned default (profiles/r01_tune_sens.log)
-        SV(38, 8, 16, 8, 48, 8)  // the same kernel by an explicit id, for batches whose default is the major-axis-pieces kernel
+        SV(0, 8, 16, 8, 16, 8)  // default: 16-plane slabs (16.8 MB of a 512^3 fp32 volume, well inside the 50 MB L2)
+        SV(38, 8, 16, 8, 48, 8)
         SV(32, 16, 8, 8, 48, 8)
         SV(33, 8, 16, 8, 128, 8)
         SV(34, 8, 16, 8, 512, 8)
@@ -826,6 +826,9 @@ cudaError_t launch_siddon_fwd_sens_grid(const float* vol, VolDims dims, const fl
         SV(30, 16, 8, 10, 48, 6)
         SV(31, 32, 8, 8, 48, 4)
         SV(21, 8, 8, 8, 32, 16)
+        SV(39, 8, 16, 8, 32, 8)
+        SV(40, 8, 16, 8, 24, 8)
+        SV(41, 8, 16, 8, 16, 8)  // the default kernel by an explicit id, for batches whose default is the major-axis pieces
         default: return cudaErrorInvalidValue;
     }
 #undef SV
@@ -840,9 +843,9 @@ cudaError_t launch_siddon_fwd_sens_pose(const float* vol, VolDims dims, const fl
         return launch_sens_slab_variant<8, 16, 8, 8, true>(vol, dims, src, nullptr, nullptr, out, sens, B, H, W, pieces, shift, eps,
                                                            stream, PoseRays{G, Wd, rows, cols});
     // slabs exist to share the volume through L2 across the poses of a batch; with one or two poses they only repeat the
-    // per-ray set-up (measured at B = 1: 0.147 ms with 48-plane slabs, 0.136 ms unslabbed)
+    // per-ray set-up
     return launch_sens_slab_variant<8, 16, 8, 8>(vol, dims, src, nullptr, nullptr, out, sens, B, H, W,
-                                                 B <= 2 ? dims.d[0] : 48, shift, eps, stream,
+                                                 B <= 2 ? dims.d[0] : 16, shift, eps, stream,
                                                  PoseRays{G, Wd, rows, cols});
 }
 
@@ -984,7 +987,7 @@ cudaError_t launch_siddon_fwd_grid(const float* vol, VolDims dims, const float* 
         if (pieces > 0) return launch_slab_variant<16, 16, 4, true>(vol, dims, src, tgt, raylen, out, B, H, W, pieces, shift, eps, stream);
     }
     switch (variant) {
-        S0(0, 16, 16, 4, 32)
+        S0(0, 16, 16, 4, 16)
         V(30, 16, 8, 4, 1)
         V(1, 16, 8, 8, 0)
         V(2, 16, 8, 2, 1)
@@ -1013,6 +1016,8 @@ cudaError_t launch_siddon_fwd_grid(const float* vol, VolDims dims, const float* 
         S(43, 16, 8, 8, 48)
         S(44, 16, 16, 8, 32)
         S(45, 8, 16, 6, 32)
+        S(46, 16, 16, 4, 16)
+        S(47, 16, 16, 4, 24)
 #undef S
 #ifdef B200DRR_EXPERIMENTS
 #define P(id, TW, TH, U, SLAB, ALIGN) \

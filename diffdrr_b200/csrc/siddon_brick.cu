@@ -1,4 +1,4 @@
-// siddon_brick.cu -- brick-major Siddon forward for sm_100a: TMA-staged voxel bricks in shared memory.
+// siddon_brick.cu -- brick-major Siddon forward for sm_90a: TMA-staged voxel bricks in shared memory.
 //
 // Persistent CTAs (one per SM).  Each CTA claims bricks from a global counter; a brick (BX x BY x BZ fp32 voxels) is
 // brought into shared memory by ONE cp.async.bulk.tensor.3d box copy (zero fill outside the volume) that completes on
@@ -72,11 +72,11 @@ __device__ __forceinline__ void tma_store_wait_read() { asm volatile("cp.async.b
 __device__ __forceinline__ void tma_store_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
 
 // volume-gradient mode: the staged brick is an ACCUMULATOR; fp32 add on a byte address in the shared window
-// (red.shared.add.f32 = an ATOMS.CAST.SPIN loop on sm_100a: there is no native fp32 shared-memory add)
+// (red.shared.add.f32 = an ATOMS.CAST.SPIN loop on sm_90a: there is no native fp32 shared-memory add)
 // SWZ: the brick rows (BZ = 32 floats = 128 B) are stored in TMA's 128-byte swizzle (16-byte chunk index ^= row index & 7, i.e.
 // address bits 4-6 ^= bits 7-9; the brick base is 1024-byte aligned), so lanes that share z but differ in y hit different banks
 // -- the un-swizzled bank is z mod 32 alone, whatever x and y are.  The TMA store of the finished brick undoes it.
-// Measured (profiles/r02_tune_brick_bwd.log): 2.19 -> 1.91 ms at 512^3 -> 256^2 x 16 poses.  -DB200DRR_BWD_SWIZZLE=0 builds the
+// Faster than the plain layout before the port to Hopper (not re-measured on the H100).  -DB200DRR_BWD_SWIZZLE=0 builds the
 // linear layout for A/B runs.
 #ifndef B200DRR_BWD_SWIZZLE
 #define B200DRR_BWD_SWIZZLE 1
@@ -894,8 +894,8 @@ cudaError_t launch_siddon_fwd_brick(const float* vol, VolDims dims, const float*
                                                                                    pix_index, (int)Nr, B, H, W, shift, stream);
     switch (variant) {
         BV(0, 24, 32, 32, 1, 512, 4, 2, 2, 0)    // two CTAs per SM, one 96 KB brick each (production shape)
-        BV(7, 24, 32, 32, 2, 1024, 4, 2, 1, 1)   // one CTA per SM with a two-stage TMA + mbarrier pipeline (measured: 1.27 ms vs 1.09)
-#ifdef B200DRR_EXPERIMENTS   // tuning variants, all measured and not chosen (profiles/r02_tune_brick_*.log); not in the shipped library
+        BV(7, 24, 32, 32, 2, 1024, 4, 2, 1, 1)   // one CTA per SM with a two-stage TMA + mbarrier pipeline (slower: CTA-wide barriers)
+#ifdef B200DRR_EXPERIMENTS   // tuning variants, all measured and not chosen before the port; not in the shipped library
         BV(1, 24, 32, 32, 1, 512, 4, 2, 2, 1)    // ... with the software-pipelined walk
         BV(2, 24, 32, 32, 1, 512, 4, 4, 2, 1)
         BV(3, 24, 32, 32, 1, 512, 4, 4, 2, 0)
@@ -948,11 +948,11 @@ cudaError_t launch_siddon_bwd_vol_brick(const float* gout, VolDims dims, const f
     if (e != cudaSuccess) return e;
     CUtensorMap map;
 #ifndef B200DRR_BWD_U
-#define B200DRR_BWD_U 4  // steps per group of the scatter walk: 2.08 ms (U = 1), 1.91 (2), 1.84 (4) at 512^3 -> 256^2 x 16
+#define B200DRR_BWD_U 4  // steps per group of the scatter walk (4 was the fastest of 1, 2, 4 before the port)
 #endif
-    // Candidate tiles per warp and round (K): bigger rounds = fewer CTA-wide barriers (27 % of the stall samples), at the price of
-    // a smaller brick to keep two CTAs per SM.  Measured (profiles/r02_tune_brick_bwd.log): 16 poses 2.14 ms (K = 2), 1.84 (K = 4,
-    // 24-plane bricks), 1.73 (K = 8, 22-plane bricks); 4 poses 0.61 / 0.55 / 0.57 -- so big batches take K = 8.
+    // Candidate tiles per warp and round (K): bigger rounds = fewer CTA-wide barriers, at the price of
+    // a smaller brick to keep two CTAs per SM.  Tuned before the port (not re-measured on the H100): K = 8
+    // with 22-plane bricks was fastest at 16 poses, K = 4 with 24-plane bricks at 4 -- so big batches take K = 8.
     if (B >= 8) {
         if (!make_volume_map(&map, g_vol, dims, 22, 32, 32, B200DRR_BWD_SWIZZLE != 0)) return cudaErrorNotSupported;
         return launch_brick_variant<22, 32, 32, 1, 512, 8, B200DRR_BWD_U, 2, 0, 1, 1>(map, dims, raytab, ltab, geo, nullptr, counter,

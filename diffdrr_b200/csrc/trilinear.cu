@@ -1,4 +1,4 @@
-// trilinear.cu -- fixed-step trilinear ray-marching DRR kernels for sm_100a (forward + backward).
+// trilinear.cu -- fixed-step trilinear ray-marching DRR kernels for sm_90a (forward + backward).
 // One thread marches one ray (ray_math.cuh); blockIdx.y is the pose, blockIdx.x tiles the rays of that pose.
 #include "kernels.h"
 #include "ray_math.cuh"
@@ -323,7 +323,7 @@ __global__ void __launch_bounds__(256) pack_corners_kernel(const float* __restri
 
 cudaError_t launch_pack_corners(const float* vol, VolDims dims, float* packed, cudaStream_t stream)
 {
-    pack_corners_kernel<<<148 * 16, 256, 0, stream>>>(vol, dims, (float4*)packed);
+    pack_corners_kernel<<<current_sm_count() * 16, 256, 0, stream>>>(vol, dims, (float4*)packed);
     return cudaGetLastError();
 }
 

@@ -1,4 +1,4 @@
-"""`DRR`: the reference's nn.Module surface (reference diffdrr/drr.py:23-312) hosted on the sm_100a renderers.
+"""`DRR`: the reference's nn.Module surface (reference diffdrr/drr.py:23-312) hosted on the sm_90a renderers.
 
 Same constructor arguments, buffers (`_affine`, `_affine_inverse`, `density`, `mask`), properties and methods
 (`forward`, `render`, `set_intrinsics_`, `rescale_detector_`, `perspective_projection`, `inverse_projection`),
@@ -28,7 +28,7 @@ _TRILINEAR_POSE_IN = os.environ.get("B200DRR_TRILINEAR_POSE_IN", "1") != "0"
 
 
 class DRR(nn.Module):
-    """PyTorch module that computes differentiable digitally reconstructed radiographs on a B200."""
+    """PyTorch module that computes differentiable digitally reconstructed radiographs on an H100."""
 
     def __init__(
         self,
@@ -81,7 +81,7 @@ class DRR(nn.Module):
             import warnings
 
             self.renderer.forward = torch.compiler.disable(self.renderer.forward)
-            warnings.warn("diffdrr_b200: compile_renderer=True has nothing to compile -- the renderer is already a fused sm_100a "
+            warnings.warn("diffdrr_b200: compile_renderer=True has nothing to compile -- the renderer is already a fused sm_90a "
                           "kernel; it is kept as an opaque call (torch.compiler.disable) so an outer torch.compile can wrap it",
                           stacklevel=2)
         self.reshape = reshape

@@ -19,9 +19,8 @@ import torch.distributed as dist
 class PeerGather:
     """All-gather of equally sized per-rank shards that uses NO SM: every rank owns a symmetric-memory buffer (CUDA VMM
     mapped into all peers of the node), a rank PUSHES its shard into every peer's buffer with plain device copies
-    (copy engines over NVLink 5 / NVSwitch) on a side stream, and a symmetric-memory barrier (signal pads) closes the
-    exchange.  The NCCL all-gather it replaces runs as a kernel that shares the SMs with the next step's walk: measured
-    on 8 B200s the walk next to it slows by 10.7 % (1.247 -> 1.381 ms), which was most of the lost scaling efficiency.
+    (copy engines over NVLink / NVSwitch) on a side stream, and a symmetric-memory barrier (signal pads) closes the
+    exchange.  The NCCL all-gather it replaces runs as a kernel that shares the SMs with the next step's walk and slows it.
 
     `slots` independent buffers allow the gather of step k to overlap the walk of step k+1 (double buffering).
     Raises if symmetric memory is unavailable (single node with P2P access is required); callers may then fall back to

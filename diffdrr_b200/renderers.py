@@ -1,4 +1,4 @@
-"""`Siddon` and `Trilinear` renderer modules backed by hand-written sm_100a CUDA kernels.
+"""`Siddon` and `Trilinear` renderer modules backed by hand-written sm_90a CUDA kernels.
 
 Drop-in for the reference's renderer slot (`DRR.renderer`, reference drr.py:94-101,210): same constructor and
 `forward` signatures as reference renderers.py:14-42 (Siddon) and 189-216 (Trilinear), same `(B, 1, N)` result.
@@ -23,11 +23,10 @@ from . import _lib
 
 _REDUCE = {"sum": 0, "max": 1}
 # Slab-major scheduling of the packed trilinear FORWARD (include/b200drr.h): 16 base-voxel planes per slab once the batch
-# has >= 8 poses to share the slab through L2 (measured on B200, 512^3 -> 512^2, n_points = 500: 60.7 % -> 77.5 % of the HBM
-# roofline at 64 poses, 59.8 % -> 74.6 % at 16; no gain at 4).  The backward stays one-CTA-per-ray-tile: its per-slab
-# reductions cost more than the L2 sharing returns (measured).
+# has >= 8 poses to share the slab through L2.  The backward stays one-CTA-per-ray-tile: its per-slab reductions cost more
+# than the L2 sharing returns.  (These thresholds have not been re-measured on the H100.)
 _PACKED_SLAB_FWD = 16
-_PACKED_SLAB_SENS = 0   # forward+sensitivities march: unslabbed is faster (measured 8.8 vs 9.5-11 ms at 16 poses)
+_PACKED_SLAB_SENS = 0   # forward+sensitivities march: unslabbed (its registers and per-slab set-up outweigh the L2 sharing)
 _PACKED_SLAB_MIN_BATCH = 8
 
 
@@ -58,12 +57,11 @@ def _stream():
 
 
 # Brick-major forward (include/b200drr.h: b200drr_siddon_fwd_brick; csrc/siddon_brick.cu): TMA-staged voxel bricks in
-# shared memory, every staged voxel serves all poses of the batch.  Measured on B200 at 512^3 -> 256^2, 16 poses: 1.04 ms
-# (41.3 % of the HBM roofline on algorithmic bytes) vs 1.13 ms (37.9 %) for the slab-major kernel; the per-(ray, brick)
-# set-up only pays off once a few poses share each staged brick, hence the batch threshold (B200DRR_BRICK_MIN_BATCH).
+# shared memory, every staged voxel serves all poses of the batch.  The per-(ray, brick) set-up only pays off once a few
+# poses share each staged brick, hence the batch threshold (B200DRR_BRICK_MIN_BATCH).
 import os as _os
 
-_BRICK_MIN_BATCH = int(_os.environ.get("B200DRR_BRICK_MIN_BATCH", "2"))  # measured cross-over at 512^3 -> 256^2: B = 2
+_BRICK_MIN_BATCH = int(_os.environ.get("B200DRR_BRICK_MIN_BATCH", "2"))
 _brick_ws: dict = {}
 
 
@@ -72,21 +70,22 @@ _BRICK_MAX_RAY_DENSITY = float(_os.environ.get("B200DRR_BRICK_MAX_RAY_DENSITY", 
 
 
 def _brick_ok(vol, B, H, W, check_density: bool = True) -> bool:
-    # 24 x 32 x 32-voxel bricks over 2 x 148 resident CTAs: below ~7 bricks per CTA the tail of the dynamic brick queue
-    # costs more than the staging returns (256^3 = 704 bricks: 0.66 ms vs 0.48 ms slab-major; 512^3 = 5632 bricks: 1.04 vs 1.13)
+    # 24 x 32 x 32-voxel bricks over 2 x 132 resident CTAs: below ~7 bricks per CTA the tail of the dynamic brick queue
+    # costs more than the staging returns (256^3 = 704 bricks, 512^3 = 5632 bricks)
     n_bricks = -(-vol.shape[0] // 24) * -(-vol.shape[1] // 32) * -(-vol.shape[2] // 32)
     # ... and only for SPARSE ray sets (detector pixels fewer than ~half the voxels of a volume cross-section, i.e. rays
-    # >= ~1.4 voxels apart): dense rays share 32-byte sectors in L1 and the slab-major gather wins (measured at 512^3 ->
-    # 1024^2, 32 poses: 24.5 ms slab-major vs 36.5 ms brick-major; at 512^3 -> 256^2 the other way round)
+    # >= ~1.4 voxels apart): dense rays share 32-byte sectors in L1 and the slab-major gather wins (at 512^3 -> 1024^2;
+    # at 512^3 -> 256^2 the other way round)
     sparse = (not check_density) or H * W <= _BRICK_MAX_RAY_DENSITY * float(vol.numel()) ** (2.0 / 3.0)
     return (B >= _BRICK_MIN_BATCH and n_bricks >= _BRICK_MIN_BRICKS and sparse and vol.shape[2] % 4 == 0 and 2 <= H <= 2048
             and 2 <= W <= 2048 and B * H * W < 2**31 and vol.data_ptr() % 16 == 0 and vol.numel() < 2**31 - 1)
 
 
-# Full detector grids: up to a load of 16 (B * H * W in units of 256^2 rays) the library's own forward kernel cuts every ray into
-# pieces along its major axis (csrc/siddon.cu small_batch_pieces) and beats the brick kernel (512^3 -> 256^2, us per launch:
-# B = 2: 152 vs 229, 8: 504 vs 591, 16: 1032 vs 1099); the brick kernel keeps the bigger batches (62 us per pose at B = 32 / 64).
-_BRICK_FULL_GRID_MIN_LOAD = float(_os.environ.get("B200DRR_BRICK_MIN_LOAD", "16"))
+# Full detector grids: at a load of 1 (B * H * W in units of 256^2 rays) the library's own forward kernel, which cuts every ray
+# into pieces along its major axis (csrc/siddon.cu small_batch_pieces), beats the brick kernel; from 2 poses on the brick kernel
+# is faster.  H100 (scripts/tune_thresholds.py, 512^3 -> 256^2, us per launch, pieces / brick): 1 pose 124 / 240, 2: 384 / 284,
+# 4: 538 / 390, 16: 2479 / 1263.
+_BRICK_FULL_GRID_MIN_LOAD = float(_os.environ.get("B200DRR_BRICK_MIN_LOAD", "1"))
 
 
 def _brick_full_grid_ok(vol, B, H, W) -> bool:
@@ -858,7 +857,7 @@ def _reduce_code(reducefn):
 
 
 class Siddon(torch.nn.Module):
-    """Differentiable X-ray renderer, Siddon's exact ray tracing -- fused sm_100a kernel (reference renderers.py:11-91)."""
+    """Differentiable X-ray renderer, Siddon's exact ray tracing -- fused sm_90a kernel (reference renderers.py:11-91)."""
 
     def __init__(self, voxel_shift: float = 0.5, mode: str = "nearest", stop_gradients_through_grid_sample: bool = False,
                  filter_intersections_outside_volume: bool = False, reducefn: str = "sum", eps: float = 1e-8):
@@ -933,7 +932,7 @@ def _get_alpha_minmax(source, target, dims, voxel_shift, eps):
 
 
 class Trilinear(torch.nn.Module):
-    """Differentiable X-ray renderer, trilinear ray marching -- fused sm_100a kernel (reference renderers.py:186-254)."""
+    """Differentiable X-ray renderer, trilinear ray marching -- fused sm_90a kernel (reference renderers.py:186-254)."""
 
     def __init__(self, voxel_shift: float = 0.5, mode: str = "bilinear", reducefn: str = "sum", eps: float = 1e-8):
         super().__init__()

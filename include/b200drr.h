@@ -1,5 +1,5 @@
 /*
- * b200drr.h -- C ABI of the B200-native DRR projector (libb200drr.so).
+ * b200drr.h -- C ABI of the H100-native (sm_90a) DRR projector (libb200drr.so).
  *
  * This is the drop-in boundary for DiffDRR's renderer slot.  The reference is pure Python/PyTorch, so
  * the "FFI" a maintainer binds is a ctypes stub (INTEGRATION.md); every entry point below names the
@@ -55,8 +55,9 @@ int b200drr_siddon_fwd(const float *vol, int D0, int D1, int D2, const float *sr
  * pixels (n = h*W + w; reference detector.py:126), which lets the kernel map compact pixel tiles onto
  * warps/CTAs for cache locality.  Same result as b200drr_siddon_fwd(reduce=0, align_corners=0).
  * variant: 0 = tuned default -- up to 16 poses of 256^2 rays (volumes >= 384 voxels; smaller ones up to 4) every ray is cut into
- * pieces along its own major axis with a thread per (ray, piece), beyond that the volume is cut into 32-plane slabs that the poses
- * of the batch share through L2 (DESIGN.md 4.1 / 4.1c); other values select kernels for benchmarking: 15 = the slab-major kernel,
+ * pieces along its own major axis with a thread per (ray, piece), beyond that the volume is cut into 16-plane slabs that the poses
+ * of the batch share through L2 (DESIGN.md 4.1 / 4.1c); other values select kernels for benchmarking: 46 / 47 / 15 = the
+ * slab-major kernel with 16- / 24- / 32-plane slabs,
  * 100+K / 200+K / 300+K / 400+K (K = 1..64) = K major-axis pieces with 16x16/U4, 8x16/U8, 16x8/U4, 8x16/U4 tiles, further ids =
  * tile-shape / unroll variants (cudaErrorInvalidValue if unknown).
  */
@@ -123,7 +124,7 @@ int b200drr_siddon_bwd_pose(const float *vol, int D0, int D1, int D2, const floa
  * and autograd's backward (what torch derives for renderers.py:40-86 given g = dLoss/dout) is the elementwise
  * b200drr_siddon_bwd_sens below.  Replaces a forward walk + a backward walk by one.  No volume gradient on this path
  * (use b200drr_siddon_bwd_grid when the volume requires grad).  variant 0 = tuned default (major-axis pieces up to 6 poses of
- * 256^2 rays, 48-plane slabs beyond); 38 = the 48-plane-slab kernel; 100+K / 300+K / 400+K = K major-axis pieces (8x16/U8, 16x8/U8,
+ * 256^2 rays, 16-plane slabs beyond); 41 / 40 / 39 / 38 = the 16- / 24- / 32- / 48-plane-slab kernels; 100+K / 300+K / 400+K = K major-axis pieces (8x16/U8, 16x8/U8,
  * 8x16/U4 tiles); further ids = tile / unroll / slab-height variants for benchmarking.
  */
 int b200drr_siddon_fwd_sens(const float *vol, int D0, int D1, int D2, const float *src, const float *tgt,

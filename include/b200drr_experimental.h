@@ -1,8 +1,8 @@
 /*
  * b200drr_experimental.h -- entry points of REJECTED kernel experiments (prefix b200drr_x_).  They are NOT part of
  * libb200drr.so: build the experimental library with `B200DRR_BUILD_EXPERIMENTS=1 python -m diffdrr_b200.build`
- * (-DB200DRR_EXPERIMENTS) to time them again with scripts/tune_siddon.py.  Measured on B200 and rejected
- * (profiles/r01_tune_chunk_reuse.log, r01_tune_plane_sync.log); kept as documented negative results.
+ * (-DB200DRR_EXPERIMENTS) to time them again with scripts/tune_siddon.py.  Measured slower than the
+ * production kernels on the predecessor GPU and rejected (not re-measured on the H100); kept as documented negative results.
  */
 #ifndef B200DRR_EXPERIMENTAL_H
 #define B200DRR_EXPERIMENTAL_H
@@ -15,7 +15,7 @@ extern "C" {
 
 /*
  * EXPERIMENTAL (prefix b200drr_x_: may change or disappear; used by scripts/tune_siddon.py only, never by the module).
- * Measured on B200 and REJECTED (profiles/r01_tune_chunk_reuse.log: 12-50 % slower than the production kernels); kept, like
+ * REJECTED (slower than the production kernels; not re-measured on the H100); kept, like
  * the plane-synchronous walk, as a documented negative result.
  * Chunk-reuse Siddon forward: the lean walk over a copy of the volume whose FASTEST axis is the rays' major axis, so a
  * lane serves several consecutive visits from one LDG.64 / LDG.128 (DESIGN.md 8).  b200drr_x_transpose_volume writes that

@@ -2,7 +2,7 @@
 # Memory check of the walk logic WITHOUT a GPU: builds tests/hostemu (the product's per-ray device math compiled for the CPU) with
 # AddressSanitizer and walks random + exact-tie rays through exact-size heap volumes with the forward / sensitivities walks cut into
 # major-axis pieces, slabs and un-cut -- an out-of-bounds voxel read (a start voxel or tail step outside its box) aborts the run.
-# The device-side twin is scripts/sanitize_small.py under compute-sanitizer (profiles/r02_compute_sanitizer.txt).
+# The device-side twin is scripts/sanitize_small.py under compute-sanitizer.
 set -e
 cd "$(dirname "$0")/.."
 g++ -O1 -g -fsanitize=address -fno-omit-frame-pointer -ffp-contract=off -fPIC -shared -std=c++17 -Wno-unknown-pragmas \

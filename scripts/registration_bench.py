@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""BASELINE config 5: 2D/3D registration loop, 512^3 CT, 256^2 target DRR, gradient steps on one B200.
+"""BASELINE config 5: 2D/3D registration loop, 512^3 CT, 256^2 target DRR, gradient steps on one H100.
 
 Mirrors the loop of notebooks/tutorials/registration.ipynb cell 10: Registration(drr, rot, xyz) -> NCC vs a fixed
 target -> backward -> optimizer step.  Prints it/s and the final pose error."""

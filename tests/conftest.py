@@ -12,7 +12,7 @@ GOLDEN = os.path.join(ROOT, "tests", "golden")
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with `-m gpu`)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100, sm_90a; select with `-m gpu`)")
 
 
 def pytest_collection_modifyitems(config, items):
@@ -25,7 +25,7 @@ def pytest_collection_modifyitems(config, items):
         has_cuda = False
     if has_cuda:
         return
-    skip = pytest.mark.skip(reason="needs a CUDA device (B200): run with -m gpu on the GPU box")
+    skip = pytest.mark.skip(reason="needs a CUDA device (H100, sm_90a)")
     for item in items:
         if "gpu" in item.keywords:
             item.add_marker(skip)

@@ -104,8 +104,10 @@ def test_brick_forward_pose_in_and_module_routing(monkeypatch):
     assert (err > IMG_TOL).sum() <= 5 and err.max() < 1e-3 and float(np.sqrt((err ** 2).mean())) < 1e-5
 
 
-@pytest.mark.parametrize("variant", [0, 38])  # 0: the default for 2 poses (rays cut into 12 major-axis pieces); 38: 48-plane slabs,
-def test_siddon_sensitivities_and_volume_gradient_vs_oracle(variant):   # the dominant kernel of the 16-pose training step
+# 0: the default for 2 poses (rays cut into 16 major-axis pieces); 41: 16-plane slabs, the default of the 16-pose training step;
+# 38: 48-plane slabs
+@pytest.mark.parametrize("variant", [0, 41, 38])
+def test_siddon_sensitivities_and_volume_gradient_vs_oracle(variant):
     """b200drr_siddon_fwd_sens_grid + _bwd_sens (the training step's dominant kernel) and b200drr_siddon_bwd_grid
     WITH g_vol (reconstruction) at 512^3 -> 256^2, rotated poses, against the fp64 closed form.  Smooth volume for the
     end-point gradients (SURVEY 8c: on noise the reference's own fp32 is 1e-2 off), noise for image / volume gradient."""

@@ -89,8 +89,14 @@ def test_full_size_properties(big):
     one = sid(vol, src[1:2], tgt[1:2, 1000:3000].contiguous(), raylen[1:2, :, 1000:3000].contiguous())
     # (not bitwise: the 4-pose call takes the locality-sorted SLAB-major kernels -- per-slab partial sums combined by
     # red.global.add in run-dependent order -- while a 2000-ray call of one pose may take another decomposition; kernels agree
-    # to fp32 round-off of the partial sums, DESIGN.md 4.1)
-    assert relerr(one[0, 0].cpu().numpy(), out[1, 0, 1000:3000].cpu().numpy()) < 1e-5
+    # to fp32 round-off of the partial sums, DESIGN.md 4.1).  Each fp32 decomposition sums ~670 visits per ray and lands
+    # ~1.5e-5 from the fp64 oracle at this size, so both are pinned to the oracle and to each other at 2e-5.
+    from oracle import oracle
+    ref = oracle.siddon_fwd(vol.cpu().numpy(), src[1:2].cpu().numpy(), tgt[1:2, 1000:3000].cpu().numpy(),
+                            raylen[1:2, :, 1000:3000].cpu().numpy(), dtype=np.float64)[0, 0]
+    assert relerr(one[0, 0].cpu().numpy(), ref) < 2e-5
+    assert relerr(out[1, 0, 1000:3000].cpu().numpy(), ref) < 2e-5
+    assert relerr(one[0, 0].cpu().numpy(), out[1, 0, 1000:3000].cpu().numpy()) < 2e-5
     # (4) the general (plane-by-plane, reference-literal) kernel: max over segments is in [0, sum] for a density >= 0
     mx = Siddon(reducefn="max")(vol, src[:1], tgt[:1, :4096].contiguous(), raylen[:1, :, :4096].contiguous())
     assert (mx >= 0).all() and (mx <= out[:1, :, :4096] + 1e-6).all()

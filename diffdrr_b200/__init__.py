@@ -9,5 +9,6 @@ from .detector import Detector  # noqa: F401
 from .drr import DRR  # noqa: F401
 from .pose import RigidTransform, convert  # noqa: F401
 from .renderers import Siddon, Trilinear  # noqa: F401
-from .metrics import NormalizedCrossCorrelation2d  # noqa: F401,E402
+from .metrics import (  # noqa: F401,E402
+    GradientNormalizedCrossCorrelation2d, MultiscaleNormalizedCrossCorrelation2d, NormalizedCrossCorrelation2d, Sobel)
 from .registration import Registration  # noqa: F401,E402

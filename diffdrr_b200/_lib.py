@@ -202,6 +202,19 @@ _SIGNATURES = {
     "b200drr_ncc_bwd": (ctypes.c_int, [
         _c_float_p, _c_float_p, _c_float_p, _c_float_p, _c_float_p, _c_float_p, ctypes.c_int, ctypes.c_int, ctypes.c_int64,
         ctypes.c_void_p]),
+    "b200drr_local_ncc_workspace_bytes": (ctypes.c_int64, [ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int]),
+    "b200drr_local_ncc_fwd": (ctypes.c_int, [
+        _c_float_p, _c_float_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_float,
+        ctypes.c_void_p, _c_float_p, _c_float_p, ctypes.c_void_p]),
+    "b200drr_local_ncc_bwd": (ctypes.c_int, [
+        _c_float_p, _c_float_p, _c_float_p, _c_float_p, _c_float_p, _c_float_p, ctypes.c_int, ctypes.c_int, ctypes.c_int,
+        ctypes.c_int, ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p]),
+    "b200drr_sobel_workspace_bytes": (ctypes.c_int64, [ctypes.c_int, ctypes.c_int, ctypes.c_int]),
+    "b200drr_sobel_fwd": (ctypes.c_int, [
+        _c_float_p, _c_float_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, _c_float_p, ctypes.c_int, ctypes.c_void_p]),
+    "b200drr_sobel_bwd": (ctypes.c_int, [
+        _c_float_p, _c_float_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, _c_float_p, ctypes.c_int, ctypes.c_void_p,
+        ctypes.c_void_p]),
 }
 
 # entry points of rejected experiments (include/b200drr_experimental.h): bound only when the experimental build is loaded

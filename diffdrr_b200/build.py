@@ -13,7 +13,7 @@ import subprocess
 _HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(_HERE, "csrc")
 LIB_PATH = os.path.join(_HERE, "libb200drr.so")
-SOURCES = ["siddon.cu", "siddon_brick.cu", "trilinear.cu", "literal.cu", "pose.cu", "ncc.cu", "capi.cu"]
+SOURCES = ["siddon.cu", "siddon_brick.cu", "trilinear.cu", "literal.cu", "pose.cu", "ncc.cu", "local_ncc.cu", "sobel.cu", "capi.cu"]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17", "-Xcompiler", "-fPIC", "-shared",
 ]

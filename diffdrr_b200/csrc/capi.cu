@@ -707,4 +707,55 @@ int b200drr_ncc_bwd(const float* x1, const float* x2, const float* stats, const 
     return ret(launch_ncc_bwd(x1, x2, stats, gscore, g_x1, g_x2, B, C, N, (cudaStream_t)stream));
 }
 
+static bool bad_local_ncc(int B, int C, int H, int W, int p)
+{
+    return B <= 0 || C <= 0 || H <= 0 || W <= 0 || p < 1 || p > H || p > W || (int64_t)B * C > 65535;
+}
+
+int64_t b200drr_local_ncc_workspace_bytes(int B, int C, int H, int W, int p)
+{
+    if (bad_local_ncc(B, C, H, W, p)) return 0;
+    return local_ncc_workspace_bytes(B, C, H, W, p);
+}
+
+int b200drr_local_ncc_fwd(const float* x1, const float* x2, int B, int C, int H, int W, int p, float eps, void* workspace,
+                          float* stats, float* score, void* stream)
+{
+    if (!x1 || !x2 || !workspace || !stats || !score || bad_local_ncc(B, C, H, W, p)) return B200DRR_EINVAL;
+    return ret(launch_local_ncc_fwd(x1, x2, B, C, H, W, p, eps, workspace, stats, score, (cudaStream_t)stream));
+}
+
+int b200drr_local_ncc_bwd(const float* x1, const float* x2, const float* stats, const float* gscore, float* g_x1, float* g_x2, int B,
+                          int C, int H, int W, int p, void* workspace, void* stream)
+{
+    if (!x1 || !x2 || !stats || !gscore || (!g_x1 && !g_x2) || !workspace || bad_local_ncc(B, C, H, W, p)) return B200DRR_EINVAL;
+    return ret(launch_local_ncc_bwd(x1, x2, stats, gscore, g_x1, g_x2, B, C, H, W, p, workspace, (cudaStream_t)stream));
+}
+
+// odd kernel size, blur radius below both image sides (reflect padding), shared-memory tiles that fit
+static bool bad_sobel(int B, int H, int W, int ksize)
+{
+    return B <= 0 || B > 65535 || H <= 0 || W <= 0 || ksize <= 0 || (ksize & 1) == 0 || ksize / 2 >= H || ksize / 2 >= W ||
+           !sobel_kernel_fits(ksize);
+}
+
+int64_t b200drr_sobel_workspace_bytes(int B, int H, int W)
+{
+    if (B <= 0 || H <= 0 || W <= 0) return 0;
+    return sobel_workspace_bytes(B, H, W);
+}
+
+int b200drr_sobel_fwd(const float* x, float* out, int B, int H, int W, const float* weights, int ksize, void* stream)
+{
+    if (!x || !out || !weights || bad_sobel(B, H, W, ksize)) return B200DRR_EINVAL;
+    return ret(launch_sobel_fwd(x, out, B, H, W, weights, ksize, (cudaStream_t)stream));
+}
+
+int b200drr_sobel_bwd(const float* gout, float* g_x, int B, int H, int W, const float* weights, int ksize, void* workspace,
+                      void* stream)
+{
+    if (!gout || !g_x || !weights || !workspace || bad_sobel(B, H, W, ksize)) return B200DRR_EINVAL;
+    return ret(launch_sobel_bwd(gout, g_x, B, H, W, weights, ksize, workspace, (cudaStream_t)stream));
+}
+
 }  // extern "C"

@@ -185,4 +185,18 @@ cudaError_t launch_ncc_fwd(const float* x1, const float* x2, int B, int C, int64
 cudaError_t launch_ncc_bwd(const float* x1, const float* x2, const float* stats, const float* gscore, float* g_x1, float* g_x2,
                            int B, int C, int64_t N, cudaStream_t stream);
 
+// patch-wise NCC (local_ncc.cu)
+int64_t local_ncc_workspace_bytes(int B, int C, int H, int W, int p);
+cudaError_t launch_local_ncc_fwd(const float* x1, const float* x2, int B, int C, int H, int W, int p, float eps, void* workspace,
+                                 float* stats, float* score, cudaStream_t stream);
+cudaError_t launch_local_ncc_bwd(const float* x1, const float* x2, const float* stats, const float* gscore, float* g_x1, float* g_x2,
+                                 int B, int C, int H, int W, int p, void* workspace, cudaStream_t stream);
+
+// blur + Sobel front end of the gradient NCC (sobel.cu)
+int64_t sobel_workspace_bytes(int B, int H, int W);
+bool sobel_kernel_fits(int k);
+cudaError_t launch_sobel_fwd(const float* x, float* out, int B, int H, int W, const float* weights, int k, cudaStream_t stream);
+cudaError_t launch_sobel_bwd(const float* gout, float* g_x, int B, int H, int W, const float* weights, int k, void* workspace,
+                             cudaStream_t stream);
+
 }  // namespace b200drr

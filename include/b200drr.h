@@ -461,6 +461,40 @@ int b200drr_ncc_fwd(const float *x1, const float *x2, int B, int C, int64_t N, f
 int b200drr_ncc_bwd(const float *x1, const float *x2, const float *stats, const float *gscore, float *g_x1, float *g_x2, int B,
                     int C, int64_t N, void *stream);
 
+/*
+ * Patch-wise (local) NCC (reference diffdrr/metrics.py:16-44, NormalizedCrossCorrelation2d(patch_size = p)).  x1, x2
+ * [B][C][H][W] (device, contiguous), 1 <= p <= min(H, W), B*C <= 65535.  Every stride-1 p x p window of every channel is
+ * normalised on its own (mean, population variance + eps); with H' = H-p+1, W' = W-p+1:
+ *   score[b] = mean over the C*H'*W' windows of  cov_w / sqrt((var1_w + eps)(var2_w + eps)).
+ * b200drr_local_ncc_fwd: box sums of the five moments (vertical p-row sums, then horizontal p-column sums; double), written as
+ *   stats [B*C][5][H'][W'] = {mean1, 1/std1, mean2, 1/std2, ncc of the window} for the backward pass, and score [B]; the
+ *   partial scores are summed in a fixed order (deterministic).
+ * b200drr_local_ncc_bwd: gscore [B] -> g_x1, g_x2 [B][C][H][W] (either may be NULL) by the closed form
+ *   d score[b] / d x2_q = gscore[b] / (C H' W' p^2) * sum over the windows w containing q of r2 ((x1_q - mu1) r1 - (x2_q - mu2) r2 L)
+ *   (symmetrically for x1), evaluated as adjoint box sums of per-window maps.
+ * workspace: b200drr_local_ncc_workspace_bytes(B, C, H, W, p) bytes, 8-byte aligned, for either call (0 for bad arguments).
+ */
+int64_t b200drr_local_ncc_workspace_bytes(int B, int C, int H, int W, int p);
+int b200drr_local_ncc_fwd(const float *x1, const float *x2, int B, int C, int H, int W, int p, float eps, void *workspace,
+                          float *stats, float *score, void *stream);
+int b200drr_local_ncc_bwd(const float *x1, const float *x2, const float *stats, const float *gscore, float *g_x1, float *g_x2, int B,
+                          int C, int H, int W, int p, void *workspace, void *stream);
+
+/*
+ * Gaussian blur + Sobel gradients of one-channel images (reference diffdrr/metrics.py:69-93, the Sobel front end of
+ * GradientNormalizedCrossCorrelation2d).  x [B][H][W] (device) -> out [B][2][H][W]:
+ *   blur   separable, 1-D weights [ksize] (device; torchvision's normalised Gaussian, ksize odd; ksize = 1 with weight 1 is no
+ *          blur) after reflect padding of ksize/2, which must be < H and < W;
+ *   Sobel  3x3 cross-correlation with zero padding, channel 0 Gx = [[1,0,-1],[2,0,-2],[1,0,-1]], channel 1 Gy = Gx transposed.
+ * b200drr_sobel_fwd: one launch.  b200drr_sobel_bwd: gout [B][2][H][W] -> g_x [B][H][W], the exact adjoint (gradient that
+ * lands on reflected positions folds back onto the mirrored pixels).  workspace: b200drr_sobel_workspace_bytes(B, H, W) bytes.
+ * B <= 65535; ksize is also bounded by the shared-memory tiles (ksize/2 up to about 800).
+ */
+int64_t b200drr_sobel_workspace_bytes(int B, int H, int W);
+int b200drr_sobel_fwd(const float *x, float *out, int B, int H, int W, const float *weights, int ksize, void *stream);
+int b200drr_sobel_bwd(const float *gout, float *g_x, int B, int H, int W, const float *weights, int ksize, void *workspace,
+                      void *stream);
+
 #ifdef __cplusplus
 }
 #endif

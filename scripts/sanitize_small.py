@@ -1,14 +1,16 @@
 #!/usr/bin/env python
 """Small invocations of the round-2 kernels for compute-sanitizer (memcheck / racecheck / synccheck): brick-major TMA forward
 (several bricks per CTA, partial bricks, two pose chunks), the locality-ordered slab kernels, the brick scatter (volume gradient),
-the mask grid kernels, the un-reduced segment kernels, fp64 and the trilinear pose-in step; PeerGather is multi-GPU only."""
+the mask grid kernels, the un-reduced segment kernels, fp64, the trilinear pose-in step and the image losses (global and
+patch-wise NCC, blur + Sobel, on sizes that are not a multiple of the tiles); PeerGather is multi-GPU only."""
 import os
 import sys
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch  # noqa: E402
 
-from diffdrr_b200 import DRR, Siddon, _lib, renderers, synthetic  # noqa: E402
+from diffdrr_b200 import (DRR, GradientNormalizedCrossCorrelation2d, MultiscaleNormalizedCrossCorrelation2d, Siddon,  # noqa: E402
+                          _lib, renderers, synthetic)
 from diffdrr_b200.pose import convert  # noqa: E402
 from diffdrr_b200.renderers import _ptr, _stream  # noqa: E402
 
@@ -73,4 +75,14 @@ img = drr(rot, xyz, parameterization="euler_angles", convention="ZXY", n_points=
 img.sum().backward()
 torch.cuda.synchronize()
 print("trilinear pose-in ok", float(img.sum()), float(rot.grad.abs().max()))
+# image losses: patch-wise NCC (p = 1, a single window row), blur + Sobel with halos past both image edges and a wide blur
+for shape, losses in (((2, 1, 37, 45), (MultiscaleNormalizedCrossCorrelation2d([None, 5, 1], [0.5, 0.3, 0.2]),
+                                        GradientNormalizedCrossCorrelation2d(patch_size=9), GradientNormalizedCrossCorrelation2d(sigma=2.5))),
+                      ((1, 1, 9, 70), (MultiscaleNormalizedCrossCorrelation2d([9], [1.0]), GradientNormalizedCrossCorrelation2d(sigma=0.0)))):
+    for loss in losses:
+        a = torch.rand(*shape, device=dev).requires_grad_(True)
+        b = torch.rand(*shape, device=dev).requires_grad_(True)
+        loss(a, b).sum().backward()
+        torch.cuda.synchronize()
+        print(shape, type(loss).__name__, "ok", float(a.grad.abs().max()), float(b.grad.abs().max()))
 print("done")

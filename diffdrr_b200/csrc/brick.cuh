@@ -614,4 +614,45 @@ B200_HD void brick_pair_bwd_lean(const St& st, float wgt, const float s[3], cons
     if (rest != 0.0f) st.add(w.off, rest * wgt);
 }
 
+// ---- per-ray sensitivities (training step) over a staged brick ------------------------------------------------------------
+// The pair runs the slab kernels' exact-frame sensitivities walk (siddon_ray_sens_box, CUT = true: every brick face inside the
+// volume is a cut on its own axis, so a tie of a crossing with a brick edge or corner goes to the same axis as in the un-cut
+// walk) on the ray rebuilt bit-identically to the slab kernel.  Only the voxel fetch differs: the walk's offsets are formed
+// with the brick's strides scaled to the loader's units (kScale), and `bias` moves them onto the staged copy.
+template <class Ld>
+struct BrickLoad {
+    Ld ld;
+    int bias;  // ld.base() - (org . strides) * kScale
+    template <int U>
+    B200_HD void batch(const float*, const int (&offs)[U], float (&v)[U]) const
+    {
+#pragma unroll
+        for (int j = 0; j < U; ++j) v[j] = ld(offs[j] + bias);
+    }
+    B200_HD float at(const float*, int off) const { return ld(off + bias); }
+};
+
+// A, C accumulated INTO (see siddon_ray_sens_box_m); returns sum v * dalpha over the brick's voxels [lo_v, hi_v).
+template <int U, class Ld>
+B200_HD float brick_pair_sens(const Ld& ld, const Ray& ray, const VolDims& dims, const int lo_v[3], const int hi_v[3],
+                              const int org[3], int st0, int st1, int st2, float shift, float A[3], float C[3])
+{
+    const int s0 = st0 * Ld::kScale, s1 = st1 * Ld::kScale, s2 = st2 * Ld::kScale;
+    const BrickLoad<Ld> load{ld, ld.base() - (org[0] * s0 + org[1] * s1 + org[2] * s2)};
+    return siddon_ray_sens_box<U, BrickLoad<Ld>, true>(nullptr, dims, lo_v, hi_v, s0, s1, s2, ray, shift, A, C, load);
+}
+
+// Sort key of the sensitivities mode: the walk branches three ways on the ray's major axis M, and a warp's 32 items mix poses,
+// so M goes into the key (bin = M * 10 + one of 10 length bins, longest first within each M): warps are M-uniform except at
+// the group boundaries.  M comes from the ray table's 1/d (largest |d| = smallest |1/d|, ties to the lower axis as in
+// siddon_ray_sens_box); a rounding near 45 degrees only costs a divergent warp, the walk itself decides on d.
+constexpr int kSensLenBins = 10;
+B200_HD int sens_bin(const float inv[3], float a_in, float a_out, float sumabs_d, float inv_width)
+{
+    const float i0 = fabsf(inv[0]), i1 = fabsf(inv[1]), i2 = fabsf(inv[2]);
+    const int M = (i0 <= i1 && i0 <= i2) ? 0 : (i1 <= i2 ? 1 : 2);
+    const int b = step_bin(a_in, a_out, sumabs_d, inv_width);
+    return M * kSensLenBins + (b < kSensLenBins - 1 ? b : kSensLenBins - 1);
+}
+
 }  // namespace b200drr

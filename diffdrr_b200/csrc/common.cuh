@@ -65,6 +65,16 @@ B200_HD void red_add(float* addr, float v)
 #endif
 }
 
+// four consecutive floats (16-byte aligned) in one red.global.add.v4.f32
+B200_HD void red_add4(float* addr, float a, float b, float c, float d)
+{
+#if defined(__CUDA_ARCH__)
+    asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(addr), "f"(a), "f"(b), "f"(c), "f"(d) : "memory");
+#else
+    addr[0] += a; addr[1] += b; addr[2] += c; addr[3] += d;
+#endif
+}
+
 #if defined(__CUDACC__)
 // SMs of the current device: the grid-stride launches size their grids from it
 inline int current_sm_count()

@@ -140,6 +140,12 @@ cudaError_t launch_siddon_bwd_vol_brick(const float* gout, VolDims dims, const f
                                         const float* G, const float* Wd, const float* rows, const float* cols, float* g_vol,
                                         void* workspace, size_t workspace_bytes, int B, int H, int W, float shift, float eps,
                                         cudaStream_t stream);
+// training step through the brick kernel's sensitivities mode (full detector grids; scratch from cudaMallocAsync on `stream`;
+// G == nullptr -> rays from tgt/raylen)
+cudaError_t launch_siddon_fwd_sens_brick(const float* vol, VolDims dims, const float* src, const float* tgt, const float* raylen,
+                                         const float* G, const float* Wd, const float* rows, const float* cols, float* out,
+                                         float* sens, int B, int H, int W, float shift, float eps, cudaStream_t stream);
+bool siddon_sens_brick_route(VolDims dims, int B, int H, int W, const float* vol, const float* sens);
 
 // experiments (b200drr_x_*): chunk-reuse forward over a major-axis-fastest copy
 cudaError_t launch_x_transpose_volume(const float* vol, VolDims dims, int axis, float* out, cudaStream_t stream);

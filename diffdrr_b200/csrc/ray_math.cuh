@@ -1001,12 +1001,12 @@ struct LoadChunk {
 
 // The sensitivities walk of one ray restricted to a box, for a ray whose major axis is M: same walk, tie order and
 // tail as siddon_ray_bwd_lean_box, two accumulated axes + the telescoping identities.  A, C accumulated INTO.
+// `loader` fetches the voxels (a loader with state, e.g. the brick kernel's shared-memory copy, is handed in).
 template <int U, int M, class Load = LoadPlain, bool CUT = false>
 B200_HD float siddon_ray_sens_box_m(const float* vol, const VolDims& dims, const int lo_v[3], const int hi_v[3], int st0,
-                                    int st1, int st2, const Ray& ray, float shift, float A[3], float C[3])
+                                    int st1, int st2, const Ray& ray, float shift, float A[3], float C[3], Load loader = Load())
 {
     using Ax = MinorAxes<M>;
-    Load loader;
     const Walk w = start_walk_frame<CUT>(ray, dims, lo_v, hi_v, shift);
     if (!w.hit) return 0.0f;
     LeanConst k;
@@ -1078,13 +1078,13 @@ B200_HD float siddon_ray_sens_box_m(const float* vol, const VolDims& dims, const
 // Dispatch on the ray's major axis (uniform per warp except for rays near a 45-degree direction).
 template <int U, class Load = LoadPlain, bool CUT = false>
 B200_HD float siddon_ray_sens_box(const float* vol, const VolDims& dims, const int lo_v[3], const int hi_v[3], int st0,
-                                  int st1, int st2, const Ray& ray, float shift, float A[3], float C[3])
+                                  int st1, int st2, const Ray& ray, float shift, float A[3], float C[3], Load loader = Load())
 {
     const float a0 = fabsf(ray.d[0]), a1 = fabsf(ray.d[1]), a2 = fabsf(ray.d[2]);
     if (a0 >= a1 && a0 >= a2)
-        return siddon_ray_sens_box_m<U, 0, Load, CUT>(vol, dims, lo_v, hi_v, st0, st1, st2, ray, shift, A, C);
-    if (a1 >= a2) return siddon_ray_sens_box_m<U, 1, Load, CUT>(vol, dims, lo_v, hi_v, st0, st1, st2, ray, shift, A, C);
-    return siddon_ray_sens_box_m<U, 2, Load, CUT>(vol, dims, lo_v, hi_v, st0, st1, st2, ray, shift, A, C);
+        return siddon_ray_sens_box_m<U, 0, Load, CUT>(vol, dims, lo_v, hi_v, st0, st1, st2, ray, shift, A, C, loader);
+    if (a1 >= a2) return siddon_ray_sens_box_m<U, 1, Load, CUT>(vol, dims, lo_v, hi_v, st0, st1, st2, ray, shift, A, C, loader);
+    return siddon_ray_sens_box_m<U, 2, Load, CUT>(vol, dims, lo_v, hi_v, st0, st1, st2, ray, shift, A, C, loader);
 }
 
 // Backward of one ray restricted to the sub-box [lo, hi) (closed form, see siddon_ray_bwd below for the algebra).

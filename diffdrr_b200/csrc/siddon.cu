@@ -578,11 +578,6 @@ cudaError_t launch_siddon_bwd_pose(const float* vol, VolDims dims, const float* 
 //   sens[r] = { dI/dt0, dI/dt1, dI/dt2, S = sum v*dalpha,  dI/ds0, dI/ds1, dI/ds2, 0 },   out[r] = L * S.
 // Same slab-major decomposition as siddon_bwd_slab_kernel; partial sums via red.global.add (zero-filled by the launcher).
 // ---------------------------------------------------------------------------------------------------
-__device__ __forceinline__ void red_add4(float* addr, float a, float b, float c, float d)
-{
-    asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(addr), "f"(a), "f"(b), "f"(c), "f"(d) : "memory");
-}
-
 // MAJ = true: `slab` is a piece COUNT and the volume is cut along each ray's own major axis (major_axis_piece; small batches).
 template <int TW, int TH, int U, int MINB, bool MAJ = false>
 __global__ void __launch_bounds__(TW* TH, MINB) siddon_sens_slab_kernel(const float* __restrict__ vol, VolDims dims,
@@ -770,6 +765,9 @@ cudaError_t launch_siddon_fwd_sens_grid(const float* vol, VolDims dims, const fl
     case id:                                                                                                             \
         return launch_sens_slab_variant<TW, TH, U, MINB>(vol, dims, src, tgt, raylen, out, sens, B, H, W, SLAB, shift, eps, \
                                                          stream);
+    if (variant == 42 || (variant == 0 && siddon_sens_brick_route(dims, B, H, W, vol, sens)))  // brick-major (siddon_brick.cu)
+        return launch_siddon_fwd_sens_brick(vol, dims, src, tgt, raylen, nullptr, nullptr, nullptr, nullptr, out, sens, B, H, W, shift,
+                                            eps, stream);
     if (variant > 100 && variant <= 164)  // tuning: 101..164 = that many major-axis pieces, whatever the batch size
         return launch_sens_slab_variant<8, 16, 8, 8, true>(vol, dims, src, tgt, raylen, out, sens, B, H, W, variant - 100, shift, eps,
                                                            stream);
@@ -838,6 +836,8 @@ cudaError_t launch_siddon_fwd_sens_pose(const float* vol, VolDims dims, const fl
                                         const float* rows, const float* cols, float* out, float* sens, int B, int H, int W,
                                         float shift, float eps, cudaStream_t stream)
 {
+    if (siddon_sens_brick_route(dims, B, H, W, vol, sens))
+        return launch_siddon_fwd_sens_brick(vol, dims, src, nullptr, nullptr, G, Wd, rows, cols, out, sens, B, H, W, shift, eps, stream);
     const int pieces = small_batch_pieces(dims, B, H, W, true);
     if (pieces > 0)
         return launch_sens_slab_variant<8, 16, 8, 8, true>(vol, dims, src, nullptr, nullptr, out, sens, B, H, W, pieces, shift, eps,

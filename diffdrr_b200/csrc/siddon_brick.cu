@@ -12,9 +12,13 @@
 //      loads served by ld.shared, one red.global.add of the partial line integral per (ray, brick).
 // The (B, N) ray table {1/d, sum|d|} (+ the ray lengths L) is written once per launch by brick_prep_kernel, which also zero-fills
 // the output and derives the per-pose detector geometry used in step 1.
+// Two more modes of the same kernel: BWD (volume gradient, the staged brick is an accumulator) and SENS (training step: each pair
+// runs the exact-frame sensitivities walk of the slab kernels and adds the ray's image and end-point derivatives).
 //
 // Replaces reference renderers.py:94-113 (alphas + sort) and 156-169 (grid_sample gather) for full detector grids.
 #include <cuda.h>  // CUtensorMap + enums only; the encoder is fetched through cudaGetDriverEntryPoint (no -lcuda)
+
+#include <mutex>
 
 #include "brick.cuh"
 #include "kernels.h"
@@ -147,6 +151,17 @@ __device__ __forceinline__ Ray make_ray_b(const PoseRaysB& pr, const float* __re
     return ray;
 }
 
+// Sensitivities mode (SENS = 1): what a pair needs to rebuild its ray exactly as siddon_sens_slab_kernel does (make_ray_b: the
+// ray table only serves the hit test) and where it adds its share: sens [B][Nr][8], as b200drr_siddon_fwd_sens_grid lays it out.
+struct SensArgs {
+    const float* src;
+    const float* tgt;
+    const float* raylen;
+    PoseRaysB pr;
+    float* sens;
+    float eps;
+};
+
 // ---- ray table + per-pose geometry + zero fill ----------------------------------------------------------------------
 __global__ void __launch_bounds__(256) brick_prep_kernel(const float* __restrict__ src, const float* __restrict__ tgt,
                                                          const float* __restrict__ raylen, PoseRaysB pr,
@@ -155,7 +170,8 @@ __global__ void __launch_bounds__(256) brick_prep_kernel(const float* __restrict
                                                          unsigned* __restrict__ counter, int H, int W, float eps,
                                                          int64_t Nr /* rays per pose */,
                                                          const float* __restrict__ corners /* [B][3][3] or nullptr */,
-                                                         const float* __restrict__ gout /* volume-gradient mode, else nullptr */)
+                                                         const float* __restrict__ gout /* volume-gradient mode, else nullptr */,
+                                                         float* __restrict__ sens = nullptr /* sensitivities mode: zero-filled */)
 {
     const int64_t n = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     const int b = blockIdx.y;
@@ -168,6 +184,10 @@ __global__ void __launch_bounds__(256) brick_prep_kernel(const float* __restrict
     raytab[r] = make_float4(ray.inv[0], ray.inv[1], ray.inv[2], fabsf(ray.d[0]) + fabsf(ray.d[1]) + fabsf(ray.d[2]));
     ltab[r] = gout ? L * __ldg(gout + r) : L;  // volume-gradient mode: the weight every chord length is scattered with
     if (out) out[r] = 0.0f;
+    if (sens) {
+        float4* s4 = reinterpret_cast<float4*>(sens) + 2 * r;
+        s4[0] = s4[1] = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+    }
     if (n == 0) {
         float t00[3], t0w[3], th0[3];
         if (corners) {  // targets of the full grid's pixels (0, 0), (0, W-1), (H-1, 0), handed in by the caller
@@ -228,16 +248,20 @@ struct BrickCfg {
 // BWD = 1: volume-gradient mode.  `tmap` then describes g_vol, the staged brick starts as zeros instead of a TMA load, every
 // pair's walk scatters (gout * L) * chord length into it (brick_pair_bwd_lean; ltab holds gout * L), and the finished brick is
 // written with ONE TMA store -- every voxel belongs to exactly one brick, so there is no global atomic and g_vol is overwritten.
-template <int BX, int BY, int BZ, int STAGES, int THREADS, int K, int U, int CTAS, int PIPE, int RAYS, int BWD = 0>
+// SENS = 1: training-step mode (full detector grids).  Every pair rebuilds its ray, runs the exact-frame sensitivities walk over
+// the staged brick (brick_pair_sens) and flushes like siddon_sens_slab_kernel: two red.global.add.v4 into sa.sens (dI/dt, S,
+// dI/ds) and L * S into out, nothing for an all-zero pair.  The work list is sorted by major axis first (sens_bin).
+template <int BX, int BY, int BZ, int STAGES, int THREADS, int K, int U, int CTAS, int PIPE, int RAYS, int BWD = 0, int SENS = 0>
 __global__ void __launch_bounds__(THREADS, CTAS)
     siddon_fwd_brick_kernel(const __grid_constant__ CUtensorMap tmap, VolDims dims, BrickGrid bg,
                             const float4* __restrict__ raytab, const float* __restrict__ ltab,
                             const PoseGeo* __restrict__ geo, float* __restrict__ out, unsigned* __restrict__ counter,
                             const int* __restrict__ pix_index /* [H*W] pixel -> ray index, -1 = no ray; nullptr = full grid */,
-                            int Nr /* rays per pose */, int B, int H, int W, float shift)
+                            int Nr /* rays per pose */, int B, int H, int W, float shift, SensArgs sa)
 {
     using Cfg = BrickCfg<BX, BY, BZ, STAGES, THREADS, K, U, CTAS, PIPE, RAYS>;
     static_assert(BWD == 0 || (STAGES == 1 && RAYS == 1), "volume-gradient mode: single stage, one pair per thread");
+    static_assert(SENS == 0 || (BWD == 0 && RAYS == 1), "sensitivities mode: forward walk, one pair per thread");
     constexpr int kRowCap = Cfg::kRowCap;
     extern __shared__ __align__(1024) unsigned char smem[];
     unsigned* s_items = reinterpret_cast<unsigned*>(smem + Cfg::oItems);
@@ -259,6 +283,7 @@ __global__ void __launch_bounds__(THREADS, CTAS)
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int n_bricks = bg.nb0 * bg.nb1 * bg.nb2;
     const float inv_bin_width = (float)kBrickBins / (float)(BX + BY + BZ + 8);
+    const float inv_sens_width = (float)kSensLenBins / (float)(BX + BY + BZ + 8);
 
     if (tid == 0) {
 #pragma unroll
@@ -599,7 +624,8 @@ __global__ void __launch_bounds__(THREADS, CTAS)
                                 const float clo3[3] = {clo.x, clo.y, clo.z}, chi3[3] = {chi.x, chi.y, chi.z};
                                 float a_in, a_out;
                                 if (brick_maybe_hit(inv, clo3, chi3, a_in, a_out)) {
-                                    const int bin = step_bin(a_in, a_out, q.w, inv_bin_width);
+                                    const int bin = SENS ? sens_bin(inv, a_in, a_out, q.w, inv_sens_width)
+                                                         : step_bin(a_in, a_out, q.w, inv_bin_width);
                                     items[j] = pack_item(bin, bl, n);
                                     atomicAdd(&s_hist[bin], 1);
                                 }
@@ -713,9 +739,11 @@ __global__ void __launch_bounds__(THREADS, CTAS)
                     itw = 0xffffffffu;
                     if (c < n_chunks && i < n_items) {
                         itw = s_items[i];
-                        const unsigned r = (unsigned)(p0 + item_pose(itw)) * (unsigned)Nr + (unsigned)item_ray(itw);
-                        q = __ldg(raytab + r);
-                        L = __ldg(ltab + r);
+                        if constexpr (SENS == 0) {  // the sensitivities walk rebuilds its ray instead
+                            const unsigned r = (unsigned)(p0 + item_pose(itw)) * (unsigned)Nr + (unsigned)item_ray(itw);
+                            q = __ldg(raytab + r);
+                            L = __ldg(ltab + r);
+                        }
                     }
                 };
                 int c = claim();
@@ -740,6 +768,28 @@ __global__ void __launch_bounds__(THREADS, CTAS)
                             if (L != 0.0f)  // L = gout * raylen here (brick_prep_kernel)
                                 brick_pair_bwd_lean<U>(StShared{ld.base_addr}, L, s3, inv3, clo3, chi3, lo_v, hi_v, org, BY * BZ, BZ, 1,
                                                        shift);
+                        } else if constexpr (SENS != 0) {
+                            const int b = p0 + bl, n = item_ray(itw);
+                            const int64_t r = (int64_t)b * Nr + n;
+                            const int py = n / W, px = n - py * W;
+                            float Lr;
+                            const Ray ray = make_ray_b(sa.pr, sa.src, sa.tgt, sa.raylen, b, r, px, py, sa.eps, Lr);
+                            float A[3] = {0.0f, 0.0f, 0.0f}, C[3] = {0.0f, 0.0f, 0.0f};
+                            const float S = brick_pair_sens<U>(ld, ray, dims, lo_v, hi_v, org, BY * BZ, BZ, 1, shift, A, C);
+                            float jt[3], js[3];
+                            bool any = S != 0.0f;
+#pragma unroll
+                            for (int a = 0; a < 3; ++a) {
+                                const float k = Lr * ray.inv[a];
+                                jt[a] = -k * A[a];
+                                js[a] = k * (A[a] - C[a]);
+                                any = any || jt[a] != 0.0f || js[a] != 0.0f;
+                            }
+                            if (any) {
+                                red_add4(sa.sens + r * 8, jt[0], jt[1], jt[2], S);
+                                red_add4(sa.sens + r * 8 + 4, js[0], js[1], js[2], 0.0f);
+                                red_add(out + r, Lr * S);
+                            }
                         } else {
                             const float part = brick_pair_fwd_lean<U, LdShared, true, PIPE != 0>(ld, s3, inv3, clo3, chi3, lo_v, hi_v, org, BY * BZ, BZ, 1, shift);
                             if (part != 0.0f)
@@ -811,13 +861,13 @@ bool make_volume_map(CUtensorMap* map, const float* vol, VolDims dims, int BX, i
 
 size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
 
-template <int BX, int BY, int BZ, int STAGES, int THREADS, int K, int U, int CTAS, int PIPE, int RAYS = 1, int BWD = 0>
+template <int BX, int BY, int BZ, int STAGES, int THREADS, int K, int U, int CTAS, int PIPE, int RAYS = 1, int BWD = 0, int SENS = 0>
 cudaError_t launch_brick_variant(const CUtensorMap& map, VolDims dims, const float4* raytab, const float* ltab,
                                  const PoseGeo* geo, float* out, unsigned* counter, const int* pix_index, int Nr, int B, int H,
-                                 int W, float shift, cudaStream_t stream)
+                                 int W, float shift, cudaStream_t stream, const SensArgs& sa = SensArgs{})
 {
     using Cfg = BrickCfg<BX, BY, BZ, STAGES, THREADS, K, U, CTAS, PIPE, RAYS>;
-    auto kern = siddon_fwd_brick_kernel<BX, BY, BZ, STAGES, THREADS, K, U, CTAS, PIPE, RAYS, BWD>;
+    auto kern = siddon_fwd_brick_kernel<BX, BY, BZ, STAGES, THREADS, K, U, CTAS, PIPE, RAYS, BWD, SENS>;
     static bool configured = false;
     if (!configured) {
         cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes);
@@ -834,7 +884,8 @@ cudaError_t launch_brick_variant(const CUtensorMap& map, VolDims dims, const flo
     static_assert(Cfg::kSmemBytes <= (233472 - 1024 * CTAS) / CTAS, "shared-memory carve-up exceeds the SM");
     const int ctas_per_sm = CTAS;
     const int grid = min(bg.nb0 * bg.nb1 * bg.nb2, sms * ctas_per_sm);
-    kern<<<grid, THREADS, Cfg::kSmemBytes, stream>>>(map, dims, bg, raytab, ltab, geo, out, counter, pix_index, Nr, B, H, W, shift);
+    kern<<<grid, THREADS, Cfg::kSmemBytes, stream>>>(map, dims, bg, raytab, ltab, geo, out, counter, pix_index, Nr, B, H, W, shift,
+                                                     sa);
     return cudaGetLastError();
 }
 
@@ -961,6 +1012,107 @@ cudaError_t launch_siddon_bwd_vol_brick(const float* gout, VolDims dims, const f
     if (!make_volume_map(&map, g_vol, dims, 24, 32, 32, B200DRR_BWD_SWIZZLE != 0)) return cudaErrorNotSupported;
     return launch_brick_variant<24, 32, 32, 1, 512, 4, B200DRR_BWD_U, 2, 0, 1, 1>(map, dims, raytab, ltab, geo, nullptr, counter,
                                                                                  nullptr, (int)Nr, B, H, W, shift, stream);
+}
+
+// ---- training step: image + per-ray sensitivities through the SENS mode ---------------------------------------------------------
+#ifndef B200DRR_SENS_U
+#define B200DRR_SENS_U 8  // walk steps per group: fits the 64 registers of 2 CTAs x 512 threads without spills (U = 4 spills 8 B)
+#endif
+// Batches of at least this many poses take the brick path.  H100 SXM, 700 W, 512^3 -> 256^2 (scripts/sens_brick_sweep.py --block 20,
+// median us per launch, brick / best of the others): 2 poses 384 / 391 (pieces), 4: 583 / 627, 8: 1098 / 1266, 16: 2115 / 2394,
+// 32: 4144 / 4487 (slab-major) -- from 4 poses on the brick kernel wins by 7-15 %; at 2 the margin is inside the noise.
+constexpr int kSensBrickMinBatch = 4;
+
+// The one routing rule of the training step (b200drr_siddon_fwd_sens_grid variant 0 and b200drr_siddon_fwd_sens_pose): the brick
+// kernel can take the shape (siddon_brick_supported, 16-byte aligned volume and sensitivities), the volume has enough bricks for
+// the dynamic queue of 2 x 132 resident CTAs to balance (>= 2048 bricks of 24 x 32 x 32), the rays are sparse (detector pixels at
+// most half the voxels of a volume cross-section, as the module's forward routing requires: dense rays share L1 sectors and the
+// slab-major gather wins) and the batch is big enough for the staged bricks to be shared.
+bool siddon_sens_brick_route(VolDims dims, int B, int H, int W, const float* vol, const float* sens)
+{
+    const int64_t n_bricks = (int64_t)((dims.d[0] + 23) / 24) * ((dims.d[1] + 31) / 32) * ((dims.d[2] + 31) / 32);
+    const double nvox = (double)dims.d[0] * dims.d[1] * dims.d[2];
+    const bool sparse = (double)H * W <= 0.5 * pow(nvox, 2.0 / 3.0);
+    return B >= kSensBrickMinBatch && n_bricks >= 2048 && sparse && (int64_t)B * H * W < ((int64_t)1 << 31) &&
+           ((uintptr_t)vol & 15u) == 0 && ((uintptr_t)sens & 15u) == 0 && siddon_brick_supported(dims, H, W);
+}
+
+// Scratch pool of the sensitivities mode, one per device.  Its release threshold is unlimited: memory freed into it stays
+// reserved for the next call, so a training loop that synchronises with the host every step does not hand the ~21 MB back to
+// the driver at each synchronisation and map it again on the next call (the default pool's threshold is 0; that cost 20-50 % of
+// the eager end-to-end step).  The pool keeps at most the largest scratch one call has needed.
+static cudaMemPool_t sens_scratch_pool(int dev)
+{
+    static cudaMemPool_t pools[64] = {};
+    static std::mutex mu;
+    if (dev < 0 || dev >= 64) return nullptr;
+    std::lock_guard<std::mutex> lock(mu);
+    if (pools[dev] == nullptr) {
+        cudaMemPoolProps props = {};
+        props.allocType = cudaMemAllocationTypePinned;
+        props.location.type = cudaMemLocationTypeDevice;
+        props.location.id = dev;
+        cudaMemPool_t pool = nullptr;
+        if (cudaMemPoolCreate(&pool, &props) != cudaSuccess) return nullptr;
+        cuuint64_t keep = ~(cuuint64_t)0;
+        if (cudaMemPoolSetAttribute(pool, cudaMemPoolAttrReleaseThreshold, &keep) != cudaSuccess) {
+            cudaMemPoolDestroy(pool);
+            return nullptr;
+        }
+        pools[dev] = pool;
+    }
+    return pools[dev];
+}
+
+// out [B][H*W] and sens [B][H*W][8] are overwritten (zero-filled by brick_prep_kernel, then summed into by the pairs).
+cudaError_t launch_siddon_fwd_sens_brick(const float* vol, VolDims dims, const float* src, const float* tgt, const float* raylen,
+                                         const float* G, const float* Wd, const float* rows, const float* cols, float* out,
+                                         float* sens, int B, int H, int W, float shift, float eps, cudaStream_t stream)
+{
+    const int64_t Nr = (int64_t)H * W;
+    if (!siddon_brick_supported(dims, H, W) || ((uintptr_t)vol & 15u) != 0 || ((uintptr_t)sens & 15u) != 0 ||
+        (int64_t)B * Nr >= ((int64_t)1 << 31))
+        return cudaErrorNotSupported;
+    CUtensorMap map;
+    if (!make_volume_map(&map, vol, dims, 24, 32, 32, B200DRR_FWD_SWIZZLE != 0)) return cudaErrorNotSupported;
+    // Scratch (claim counter, per-pose geometry, ray table: ~21 MB at 16 poses of 256^2) from the stream-ordered allocator: no
+    // workspace argument, nothing shared across streams, no device-wide sync.  Eager calls take it from sens_scratch_pool; inside
+    // CUDA-graph capture the allocation becomes a pair of allocation / free nodes whose memory the graph itself keeps.
+    const size_t bytes = siddon_brick_workspace_bytes(B, H, W);
+    cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
+    cudaError_t e = cudaStreamIsCapturing(stream, &cap);
+    if (e != cudaSuccess) return e;
+    void* ws = nullptr;
+    if (cap == cudaStreamCaptureStatusNone) {
+        int dev = 0;
+        e = cudaGetDevice(&dev);
+        if (e != cudaSuccess) return e;
+        cudaMemPool_t pool = sens_scratch_pool(dev);
+        if (pool == nullptr) return cudaErrorMemoryAllocation;
+        e = cudaMallocFromPoolAsync(&ws, bytes, pool, stream);
+    } else {
+        e = cudaMallocAsync(&ws, bytes, stream);
+    }
+    if (e != cudaSuccess) return e;
+    unsigned char* w8 = static_cast<unsigned char*>(ws);
+    unsigned* counter = reinterpret_cast<unsigned*>(w8);
+    PoseGeo* geo = reinterpret_cast<PoseGeo*>(w8 + 256);
+    float4* raytab = reinterpret_cast<float4*>(w8 + 256 + align_up(sizeof(PoseGeo) * (size_t)B, 256));
+    float* ltab = reinterpret_cast<float*>(raytab + (size_t)B * Nr);
+    const PoseRaysB pr{G, Wd, rows, cols};
+    if (((uintptr_t)ws & 15u) != 0) e = cudaErrorInvalidValue;
+    if (e == cudaSuccess) {
+        brick_prep_kernel<<<dim3((unsigned)((Nr + 255) / 256), (unsigned)B), 256, 0, stream>>>(
+            src, tgt, raylen, pr, raytab, ltab, geo, out, counter, H, W, eps, Nr, nullptr, nullptr, sens);
+        e = cudaGetLastError();
+    }
+    if (e == cudaSuccess) {
+        const SensArgs sa{src, tgt, raylen, pr, sens, eps};
+        e = launch_brick_variant<24, 32, 32, 1, 512, 4, B200DRR_SENS_U, 2, 0, 1, 0, 1>(map, dims, raytab, ltab, geo, out, counter,
+                                                                                      nullptr, (int)Nr, B, H, W, shift, stream, sa);
+    }
+    const cudaError_t ef = cudaFreeAsync(ws, stream);
+    return e != cudaSuccess ? e : ef;
 }
 
 }  // namespace b200drr

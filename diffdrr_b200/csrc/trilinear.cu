@@ -384,11 +384,6 @@ cudaError_t launch_trilinear_bwd_packed(const float* packed, VolDims dims, const
 //   out[r] = L * step * sum V     and     sens[r] = { dI/dtgt[3], step*sum V | dI/dsrc[3], dI/dalphamin | dI/dalphamax, 0, 0, 0 }
 // and the backward pass is the elementwise trilinear_sens_bwd_kernel.
 // ---------------------------------------------------------------------------------------------------
-__device__ __forceinline__ void red_add4(float* addr, float a, float b, float c, float d)
-{
-    asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(addr), "f"(a), "f"(b), "f"(c), "f"(d) : "memory");
-}
-
 template <int TW, int TH, bool SLAB>
 __global__ void __launch_bounds__(TW* TH) trilinear_sens_packed_kernel(
     const float4* __restrict__ packed, VolDims dims, const float* __restrict__ src, const float* __restrict__ tgt,

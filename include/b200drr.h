@@ -123,9 +123,15 @@ int b200drr_siddon_bwd_pose(const float *vol, int D0, int D1, int D2, const floa
  *   sens [B][H*W][8]  { dI/dtgt0, dI/dtgt1, dI/dtgt2, S = out/raylen, dI/dsrc0, dI/dsrc1, dI/dsrc2, 0 }
  * and autograd's backward (what torch derives for renderers.py:40-86 given g = dLoss/dout) is the elementwise
  * b200drr_siddon_bwd_sens below.  Replaces a forward walk + a backward walk by one.  No volume gradient on this path
- * (use b200drr_siddon_bwd_grid when the volume requires grad).  variant 0 = tuned default (major-axis pieces up to 6 poses of
- * 256^2 rays, 16-plane slabs beyond); 41 / 40 / 39 / 38 = the 16- / 24- / 32- / 48-plane-slab kernels; 100+K / 300+K / 400+K = K major-axis pieces (8x16/U8, 16x8/U8,
- * 8x16/U4 tiles); further ids = tile / unroll / slab-height variants for benchmarking.
+ * (use b200drr_siddon_bwd_grid when the volume requires grad).  variant 0 = tuned default: the brick-major kernel (id 42) when
+ * the shape allows it -- at least 4 poses, >= 2048 bricks of 24x32x32 voxels, sparse rays (H*W <= half the voxels of a volume
+ * cross-section), D2 % 4 == 0, H, W in [2, 2048], 16-byte aligned vol and sens -- else major-axis pieces up to 6 poses of
+ * 256^2 rays, 16-plane slabs beyond.  b200drr_siddon_fwd_sens_pose follows the same rule.  41 / 40 / 39 / 38 = the 16- / 24- /
+ * 32- / 48-plane-slab kernels (41 = the slab-major kernel by an explicit id); 42 = the brick-major kernel (TMA-staged 24x32x32
+ * bricks, the slab kernels' sensitivities walk per (ray, brick); ~20 B per ray of scratch from a stream-ordered memory pool of
+ * the library that keeps its memory between calls; cudaErrorNotSupported outside the brick kernel's range); 100+K / 300+K /
+ * 400+K = K major-axis pieces (8x16/U8, 16x8/U8, 8x16/U4 tiles); further ids = tile / unroll / slab-height variants for
+ * benchmarking.
  */
 int b200drr_siddon_fwd_sens(const float *vol, int D0, int D1, int D2, const float *src, const float *tgt,
                             const float *raylen, float *out, float *sens, int B, int64_t N, float voxel_shift, float eps,

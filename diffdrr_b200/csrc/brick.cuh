@@ -233,12 +233,15 @@ B200_HD int step_bin(float a_in, float a_out, float sumabs_d, float inv_width)
 }
 
 // Host emulation loader: the brick is a plain array, offsets are element offsets.
-struct LdHost {
-    const float* brick;
+// V = the staged voxel type (float, or a 16-bit VoxF16 / VoxBF16 widened by ldg).
+template <class V>
+struct LdHostT {
+    const V* brick;
     static constexpr int kScale = 1;
     B200_HD int base() const { return 0; }
-    B200_HD float operator()(int off) const { return brick[off]; }
+    B200_HD float operator()(int off) const { return ldg(brick + off); }
 };
+using LdHost = LdHostT<float>;
 
 // Line integral (sum of v * dalpha) of one ray over the voxels [lo_v, hi_v) of a brick whose voxel (org) sits at element
 // 0 of the staged copy with element strides (st0, st1, st2).  Same walk, same order, same rounding as
@@ -639,7 +642,7 @@ B200_HD float brick_pair_sens(const Ld& ld, const Ray& ray, const VolDims& dims,
 {
     const int s0 = st0 * Ld::kScale, s1 = st1 * Ld::kScale, s2 = st2 * Ld::kScale;
     const BrickLoad<Ld> load{ld, ld.base() - (org[0] * s0 + org[1] * s1 + org[2] * s2)};
-    return siddon_ray_sens_box<U, BrickLoad<Ld>, true>(nullptr, dims, lo_v, hi_v, s0, s1, s2, ray, shift, A, C, load);
+    return siddon_ray_sens_box<U, BrickLoad<Ld>, true>(static_cast<const float*>(nullptr), dims, lo_v, hi_v, s0, s1, s2, ray, shift, A, C, load);
 }
 
 // Sort key of the sensitivities mode: the walk branches three ways on the ray's major axis M, and a warp's 32 items mix poses,

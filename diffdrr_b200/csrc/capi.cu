@@ -48,6 +48,16 @@ int segments_bwd(int kind, const void* vol, int D0, int D1, int D2, const void* 
                                                (const R*)gseg, (R*)g_src, (R*)g_tgt, (R*)g_raylen, (R*)g_vol, (R*)g_alpha_range, B, N,
                                                (R)shift, (R)eps, n_points, (const R*)alpha_range, align_corners, (cudaStream_t)stream));
 }
+
+// Calls f with a value of the voxel type vol_type names (VoxF16 / VoxBF16); B200DRR_EINVAL for anything else.
+template <class F>
+int with_vox16(int vol_type, F&& f)
+{
+    if (vol_type == B200DRR_VOL_F16) return f(VoxF16{});
+    if (vol_type == B200DRR_VOL_BF16) return f(VoxBF16{});
+    return B200DRR_EINVAL;
+}
+inline bool too_big(int D0, int D1, int D2) { return (int64_t)D0 * D1 * D2 >= (int64_t)INT32_MAX; }
 }  // namespace
 
 extern "C" {
@@ -609,6 +619,256 @@ int b200drr_trilinear_bwd_mask(const float* vol, const float* mask, int D0, int 
     return ret(launch_trilinear_bwd_mask(vol, mask, mk(D0, D1, D2), src, tgt, raylen, gout, g_src, g_tgt, g_raylen, g_vol,
                                          g_alpha_range, B, N, C, voxel_shift, eps, n_points, alpha_range, align_corners != 0,
                                          (cudaStream_t)stream));
+}
+
+// ---- 16-bit volumes: twins of the Siddon forward entry points (include/b200drr.h, DESIGN.md 4.5) -------------------------------
+int b200drr_siddon_fwd_v16(const void* vol, int vol_type, int D0, int D1, int D2, const float* src, const float* tgt,
+                           const float* raylen, float* out, int B, int64_t N, float voxel_shift, float eps, int reduce,
+                           int align_corners, void* stream)
+{
+    if (!vol || !src || !tgt || !raylen || !out || bad_dims(D0, D1, D2) || bad_rays(B, N) || reduce != 0 || align_corners != 0)
+        return B200DRR_EINVAL;
+    return with_vox16(vol_type, [&](auto v) {
+        using V = decltype(v);
+        return ret(launch_siddon_fwd_fast((const V*)vol, mk(D0, D1, D2), src, tgt, raylen, out, B, N, voxel_shift, eps,
+                                          (cudaStream_t)stream));
+    });
+}
+
+int b200drr_siddon_fwd_sens_v16(const void* vol, int vol_type, int D0, int D1, int D2, const float* src, const float* tgt,
+                                const float* raylen, float* out, float* sens, int B, int64_t N, float voxel_shift, float eps,
+                                void* stream)
+{
+    if (!vol || !src || !tgt || !raylen || !out || !sens || bad_dims(D0, D1, D2) || bad_rays(B, N)) return B200DRR_EINVAL;
+    return with_vox16(vol_type, [&](auto v) {
+        using V = decltype(v);
+        if (too_big(D0, D1, D2)) return (int)B200DRR_EUNSUPPORTED;
+        return ret(launch_siddon_fwd_sens((const V*)vol, mk(D0, D1, D2), src, tgt, raylen, out, sens, B, N, voxel_shift, eps,
+                                          (cudaStream_t)stream));
+    });
+}
+
+int b200drr_siddon_fwd_sorted_v16(const void* vol, int vol_type, int D0, int D1, int D2, const float* src, const float* tgt,
+                                  const float* raylen, float* out, int B, int64_t N, float voxel_shift, float eps, void* stream)
+{
+    if (!vol || !src || !tgt || !raylen || !out || bad_dims(D0, D1, D2) || bad_rays(B, N)) return B200DRR_EINVAL;
+    return with_vox16(vol_type, [&](auto v) {
+        using V = decltype(v);
+        if (too_big(D0, D1, D2)) return (int)B200DRR_EUNSUPPORTED;
+        return ret(launch_siddon_fwd_sorted((const V*)vol, mk(D0, D1, D2), src, tgt, raylen, out, B, N, voxel_shift, eps,
+                                            (cudaStream_t)stream));
+    });
+}
+
+int b200drr_siddon_fwd_sens_sorted_v16(const void* vol, int vol_type, int D0, int D1, int D2, const float* src, const float* tgt,
+                                       const float* raylen, float* out, float* sens, int B, int64_t N, float voxel_shift, float eps,
+                                       void* stream)
+{
+    if (!vol || !src || !tgt || !raylen || !out || !sens || bad_dims(D0, D1, D2) || bad_rays(B, N)) return B200DRR_EINVAL;
+    return with_vox16(vol_type, [&](auto v) {
+        using V = decltype(v);
+        if (too_big(D0, D1, D2)) return (int)B200DRR_EUNSUPPORTED;
+        return ret(launch_siddon_fwd_sens_sorted((const V*)vol, mk(D0, D1, D2), src, tgt, raylen, out, sens, B, N, voxel_shift, eps,
+                                                 (cudaStream_t)stream));
+    });
+}
+
+int b200drr_siddon_fwd_grid_v16(const void* vol, int vol_type, int D0, int D1, int D2, const float* src, const float* tgt,
+                                const float* raylen, float* out, int B, int H, int W, float voxel_shift, float eps, int variant,
+                                void* stream)
+{
+    if (!vol || !src || !tgt || !raylen || !out || bad_dims(D0, D1, D2) || bad_rays(B, (int64_t)H * W) || H <= 0 || W <= 0)
+        return B200DRR_EINVAL;
+    return with_vox16(vol_type, [&](auto v) {
+        using V = decltype(v);
+        if (variant != 0) return (int)B200DRR_EUNSUPPORTED;  // the tuning variants are fp32-only
+        return ret(launch_siddon_fwd_grid_default((const V*)vol, mk(D0, D1, D2), src, tgt, raylen, out, B, H, W, voxel_shift, eps,
+                                                  (cudaStream_t)stream));
+    });
+}
+
+int b200drr_siddon_fwd_sens_grid_v16(const void* vol, int vol_type, int D0, int D1, int D2, const float* src, const float* tgt,
+                                     const float* raylen, float* out, float* sens, int B, int H, int W, float voxel_shift, float eps,
+                                     int variant, void* stream)
+{
+    if (!vol || !src || !tgt || !raylen || !out || !sens || bad_dims(D0, D1, D2) || bad_rays(B, (int64_t)H * W) || H <= 0 ||
+        W <= 0)
+        return B200DRR_EINVAL;
+    return with_vox16(vol_type, [&](auto v) {
+        using V = decltype(v);
+        if (variant != 0 || too_big(D0, D1, D2)) return (int)B200DRR_EUNSUPPORTED;
+        return ret(launch_siddon_fwd_sens_grid_default((const V*)vol, mk(D0, D1, D2), src, tgt, raylen, out, sens, B, H, W,
+                                                       voxel_shift, eps, (cudaStream_t)stream));
+    });
+}
+
+int b200drr_siddon_fwd_brick_v16(const void* vol, int vol_type, int D0, int D1, int D2, const float* src, const float* tgt,
+                                 const float* raylen, const float* G, const float* Wd, const float* rows, const float* cols,
+                                 float* out, void* workspace, int64_t workspace_bytes, int B, int H, int W, float voxel_shift,
+                                 float eps, int variant, void* stream)
+{
+    const bool pose_in = G != nullptr;
+    if (!vol || !src || !out || !workspace || bad_dims(D0, D1, D2) || bad_rays(B, (int64_t)H * W) || H <= 0 || W <= 0)
+        return B200DRR_EINVAL;
+    if (pose_in ? (!Wd || !rows || !cols) : (!tgt || !raylen)) return B200DRR_EINVAL;
+    return with_vox16(vol_type, [&](auto v) {
+        using V = decltype(v);
+        if (variant != 0) return (int)B200DRR_EUNSUPPORTED;  // the tuning variants are fp32-only
+        if (!siddon_brick_supported(mk(D0, D1, D2), H, W, 2) || ((uintptr_t)vol & 15u) != 0) return (int)B200DRR_EUNSUPPORTED;
+        if (workspace_bytes < (int64_t)siddon_brick_workspace_bytes(B, H, W) || ((uintptr_t)workspace & 255u) != 0)
+            return (int)B200DRR_EINVAL;
+        return ret(launch_siddon_fwd_brick((const V*)vol, mk(D0, D1, D2), src, tgt, raylen, G, Wd, rows, cols, out, workspace,
+                                           (size_t)workspace_bytes, B, H, W, voxel_shift, eps, variant, (cudaStream_t)stream));
+    });
+}
+
+int b200drr_siddon_fwd_brick_subset_v16(const void* vol, int vol_type, int D0, int D1, int D2, const float* src, const float* tgt,
+                                        const float* raylen, const int32_t* pix_index, const float* corners, float* out,
+                                        void* workspace, int64_t workspace_bytes, int B, int H, int W, int64_t Nsub,
+                                        float voxel_shift, float eps, int variant, void* stream)
+{
+    if (!vol || !src || !tgt || !raylen || !pix_index || !corners || !out || !workspace || bad_dims(D0, D1, D2) ||
+        bad_rays(B, Nsub) || H <= 0 || W <= 0 || Nsub > (int64_t)H * W)
+        return B200DRR_EINVAL;
+    return with_vox16(vol_type, [&](auto v) {
+        using V = decltype(v);
+        if (variant != 0) return (int)B200DRR_EUNSUPPORTED;  // the tuning variants are fp32-only
+        if (!siddon_brick_supported(mk(D0, D1, D2), H, W, 2) || ((uintptr_t)vol & 15u) != 0) return (int)B200DRR_EUNSUPPORTED;
+        if (workspace_bytes < (int64_t)siddon_brick_workspace_bytes(B, 1, (int)Nsub) || ((uintptr_t)workspace & 255u) != 0)
+            return (int)B200DRR_EINVAL;
+        return ret(launch_siddon_fwd_brick((const V*)vol, mk(D0, D1, D2), src, tgt, raylen, nullptr, nullptr, nullptr, nullptr, out,
+                                           workspace, (size_t)workspace_bytes, B, H, W, voxel_shift, eps, variant,
+                                           (cudaStream_t)stream, pix_index, corners, Nsub));
+    });
+}
+
+int b200drr_siddon_fwd_pose_v16(const void* vol, int vol_type, int D0, int D1, int D2, const float* src, const float* G,
+                                const float* Wd, const float* rows, const float* cols, float* out, int B, int H, int W,
+                                float voxel_shift, float eps, void* stream)
+{
+    if (!vol || !src || !G || !Wd || !rows || !cols || !out || bad_dims(D0, D1, D2) || bad_rays(B, (int64_t)H * W) || H <= 0 ||
+        W <= 0)
+        return B200DRR_EINVAL;
+    return with_vox16(vol_type, [&](auto v) {
+        using V = decltype(v);
+        if (too_big(D0, D1, D2)) return (int)B200DRR_EUNSUPPORTED;
+        return ret(launch_siddon_fwd_pose((const V*)vol, mk(D0, D1, D2), src, G, Wd, rows, cols, out, B, H, W, voxel_shift, eps,
+                                          (cudaStream_t)stream));
+    });
+}
+
+int b200drr_siddon_fwd_sens_pose_v16(const void* vol, int vol_type, int D0, int D1, int D2, const float* src, const float* G,
+                                     const float* Wd, const float* rows, const float* cols, float* out, float* sens, int B, int H,
+                                     int W, float voxel_shift, float eps, void* stream)
+{
+    if (!vol || !src || !G || !Wd || !rows || !cols || !out || !sens || bad_dims(D0, D1, D2) || bad_rays(B, (int64_t)H * W) ||
+        H <= 0 || W <= 0)
+        return B200DRR_EINVAL;
+    return with_vox16(vol_type, [&](auto v) {
+        using V = decltype(v);
+        if (too_big(D0, D1, D2)) return (int)B200DRR_EUNSUPPORTED;
+        return ret(launch_siddon_fwd_sens_pose((const V*)vol, mk(D0, D1, D2), src, G, Wd, rows, cols, out, sens, B, H, W,
+                                               voxel_shift, eps, (cudaStream_t)stream));
+    });
+}
+
+// ---- 16-bit volumes: twins of the Trilinear entry points --------------------------------------------------------------------------
+int b200drr_pack_corners_v16(const void* vol, int vol_type, int D0, int D1, int D2, void* packed, void* stream)
+{
+    if (!vol || !packed || bad_dims(D0, D1, D2)) return B200DRR_EINVAL;
+    return with_vox16(vol_type, [&](auto v) {
+        using V = decltype(v);
+        if (((uintptr_t)packed & 15u) != 0) return (int)B200DRR_EINVAL;
+        return ret(launch_pack_corners16((const V*)vol, mk(D0, D1, D2), (Cell16<V>*)packed, (cudaStream_t)stream));
+    });
+}
+
+int b200drr_trilinear_fwd_v16(const void* vol, int vol_type, int D0, int D1, int D2, const float* src, const float* tgt,
+                              const float* raylen, float* out, int B, int64_t N, float voxel_shift, float eps, int n_points,
+                              const float* alpha_range, int reduce, int align_corners, void* stream)
+{
+    if (!vol || !src || !tgt || !raylen || !out || !alpha_range || bad_dims(D0, D1, D2) || bad_rays(B, N) || n_points < 2 ||
+        reduce != 0 || align_corners != 0)
+        return B200DRR_EINVAL;
+    return with_vox16(vol_type, [&](auto v) {
+        using V = decltype(v);
+        return ret(launch_trilinear_fwd((const V*)vol, mk(D0, D1, D2), src, tgt, raylen, out, B, N, voxel_shift, eps, n_points,
+                                        alpha_range, 0, 0, (cudaStream_t)stream));
+    });
+}
+
+int b200drr_trilinear_fwd_grid_v16(const void* vol, int vol_type, int D0, int D1, int D2, const float* src, const float* tgt,
+                                   const float* raylen, float* out, int B, int H, int W, float voxel_shift, float eps, int n_points,
+                                   const float* alpha_range, int variant, void* stream)
+{
+    if (!vol || !src || !tgt || !raylen || !out || !alpha_range || bad_dims(D0, D1, D2) || bad_rays(B, (int64_t)H * W) ||
+        H <= 0 || W <= 0 || n_points < 2)
+        return B200DRR_EINVAL;
+    return with_vox16(vol_type, [&](auto v) {
+        using V = decltype(v);
+        return ret(launch_trilinear_fwd_grid((const V*)vol, mk(D0, D1, D2), src, tgt, raylen, out, B, H, W, voxel_shift, eps,
+                                             n_points, alpha_range, variant, (cudaStream_t)stream));
+    });
+}
+
+int b200drr_trilinear_fwd_sens_v16(const void* vol, int vol_type, int D0, int D1, int D2, const float* src, const float* tgt,
+                                   const float* raylen, float* out, float* sens, int B, int64_t N, int H, int W, float voxel_shift,
+                                   float eps, int n_points, const float* alpha_range, int align_corners, void* stream)
+{
+    if (!vol || !src || !tgt || !raylen || !out || !sens || !alpha_range || bad_dims(D0, D1, D2) || bad_rays(B, N) ||
+        n_points < 2 || H < 0 || W < 0 || (H > 0 && (int64_t)H * W != N) || align_corners != 0)
+        return B200DRR_EINVAL;
+    return with_vox16(vol_type, [&](auto v) {
+        using V = decltype(v);
+        return ret(launch_trilinear_fwd_sens((const V*)vol, mk(D0, D1, D2), src, tgt, raylen, out, sens, B, N, H, W, voxel_shift,
+                                             eps, n_points, alpha_range, 0, (cudaStream_t)stream));
+    });
+}
+
+int b200drr_trilinear_fwd_packed_v16(const void* packed, int vol_type, int D0, int D1, int D2, const float* src, const float* tgt,
+                                     const float* raylen, float* out, int B, int H, int W, float voxel_shift, float eps, int n_points,
+                                     const float* alpha_range, int slab, void* stream)
+{
+    if (!packed || slab < 0 || !src || !tgt || !raylen || !out || !alpha_range || bad_dims(D0, D1, D2) ||
+        bad_rays(B, (int64_t)H * W) || H <= 0 || W <= 0 || n_points < 2)
+        return B200DRR_EINVAL;
+    return with_vox16(vol_type, [&](auto v) {
+        using V = decltype(v);
+        return ret(launch_trilinear_fwd_packed_t((const Cell16<V>*)packed, mk(D0, D1, D2), src, tgt, raylen, out, B, H, W,
+                                                 voxel_shift, eps, n_points, alpha_range, slab, (cudaStream_t)stream));
+    });
+}
+
+int b200drr_trilinear_fwd_sens_packed_v16(const void* packed, int vol_type, int D0, int D1, int D2, const float* src,
+                                          const float* tgt, const float* raylen, float* out, float* sens, int B, int H, int W,
+                                          float voxel_shift, float eps, int n_points, const float* alpha_range, int slab,
+                                          void* stream)
+{
+    if (!packed || !src || !tgt || !raylen || !out || !sens || !alpha_range || bad_dims(D0, D1, D2) ||
+        bad_rays(B, (int64_t)H * W) || H <= 0 || W <= 0 || n_points < 2 || slab < 0)
+        return B200DRR_EINVAL;
+    return with_vox16(vol_type, [&](auto v) {
+        using V = decltype(v);
+        return ret(launch_trilinear_fwd_sens_packed16((const Cell16<V>*)packed, mk(D0, D1, D2), src, tgt, raylen, nullptr, nullptr,
+                                                      nullptr, nullptr, out, sens, B, H, W, voxel_shift, eps, n_points, alpha_range,
+                                                      slab, (cudaStream_t)stream));
+    });
+}
+
+int b200drr_trilinear_fwd_sens_pose_v16(const void* packed, int vol_type, int D0, int D1, int D2, const float* src, const float* G,
+                                        const float* Wd, const float* rows, const float* cols, float* out, float* sens, int B, int H,
+                                        int W, float voxel_shift, float eps, int n_points, const float* alpha_range, int slab,
+                                        void* stream)
+{
+    if (!packed || !src || !G || !Wd || !rows || !cols || !out || !sens || !alpha_range || bad_dims(D0, D1, D2) ||
+        bad_rays(B, (int64_t)H * W) || H <= 0 || W <= 0 || n_points < 2 || slab < 0)
+        return B200DRR_EINVAL;
+    return with_vox16(vol_type, [&](auto v) {
+        using V = decltype(v);
+        return ret(launch_trilinear_fwd_sens_packed16((const Cell16<V>*)packed, mk(D0, D1, D2), src, nullptr, nullptr, G, Wd, rows,
+                                                      cols, out, sens, B, H, W, voxel_shift, eps, n_points, alpha_range, slab,
+                                                      (cudaStream_t)stream));
+    });
 }
 
 #ifdef B200DRR_EXPERIMENTS

@@ -16,6 +16,9 @@
 struct float4 {  // host emulation only (tests/hostemu): the CUDA headers provide it for device builds
     float x, y, z, w;
 };
+struct uint4 {
+    unsigned x, y, z, w;
+};
 #endif
 
 namespace b200drr {
@@ -32,6 +35,72 @@ B200_HD float ldg(const float* p)
     return __ldg(p);  // (an L2::256B prefetch hint was tried: no effect)
 #else
     return *p;
+#endif
+}
+
+// 16-bit voxel storage (DESIGN.md 4.5): the volume may be stored as IEEE binary16 or bfloat16; every voxel read widens it to fp32
+// and all geometry and accumulation stay fp32.  The kernels take the voxel type V = float | VoxF16 | VoxBF16 as a template
+// parameter and read through ldg(vol + off), so the fp32 instantiations are the unchanged fp32 kernels.
+struct VoxF16 {
+    uint16_t bits;
+    static constexpr bool kBF16 = false;
+};
+struct VoxBF16 {
+    uint16_t bits;
+    static constexpr bool kBF16 = true;
+};
+
+B200_HD float f32_from_bits(uint32_t u)
+{
+#if defined(__CUDA_ARCH__)
+    return __uint_as_float(u);
+#else
+    float f;
+    __builtin_memcpy(&f, &u, 4);
+    return f;
+#endif
+}
+
+// The one 16-bit -> fp32 conversion (exact: both formats are subsets of fp32).  bf16 is the top half of an fp32; binary16 is
+// decoded by hand on the host (subnormals, infinities and NaN payloads as numpy's float16 -> float32) and by cvt on the device.
+B200_HD float vox16_to_f32(uint16_t h, bool bf16)
+{
+    if (bf16) return f32_from_bits((uint32_t)h << 16);
+#if defined(__CUDA_ARCH__)
+    float f;
+    asm("cvt.f32.f16 %0, %1;" : "=f"(f) : "h"(h));
+    return f;
+#else
+    const uint32_t sign = (uint32_t)(h & 0x8000u) << 16;
+    uint32_t e = (h >> 10) & 0x1fu, m = h & 0x3ffu;
+    if (e == 0x1fu) return f32_from_bits(sign | 0x7f800000u | (m << 13));  // inf / NaN
+    if (e == 0) {
+        if (m == 0) return f32_from_bits(sign);
+        e = 113;  // subnormal m * 2^-24: normalise the mantissa
+        while ((m & 0x400u) == 0) {
+            m <<= 1;
+            --e;
+        }
+        return f32_from_bits(sign | (e << 23) | ((m & 0x3ffu) << 13));
+    }
+    return f32_from_bits(sign | ((e + 112) << 23) | (m << 13));
+#endif
+}
+
+B200_HD float ldg(const VoxF16* p)
+{
+#if defined(__CUDA_ARCH__)
+    return vox16_to_f32(__ldg(reinterpret_cast<const unsigned short*>(p)), false);
+#else
+    return vox16_to_f32(p->bits, false);
+#endif
+}
+B200_HD float ldg(const VoxBF16* p)
+{
+#if defined(__CUDA_ARCH__)
+    return vox16_to_f32(__ldg(reinterpret_cast<const unsigned short*>(p)), true);
+#else
+    return vox16_to_f32(p->bits, true);
 #endif
 }
 

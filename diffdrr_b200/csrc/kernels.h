@@ -24,7 +24,8 @@ cudaError_t launch_siddon_bwd(const float* vol, VolDims dims, const float* src, 
                               const float* raylen, const float* gout, float* g_src, float* g_tgt, float* g_raylen,
                               float* g_vol, int B, int64_t N, float shift, float eps, int stop_grad,
                               cudaStream_t stream);
-cudaError_t launch_trilinear_fwd(const float* vol, VolDims dims, const float* src, const float* tgt,
+template <class V>  // V = float | VoxF16 | VoxBF16
+cudaError_t launch_trilinear_fwd(const V* vol, VolDims dims, const float* src, const float* tgt,
                                  const float* raylen, float* out, int B, int64_t N, float shift, float eps,
                                  int n_points, const float* alpha_range, int reduce, int align_corners,
                                  cudaStream_t stream);
@@ -34,7 +35,8 @@ cudaError_t launch_trilinear_bwd(const float* vol, VolDims dims, const float* sr
                                  int n_points, const float* alpha_range, int align_corners, cudaStream_t stream,
                                  int reduce = 0);
 
-cudaError_t launch_trilinear_fwd_grid(const float* vol, VolDims dims, const float* src, const float* tgt,
+template <class V>
+cudaError_t launch_trilinear_fwd_grid(const V* vol, VolDims dims, const float* src, const float* tgt,
                                       const float* raylen, float* out, int B, int H, int W, float shift, float eps,
                                       int n_points, const float* alpha_range, int variant, cudaStream_t stream);
 cudaError_t launch_trilinear_bwd_grid(const float* vol, VolDims dims, const float* src, const float* tgt,
@@ -42,7 +44,8 @@ cudaError_t launch_trilinear_bwd_grid(const float* vol, VolDims dims, const floa
                                       float* g_raylen, float* g_vol, float* g_alpha_range, int B, int H, int W, float shift,
                                       float eps, int n_points, const float* alpha_range, int variant, cudaStream_t stream);
 
-cudaError_t launch_siddon_fwd_pose(const float* vol, VolDims dims, const float* src, const float* G, const float* Wd,
+template <class V>  // V = float | VoxF16 | VoxBF16 (common.cuh) here and below where marked
+cudaError_t launch_siddon_fwd_pose(const V* vol, VolDims dims, const float* src, const float* G, const float* Wd,
                                    const float* rows, const float* cols, float* out, int B, int H, int W, float shift,
                                    float eps, cudaStream_t stream);
 cudaError_t launch_siddon_bwd_pose(const float* vol, VolDims dims, const float* src, const float* G, const float* Wd,
@@ -51,12 +54,14 @@ cudaError_t launch_siddon_bwd_pose(const float* vol, VolDims dims, const float* 
                                    float eps, int stop_grad, cudaStream_t stream);
 
 // forward with per-ray end-point sensitivities (sens: 8 floats per ray) and the backward that consumes them
-cudaError_t launch_siddon_fwd_sens(const float* vol, VolDims dims, const float* src, const float* tgt, const float* raylen,
+template <class V>
+cudaError_t launch_siddon_fwd_sens(const V* vol, VolDims dims, const float* src, const float* tgt, const float* raylen,
                                    float* out, float* sens, int B, int64_t N, float shift, float eps, cudaStream_t stream);
 cudaError_t launch_siddon_fwd_sens_grid(const float* vol, VolDims dims, const float* src, const float* tgt,
                                         const float* raylen, float* out, float* sens, int B, int H, int W, float shift,
                                         float eps, int variant, cudaStream_t stream);
-cudaError_t launch_siddon_fwd_sens_pose(const float* vol, VolDims dims, const float* src, const float* G, const float* Wd,
+template <class V>
+cudaError_t launch_siddon_fwd_sens_pose(const V* vol, VolDims dims, const float* src, const float* G, const float* Wd,
                                         const float* rows, const float* cols, float* out, float* sens, int B, int H, int W,
                                         float shift, float eps, cudaStream_t stream);
 cudaError_t launch_siddon_bwd_sens(const float* sens, const float* gout, float* g_src, float* g_tgt, float* g_raylen,
@@ -65,7 +70,8 @@ cudaError_t launch_siddon_bwd_sens_pose(const float* sens, const float* gout, co
                                         const float* cols, float* g_src, float* g_G, float* g_Wd, int B, int H, int W,
                                         int stop_grad, cudaStream_t stream);
 
-cudaError_t launch_trilinear_fwd_sens(const float* vol, VolDims dims, const float* src, const float* tgt, const float* raylen,
+template <class V>
+cudaError_t launch_trilinear_fwd_sens(const V* vol, VolDims dims, const float* src, const float* tgt, const float* raylen,
                                       float* out, float* sens, int B, int64_t N, int H, int W, float shift, float eps,
                                       int n_points, const float* alpha_range, int align_corners, cudaStream_t stream);
 cudaError_t launch_trilinear_fwd_sens_packed(const float* packed, VolDims dims, const float* src, const float* tgt,
@@ -122,15 +128,18 @@ cudaError_t launch_trilinear_bwd_literal(const R* vol, VolDims dims, const R* sr
                                          cudaStream_t stream);
 
 // arbitrary ray sets in a caller-provided locality order (slab-major, thread i = ray i)
-cudaError_t launch_siddon_fwd_sorted(const float* vol, VolDims dims, const float* src, const float* tgt, const float* raylen,
+template <class V>
+cudaError_t launch_siddon_fwd_sorted(const V* vol, VolDims dims, const float* src, const float* tgt, const float* raylen,
                                      float* out, int B, int64_t N, float shift, float eps, cudaStream_t stream);
-cudaError_t launch_siddon_fwd_sens_sorted(const float* vol, VolDims dims, const float* src, const float* tgt, const float* raylen,
+template <class V>
+cudaError_t launch_siddon_fwd_sens_sorted(const V* vol, VolDims dims, const float* src, const float* tgt, const float* raylen,
                                           float* out, float* sens, int B, int64_t N, float shift, float eps, cudaStream_t stream);
 
 // brick-major Siddon forward (siddon_brick.cu): TMA-staged voxel bricks in shared memory; G == nullptr -> rays from tgt/raylen
 size_t siddon_brick_workspace_bytes(int B, int H, int W);
-bool siddon_brick_supported(VolDims dims, int H, int W);
-cudaError_t launch_siddon_fwd_brick(const float* vol, VolDims dims, const float* src, const float* tgt, const float* raylen,
+bool siddon_brick_supported(VolDims dims, int H, int W, int elem_bytes = 4);  // 16-byte global strides for the TMA map
+template <class V>
+cudaError_t launch_siddon_fwd_brick(const V* vol, VolDims dims, const float* src, const float* tgt, const float* raylen,
                                     const float* G, const float* Wd, const float* rows, const float* cols, float* out,
                                     void* workspace, size_t workspace_bytes, int B, int H, int W, float shift, float eps,
                                     int variant, cudaStream_t stream, const int* pix_index = nullptr,
@@ -142,10 +151,23 @@ cudaError_t launch_siddon_bwd_vol_brick(const float* gout, VolDims dims, const f
                                         cudaStream_t stream);
 // training step through the brick kernel's sensitivities mode (full detector grids; scratch from cudaMallocAsync on `stream`;
 // G == nullptr -> rays from tgt/raylen)
-cudaError_t launch_siddon_fwd_sens_brick(const float* vol, VolDims dims, const float* src, const float* tgt, const float* raylen,
+template <class V>
+cudaError_t launch_siddon_fwd_sens_brick(const V* vol, VolDims dims, const float* src, const float* tgt, const float* raylen,
                                          const float* G, const float* Wd, const float* rows, const float* cols, float* out,
                                          float* sens, int B, int H, int W, float shift, float eps, cudaStream_t stream);
-bool siddon_sens_brick_route(VolDims dims, int B, int H, int W, const float* vol, const float* sens);
+bool siddon_sens_brick_route(VolDims dims, int B, int H, int W, const void* vol, const float* sens, int elem_bytes = 4);
+
+// the library's default routes, shared by the fp32 entry points (variant 0 / default options) and the 16-bit twins
+template <class V>
+cudaError_t launch_siddon_fwd_fast(const V* vol, VolDims dims, const float* src, const float* tgt, const float* raylen, float* out,
+                                   int B, int64_t N, float shift, float eps, cudaStream_t stream);
+template <class V>
+cudaError_t launch_siddon_fwd_grid_default(const V* vol, VolDims dims, const float* src, const float* tgt, const float* raylen,
+                                           float* out, int B, int H, int W, float shift, float eps, cudaStream_t stream);
+template <class V>
+cudaError_t launch_siddon_fwd_sens_grid_default(const V* vol, VolDims dims, const float* src, const float* tgt, const float* raylen,
+                                                float* out, float* sens, int B, int H, int W, float shift, float eps,
+                                                cudaStream_t stream);
 
 // experiments (b200drr_x_*): chunk-reuse forward over a major-axis-fastest copy
 cudaError_t launch_x_transpose_volume(const float* vol, VolDims dims, int axis, float* out, cudaStream_t stream);
@@ -176,6 +198,20 @@ cudaError_t launch_trilinear_fwd_mask(const float* vol, const float* mask, VolDi
                                       cudaStream_t stream, int W = 0);
 
 cudaError_t launch_pack_corners(const float* vol, VolDims dims, float* packed, cudaStream_t stream);
+// 16-bit volumes: packed cells of 8 corners in the volume's own type (ray_math.cuh: Cell16); G == nullptr -> rays from tgt/raylen
+template <class V>
+struct Cell16;
+template <class V>
+cudaError_t launch_pack_corners16(const V* vol, VolDims dims, Cell16<V>* packed, cudaStream_t stream);
+template <class PK>
+cudaError_t launch_trilinear_fwd_packed_t(const PK* packed, VolDims dims, const float* src, const float* tgt, const float* raylen,
+                                          float* out, int B, int H, int W, float shift, float eps, int n_points,
+                                          const float* alpha_range, int slab, cudaStream_t stream);
+template <class V>
+cudaError_t launch_trilinear_fwd_sens_packed16(const Cell16<V>* packed, VolDims dims, const float* src, const float* tgt,
+                                               const float* raylen, const float* G, const float* Wd, const float* rows,
+                                               const float* cols, float* out, float* sens, int B, int H, int W, float shift,
+                                               float eps, int n_points, const float* alpha_range, int slab, cudaStream_t stream);
 cudaError_t launch_trilinear_fwd_packed(const float* packed, VolDims dims, const float* src, const float* tgt,
                                         const float* raylen, float* out, int B, int H, int W, float shift, float eps,
                                         int n_points, const float* alpha_range, int slab, cudaStream_t stream);

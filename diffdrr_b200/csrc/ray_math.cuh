@@ -461,8 +461,8 @@ B200_HD int step_walk(Walk& w, const VolDims& dims, float anext, int64_t& off, c
 
 // Sum of v * (alpha_{j+1} - alpha_j) over the voxels the line crosses (multiply by raylen outside).
 // COUNT=true skips the loads and returns the number of voxels visited instead.
-template <bool COUNT>
-B200_HD float siddon_ray_fast(const float* vol, const VolDims& dims, const Ray& ray, float shift, int* visits)
+template <bool COUNT, class V = float>
+B200_HD float siddon_ray_fast(const V* vol, const VolDims& dims, const Ray& ray, float shift, int* visits)
 {
     Walk w = start_walk(ray, dims, shift);
     if (!w.hit) {
@@ -485,6 +485,12 @@ B200_HD float siddon_ray_fast(const float* vol, const VolDims& dims, const Ray& 
     }
     if (COUNT) *visits = count;
     return acc;
+}
+// the visit counter reads no voxels: siddon_ray_fast<true>(nullptr, ...)
+template <bool COUNT>
+B200_HD float siddon_ray_fast(decltype(nullptr), const VolDims& dims, const Ray& ray, float shift, int* visits)
+{
+    return siddon_ray_fast<COUNT, float>(static_cast<const float*>(nullptr), dims, ray, shift, visits);
 }
 
 // Same sum as siddon_ray_fast, software-pipelined: U walk steps are resolved (index + segment length) before their
@@ -616,8 +622,8 @@ B200_HD void lean_init(const Walk& w, int st0, int st1, int st2, LeanState& s, L
 }
 
 // Lean walk over the sub-box [lo, hi) of a volume whose element strides are (st0, st1, st2).
-template <int U>
-B200_HD float siddon_ray_lean_box(const float* vol, const int lo_v[3], const int hi_v[3], int st0, int st1, int st2,
+template <int U, class V = float>
+B200_HD float siddon_ray_lean_box(const V* vol, const int lo_v[3], const int hi_v[3], int st0, int st1, int st2,
                                   const Ray& ray, float shift)
 {
     const Walk w = start_walk_box(ray, lo_v, hi_v, shift);
@@ -964,13 +970,14 @@ B200_HD void minor_accumulate(int ax, float coef, float alpha, float& Au, float&
 // How the sensitivities walk fetches its voxels: one scalar load per visit from the volume as stored (production), or --
 // EXPERIMENT, see siddon_ray_lean_box_chunk -- W-voxel chunks from a major-axis-fastest copy, re-used across visits.
 struct LoadPlain {
-    template <int U>
-    B200_HD void batch(const float* vol, const int (&offs)[U], float (&v)[U])
+    template <int U, class V>
+    B200_HD void batch(const V* vol, const int (&offs)[U], float (&v)[U])
     {
 #pragma unroll
         for (int j = 0; j < U; ++j) v[j] = ldg(vol + offs[j]);
     }
-    B200_HD float at(const float* vol, int off) const { return ldg(vol + off); }
+    template <class V>
+    B200_HD float at(const V* vol, int off) const { return ldg(vol + off); }
 };
 
 template <int W>
@@ -1002,8 +1009,8 @@ struct LoadChunk {
 // The sensitivities walk of one ray restricted to a box, for a ray whose major axis is M: same walk, tie order and
 // tail as siddon_ray_bwd_lean_box, two accumulated axes + the telescoping identities.  A, C accumulated INTO.
 // `loader` fetches the voxels (a loader with state, e.g. the brick kernel's shared-memory copy, is handed in).
-template <int U, int M, class Load = LoadPlain, bool CUT = false>
-B200_HD float siddon_ray_sens_box_m(const float* vol, const VolDims& dims, const int lo_v[3], const int hi_v[3], int st0,
+template <int U, int M, class Load = LoadPlain, bool CUT = false, class V = float>
+B200_HD float siddon_ray_sens_box_m(const V* vol, const VolDims& dims, const int lo_v[3], const int hi_v[3], int st0,
                                     int st1, int st2, const Ray& ray, float shift, float A[3], float C[3], Load loader = Load())
 {
     using Ax = MinorAxes<M>;
@@ -1076,8 +1083,8 @@ B200_HD float siddon_ray_sens_box_m(const float* vol, const VolDims& dims, const
 }
 
 // Dispatch on the ray's major axis (uniform per warp except for rays near a 45-degree direction).
-template <int U, class Load = LoadPlain, bool CUT = false>
-B200_HD float siddon_ray_sens_box(const float* vol, const VolDims& dims, const int lo_v[3], const int hi_v[3], int st0,
+template <int U, class Load = LoadPlain, bool CUT = false, class V = float>
+B200_HD float siddon_ray_sens_box(const V* vol, const VolDims& dims, const int lo_v[3], const int hi_v[3], int st0,
                                   int st1, int st2, const Ray& ray, float shift, float A[3], float C[3], Load loader = Load())
 {
     const float a0 = fabsf(ray.d[0]), a1 = fabsf(ray.d[1]), a2 = fabsf(ray.d[2]);
@@ -1340,7 +1347,8 @@ B200_HD int64_t corner_off(const VolDims& dims, int c)
     return (int64_t)(c & 1) * dims.d[1] * dims.d[2] + (int64_t)((c >> 1) & 1) * dims.d[2] + ((c >> 2) & 1);
 }
 
-B200_HD Corner8 gather8(const float* vol, const VolDims& dims, const float pix[3])
+template <class V = float>
+B200_HD Corner8 gather8(const V* vol, const VolDims& dims, const float pix[3])
 {
     Corner8 k;
     int i0[3];
@@ -1373,10 +1381,12 @@ B200_HD Corner8 gather8(const float* vol, const VolDims& dims, const float pix[3
 
 // Gather policies for the trilinear marchers: 8 scalar loads from the plain volume, or one 32-byte read from the
 // packed-corner copy (see trilinear_ray_fwd_packed).
-struct GatherPlain {
-    const float* vol;
+template <class V>
+struct GatherPlainT {
+    const V* vol;
     B200_HD Corner8 operator()(const VolDims& dims, const float pix[3]) const { return gather8(vol, dims, pix); }
 };
+using GatherPlain = GatherPlainT<float>;
 
 struct GatherPacked {
     const float4* packed;
@@ -1405,6 +1415,45 @@ struct GatherPacked {
     }
 };
 
+// Packed-corner cell of a 16-bit volume (DESIGN.md 4.5): the same 8 corners in the volume's own 16-bit type V, 16 bytes per base
+// voxel (one LDG.128 per sample); word k holds corner 2k in its low half and corner 2k+1 in its high half.
+template <class V>
+struct alignas(16) Cell16 {
+    uint32_t w[4];
+};
+
+template <class V>
+struct GatherPacked16 {
+    const Cell16<V>* packed;
+    B200_HD Corner8 operator()(const VolDims& dims, const float pix[3]) const
+    {
+        Corner8 k;
+        int i0[3];
+#pragma unroll
+        for (int a = 0; a < 3; ++a) {
+            const float fl = floorf(pix[a]);
+            k.f[a] = pix[a] - fl;
+            i0[a] = (int)fl + 1;  // the packed array starts at base index -1
+        }
+        const int64_t p1 = dims.d[2] + 1, p0 = (int64_t)(dims.d[1] + 1) * p1;
+        const Cell16<V>* cell = packed + ((int64_t)i0[0] * p0 + (int64_t)i0[1] * p1 + i0[2]);
+#if defined(__CUDA_ARCH__)
+        const uint4 q = __ldg(reinterpret_cast<const uint4*>(cell));
+        const uint32_t w[4] = {q.x, q.y, q.z, q.w};
+#else
+        const uint32_t w[4] = {cell->w[0], cell->w[1], cell->w[2], cell->w[3]};
+#endif
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+            k.v[2 * j] = vox16_to_f32((uint16_t)(w[j] & 0xffffu), V::kBF16);
+            k.v[2 * j + 1] = vox16_to_f32((uint16_t)(w[j] >> 16), V::kBF16);
+        }
+        k.base = 0;
+        k.mask = 0u;
+        return k;
+    }
+};
+
 B200_HD bool outside_padded(const float pix[3], const VolDims& dims)
 {
     return pix[0] <= -1.0f || pix[1] <= -1.0f || pix[2] <= -1.0f || pix[0] >= (float)dims.d[0] ||
@@ -1425,7 +1474,8 @@ B200_HD float lerp8(const Corner8& k)
 }
 
 // sum (or max) over the samples of tri(V, x_m); multiply by raylen * step outside.
-B200_HD float trilinear_ray_fwd(const float* vol, const VolDims& dims, const Ray& ray, float shift, int P, float amin,
+template <class V = float>
+B200_HD float trilinear_ray_fwd(const V* vol, const VolDims& dims, const Ray& ray, float shift, int P, float amin,
                                 float amax, int reduce, int align_corners)
 {
     const PixLine pl = make_pixline(ray, dims, shift, align_corners);
@@ -1491,8 +1541,9 @@ B200_HD void trilinear_ray_fwd_mask(const float* vol, const float* mask, const V
 // ---- packed-corner volume: packed[(i0+1)][(i1+1)][(i2+1)][8] holds the 8 corner values of the interpolation cell
 // whose base voxel is (i0, i1, i2), i in [-1, D-1], zero padding included, corner c = o0 | o1<<1 | o2<<2.  One sample is
 // then ONE aligned 32-byte read (two LDG.128) instead of 8 scalar gathers -- exactly the 32 algorithmic bytes/sample.
-B200_HD float trilinear_ray_fwd_packed(const float4* packed, const VolDims& dims, const Ray& ray, float shift, int P,
-                                       float amin, float amax, float s_lo = -INFINITY, float s_hi = INFINITY)
+template <class Gather>
+B200_HD float trilinear_ray_fwd_packed_g(const Gather& gather, const VolDims& dims, const Ray& ray, float shift, int P, float amin,
+                                         float amax, float s_lo, float s_hi)
 {
     const PixLine pl = make_pixline(ray, dims, shift, 0);
     const float range = amax - amin;
@@ -1500,7 +1551,6 @@ B200_HD float trilinear_ray_fwd_packed(const float4* packed, const VolDims& dims
     int m_lo, m_hi;
     sample_range(pl, dims, amin, range, P, m_lo, m_hi);
     sample_range_slab(pl, amin, range, P, s_lo, s_hi, m_lo, m_hi);
-    const GatherPacked gather{packed};
     float acc = 0.0f;
     for (int m = m_lo; m <= m_hi; ++m) {
         const float alpha = add_rn(mul_rn(linspace01(m, P, lstep), range), amin);
@@ -1511,6 +1561,17 @@ B200_HD float trilinear_ray_fwd_packed(const float4* packed, const VolDims& dims
         acc += lerp8(gather(dims, pix));
     }
     return acc;
+}
+B200_HD float trilinear_ray_fwd_packed(const float4* packed, const VolDims& dims, const Ray& ray, float shift, int P,
+                                       float amin, float amax, float s_lo = -INFINITY, float s_hi = INFINITY)
+{
+    return trilinear_ray_fwd_packed_g(GatherPacked{packed}, dims, ray, shift, P, amin, amax, s_lo, s_hi);
+}
+template <class V>
+B200_HD float trilinear_ray_fwd_packed(const Cell16<V>* packed, const VolDims& dims, const Ray& ray, float shift, int P,
+                                       float amin, float amax, float s_lo = -INFINITY, float s_hi = INFINITY)
+{
+    return trilinear_ray_fwd_packed_g(GatherPacked16<V>{packed}, dims, ray, shift, P, amin, amax, s_lo, s_hi);
 }
 
 struct TriGrad {
@@ -1619,10 +1680,11 @@ B200_HD TriGrad trilinear_ray_bwd_g(const Gather& gather, const VolDims& dims, c
     return out;
 }
 
-B200_HD TriGrad trilinear_ray_bwd(const float* vol, const VolDims& dims, const Ray& ray, float shift, int P, float amin,
+template <class V = float>
+B200_HD TriGrad trilinear_ray_bwd(const V* vol, const VolDims& dims, const Ray& ray, float shift, int P, float amin,
                                   float amax, int align_corners, float g, float L, float* g_vol)
 {
-    return trilinear_ray_bwd_g(GatherPlain{vol}, dims, ray, shift, P, amin, amax, align_corners, g, L, g_vol);
+    return trilinear_ray_bwd_g(GatherPlainT<V>{vol}, dims, ray, shift, P, amin, amax, align_corners, g, L, g_vol);
 }
 
 // reducefn="max" (renderers.py:175-183 on Trilinear.forward): I = max_m (L V_m) step; the gradient flows through the
@@ -1663,6 +1725,13 @@ B200_HD TriGrad trilinear_ray_bwd_packed(const float4* packed, const VolDims& di
                                          float s_hi = INFINITY)
 {
     return trilinear_ray_bwd_g(GatherPacked{packed}, dims, ray, shift, P, amin, amax, 0, g, L, nullptr, s_lo, s_hi);
+}
+template <class V>
+B200_HD TriGrad trilinear_ray_bwd_packed(const Cell16<V>* packed, const VolDims& dims, const Ray& ray, float shift, int P,
+                                         float amin, float amax, float g, float L, float s_lo = -INFINITY,
+                                         float s_hi = INFINITY)
+{
+    return trilinear_ray_bwd_g(GatherPacked16<V>{packed}, dims, ray, shift, P, amin, amax, 0, g, L, nullptr, s_lo, s_hi);
 }
 
 // ===================================================================================================

@@ -27,7 +27,8 @@ __global__ void __launch_bounds__(kThreads) siddon_fwd_general_kernel(const floa
     out[r] = siddon_ray_general(vol, dims, ray, __ldg(raylen + r), shift, reduce, align_corners);
 }
 
-__global__ void __launch_bounds__(kThreads) siddon_fwd_fast_kernel(const float* __restrict__ vol, VolDims dims,
+template <class V>
+__global__ void __launch_bounds__(kThreads) siddon_fwd_fast_kernel(const V* __restrict__ vol, VolDims dims,
                                                                    const float* __restrict__ src,
                                                                    const float* __restrict__ tgt,
                                                                    const float* __restrict__ raylen,
@@ -55,7 +56,7 @@ __global__ void __launch_bounds__(kThreads) siddon_visits_kernel(VolDims dims, c
     const int64_t r = (int64_t)b * N + n;
     const Ray ray = load_ray(src, tgt, b, r, eps);
     int count = 0;
-    siddon_ray_fast<true>(nullptr, dims, ray, shift, &count);
+    siddon_ray_fast<true, float>(nullptr, dims, ray, shift, &count);
     visits[r] = count;
 }
 
@@ -149,8 +150,8 @@ __global__ void __launch_bounds__(TW* TH) siddon_fwd_grid_kernel(const float* __
 // (out is zero-filled by the launcher).
 // ---------------------------------------------------------------------------------------------------
 // MAJ = true: `slab` is a piece COUNT along each ray's own major axis (major_axis_piece; batches of one or two poses).
-template <int TW, int TH, int U, bool MAJ = false>
-__global__ void __launch_bounds__(TW* TH) siddon_fwd_slab_kernel(const float* __restrict__ vol, VolDims dims,
+template <int TW, int TH, int U, bool MAJ = false, class V = float>
+__global__ void __launch_bounds__(TW* TH) siddon_fwd_slab_kernel(const V* __restrict__ vol, VolDims dims,
                                                                  const float* __restrict__ src,
                                                                  const float* __restrict__ tgt,
                                                                  const float* __restrict__ raylen,
@@ -181,8 +182,8 @@ __global__ void __launch_bounds__(TW* TH) siddon_fwd_slab_kernel(const float* __
     if (part != 0.0f) red_add(out + r, L * part);
 }
 
-template <int TW, int TH, int U, bool MAJ = false>
-static cudaError_t launch_slab_variant(const float* vol, VolDims dims, const float* src, const float* tgt,
+template <int TW, int TH, int U, bool MAJ = false, class V = float>
+static cudaError_t launch_slab_variant(const V* vol, VolDims dims, const float* src, const float* tgt,
                                        const float* raylen, float* out, int B, int H, int W, int slab, float shift,
                                        float eps, cudaStream_t stream, PoseRays pr = PoseRays{nullptr, nullptr, nullptr, nullptr})
 {
@@ -191,7 +192,7 @@ static cudaError_t launch_slab_variant(const float* vol, VolDims dims, const flo
     if (blocks > INT32_MAX) return cudaErrorInvalidValue;
     cudaError_t e = cudaMemsetAsync(out, 0, sizeof(float) * (size_t)B * H * W, stream);
     if (e != cudaSuccess) return e;
-    siddon_fwd_slab_kernel<TW, TH, U, MAJ><<<(unsigned)blocks, TW * TH, 0, stream>>>(vol, dims, src, tgt, raylen, out, B, H, W,
+    siddon_fwd_slab_kernel<TW, TH, U, MAJ, V><<<(unsigned)blocks, TW * TH, 0, stream>>>(vol, dims, src, tgt, raylen, out, B, H, W,
                                                                                    slab, shift, eps, pr);
     return cudaGetLastError();
 }
@@ -490,7 +491,8 @@ static cudaError_t launch_grid_variant(const float* vol, VolDims dims, const flo
 // ---------------------------------------------------------------------------------------------------
 int small_batch_pieces(const VolDims& dims, int B, int H, int W, bool sens);  // defined next to the sensitivities launchers below
 
-cudaError_t launch_siddon_fwd_pose(const float* vol, VolDims dims, const float* src, const float* G, const float* Wd,
+template <class V>
+cudaError_t launch_siddon_fwd_pose(const V* vol, VolDims dims, const float* src, const float* G, const float* Wd,
                                    const float* rows, const float* cols, float* out, int B, int H, int W, float shift,
                                    float eps, cudaStream_t stream)
 {
@@ -501,6 +503,13 @@ cudaError_t launch_siddon_fwd_pose(const float* vol, VolDims dims, const float* 
     return launch_slab_variant<16, 16, 4>(vol, dims, src, nullptr, nullptr, out, B, H, W, 16, shift, eps, stream,
                                           PoseRays{G, Wd, rows, cols});
 }
+#define B200DRR_FWD_POSE(V)                                                                                                         \
+    template cudaError_t launch_siddon_fwd_pose<V>(const V*, VolDims, const float*, const float*, const float*, const float*,        \
+                                                   const float*, float*, int, int, int, float, float, cudaStream_t);
+B200DRR_FWD_POSE(float)
+B200DRR_FWD_POSE(VoxF16)
+B200DRR_FWD_POSE(VoxBF16)
+#undef B200DRR_FWD_POSE
 
 // g_G[b][a][k] = sum_n g_tgt[b][n][a] * p_k(n),  g_Wd[b][a][k] = sum_n g_raylen[b][n] * delta_a(n)/L(n) * p_k(n),
 // p(n) = (cols[w], rows[h], 1, 1): the chain rule through the in-kernel ray generation of make_ray().
@@ -579,8 +588,8 @@ cudaError_t launch_siddon_bwd_pose(const float* vol, VolDims dims, const float* 
 // Same slab-major decomposition as siddon_bwd_slab_kernel; partial sums via red.global.add (zero-filled by the launcher).
 // ---------------------------------------------------------------------------------------------------
 // MAJ = true: `slab` is a piece COUNT and the volume is cut along each ray's own major axis (major_axis_piece; small batches).
-template <int TW, int TH, int U, int MINB, bool MAJ = false>
-__global__ void __launch_bounds__(TW* TH, MINB) siddon_sens_slab_kernel(const float* __restrict__ vol, VolDims dims,
+template <int TW, int TH, int U, int MINB, bool MAJ = false, class V = float>
+__global__ void __launch_bounds__(TW* TH, MINB) siddon_sens_slab_kernel(const V* __restrict__ vol, VolDims dims,
                                                                   const float* __restrict__ src,
                                                                   const float* __restrict__ tgt,
                                                                   const float* __restrict__ raylen, float* __restrict__ out,
@@ -625,8 +634,8 @@ __global__ void __launch_bounds__(TW* TH, MINB) siddon_sens_slab_kernel(const fl
     }
 }
 
-template <int TW, int TH, int U, int MINB, bool MAJ = false>
-static cudaError_t launch_sens_slab_variant(const float* vol, VolDims dims, const float* src, const float* tgt,
+template <int TW, int TH, int U, int MINB, bool MAJ = false, class V = float>
+static cudaError_t launch_sens_slab_variant(const V* vol, VolDims dims, const float* src, const float* tgt,
                                             const float* raylen, float* out, float* sens, int B, int H, int W, int slab,
                                             float shift, float eps, cudaStream_t stream,
                                             PoseRays pr = PoseRays{nullptr, nullptr, nullptr, nullptr})
@@ -638,7 +647,7 @@ static cudaError_t launch_sens_slab_variant(const float* vol, VolDims dims, cons
     cudaError_t e = cudaMemsetAsync(out, 0, sizeof(float) * n, stream);
     if (e == cudaSuccess) e = cudaMemsetAsync(sens, 0, sizeof(float) * 8 * n, stream);
     if (e != cudaSuccess) return e;
-    siddon_sens_slab_kernel<TW, TH, U, MINB, MAJ><<<(unsigned)blocks, TW * TH, 0, stream>>>(vol, dims, src, tgt, raylen, out, sens,
+    siddon_sens_slab_kernel<TW, TH, U, MINB, MAJ, V><<<(unsigned)blocks, TW * TH, 0, stream>>>(vol, dims, src, tgt, raylen, out, sens,
                                                                                          B, H, W, slab, shift, eps, pr);
     return cudaGetLastError();
 }
@@ -757,6 +766,31 @@ int small_batch_pieces(const VolDims& dims, int B, int H, int W, bool sens)
     return k < 2 ? 0 : k;
 }
 
+// The library's choice for a full detector grid (variant 0): the brick kernel (siddon_sens_brick_route), the major-axis pieces for
+// small loads, one whole-volume slab for one or two poses, 16-plane slabs otherwise (16.8 MB of a 512^3 fp32 volume, well inside
+// the 50 MB L2).  The same rule for every voxel type: only the brick kernel's alignment differs (siddon_brick_supported).
+template <class V>
+cudaError_t launch_siddon_fwd_sens_grid_default(const V* vol, VolDims dims, const float* src, const float* tgt, const float* raylen,
+                                                float* out, float* sens, int B, int H, int W, float shift, float eps,
+                                                cudaStream_t stream)
+{
+    if (siddon_sens_brick_route(dims, B, H, W, vol, sens, (int)sizeof(V)))  // brick-major (siddon_brick.cu)
+        return launch_siddon_fwd_sens_brick(vol, dims, src, tgt, raylen, nullptr, nullptr, nullptr, nullptr, out, sens, B, H, W, shift,
+                                            eps, stream);
+    const int pieces = small_batch_pieces(dims, B, H, W, true);
+    if (pieces > 0)
+        return launch_sens_slab_variant<8, 16, 8, 8, true>(vol, dims, src, tgt, raylen, out, sens, B, H, W, pieces, shift, eps, stream);
+    if (B <= 2)  // few poses: no cross-pose L2 sharing to win, skip the slab decomposition
+        return launch_sens_slab_variant<8, 16, 8, 8>(vol, dims, src, tgt, raylen, out, sens, B, H, W, dims.d[0], shift, eps, stream);
+    return launch_sens_slab_variant<8, 16, 8, 8>(vol, dims, src, tgt, raylen, out, sens, B, H, W, 16, shift, eps, stream);
+}
+#define B200DRR_SENS_GRID(V)                                                                                                        \
+    template cudaError_t launch_siddon_fwd_sens_grid_default<V>(const V*, VolDims, const float*, const float*, const float*, float*, \
+                                                                float*, int, int, int, float, float, cudaStream_t);
+B200DRR_SENS_GRID(VoxF16)
+B200DRR_SENS_GRID(VoxBF16)
+#undef B200DRR_SENS_GRID
+
 cudaError_t launch_siddon_fwd_sens_grid(const float* vol, VolDims dims, const float* src, const float* tgt,
                                         const float* raylen, float* out, float* sens, int B, int H, int W, float shift,
                                         float eps, int variant, cudaStream_t stream)
@@ -765,7 +799,8 @@ cudaError_t launch_siddon_fwd_sens_grid(const float* vol, VolDims dims, const fl
     case id:                                                                                                             \
         return launch_sens_slab_variant<TW, TH, U, MINB>(vol, dims, src, tgt, raylen, out, sens, B, H, W, SLAB, shift, eps, \
                                                          stream);
-    if (variant == 42 || (variant == 0 && siddon_sens_brick_route(dims, B, H, W, vol, sens)))  // brick-major (siddon_brick.cu)
+    if (variant == 0) return launch_siddon_fwd_sens_grid_default(vol, dims, src, tgt, raylen, out, sens, B, H, W, shift, eps, stream);
+    if (variant == 42)  // brick-major (siddon_brick.cu)
         return launch_siddon_fwd_sens_brick(vol, dims, src, tgt, raylen, nullptr, nullptr, nullptr, nullptr, out, sens, B, H, W, shift,
                                             eps, stream);
     if (variant > 100 && variant <= 164)  // tuning: 101..164 = that many major-axis pieces, whatever the batch size
@@ -777,17 +812,7 @@ cudaError_t launch_siddon_fwd_sens_grid(const float* vol, VolDims dims, const fl
     if (variant > 400 && variant <= 464)
         return launch_sens_slab_variant<8, 16, 4, 8, true>(vol, dims, src, tgt, raylen, out, sens, B, H, W, variant - 400, shift, eps,
                                                            stream);
-    if (variant == 0) {
-        const int pieces = small_batch_pieces(dims, B, H, W, true);
-        if (pieces > 0)
-            return launch_sens_slab_variant<8, 16, 8, 8, true>(vol, dims, src, tgt, raylen, out, sens, B, H, W, pieces, shift, eps,
-                                                               stream);
-    }
-    if (variant == 0 && B <= 2)  // few poses: no cross-pose L2 sharing to win, skip the slab decomposition
-        return launch_sens_slab_variant<8, 16, 8, 8>(vol, dims, src, tgt, raylen, out, sens, B, H, W, dims.d[0], shift, eps,
-                                                     stream);
     switch (variant) {
-        SV(0, 8, 16, 8, 16, 8)  // default: 16-plane slabs (16.8 MB of a 512^3 fp32 volume, well inside the 50 MB L2)
         SV(38, 8, 16, 8, 48, 8)
         SV(32, 16, 8, 8, 48, 8)
         SV(33, 8, 16, 8, 128, 8)
@@ -832,11 +857,12 @@ cudaError_t launch_siddon_fwd_sens_grid(const float* vol, VolDims dims, const fl
 #undef SV
 }
 
-cudaError_t launch_siddon_fwd_sens_pose(const float* vol, VolDims dims, const float* src, const float* G, const float* Wd,
+template <class V>
+cudaError_t launch_siddon_fwd_sens_pose(const V* vol, VolDims dims, const float* src, const float* G, const float* Wd,
                                         const float* rows, const float* cols, float* out, float* sens, int B, int H, int W,
                                         float shift, float eps, cudaStream_t stream)
 {
-    if (siddon_sens_brick_route(dims, B, H, W, vol, sens))
+    if (siddon_sens_brick_route(dims, B, H, W, vol, sens, (int)sizeof(V)))
         return launch_siddon_fwd_sens_brick(vol, dims, src, nullptr, nullptr, G, Wd, rows, cols, out, sens, B, H, W, shift, eps, stream);
     const int pieces = small_batch_pieces(dims, B, H, W, true);
     if (pieces > 0)
@@ -848,6 +874,13 @@ cudaError_t launch_siddon_fwd_sens_pose(const float* vol, VolDims dims, const fl
                                                  B <= 2 ? dims.d[0] : 16, shift, eps, stream,
                                                  PoseRays{G, Wd, rows, cols});
 }
+#define B200DRR_SENS_POSE(V)                                                                                                        \
+    template cudaError_t launch_siddon_fwd_sens_pose<V>(const V*, VolDims, const float*, const float*, const float*, const float*,   \
+                                                        const float*, float*, float*, int, int, int, float, float, cudaStream_t);
+B200DRR_SENS_POSE(float)
+B200DRR_SENS_POSE(VoxF16)
+B200DRR_SENS_POSE(VoxBF16)
+#undef B200DRR_SENS_POSE
 
 // Backward from the saved sensitivities, arbitrary-ray layout: g_tgt = g * dI/dt, g_raylen = g * S, g_src = sum_n g * dI/ds.
 __global__ void __launch_bounds__(256) sens_bwd_kernel(const float4* __restrict__ sens, const float* __restrict__ gout,
@@ -966,14 +999,28 @@ cudaError_t launch_siddon_bwd_sens_pose(const float* sens, const float* gout, co
     return cudaGetLastError();
 }
 
+// The library's choice for a full detector grid (variant 0): the major-axis pieces for small loads, 16-plane slabs otherwise.
+template <class V>
+cudaError_t launch_siddon_fwd_grid_default(const V* vol, VolDims dims, const float* src, const float* tgt, const float* raylen,
+                                           float* out, int B, int H, int W, float shift, float eps, cudaStream_t stream)
+{
+    const int pieces = small_batch_pieces(dims, B, H, W, false);
+    if (pieces > 0) return launch_slab_variant<16, 16, 4, true>(vol, dims, src, tgt, raylen, out, B, H, W, pieces, shift, eps, stream);
+    return launch_slab_variant<16, 16, 4>(vol, dims, src, tgt, raylen, out, B, H, W, 16, shift, eps, stream);
+}
+#define B200DRR_FWD_GRID(V)                                                                                                         \
+    template cudaError_t launch_siddon_fwd_grid_default<V>(const V*, VolDims, const float*, const float*, const float*, float*, int, \
+                                                           int, int, float, float, cudaStream_t);
+B200DRR_FWD_GRID(VoxF16)
+B200DRR_FWD_GRID(VoxBF16)
+#undef B200DRR_FWD_GRID
+
 cudaError_t launch_siddon_fwd_grid(const float* vol, VolDims dims, const float* src, const float* tgt,
                                    const float* raylen, float* out, int B, int H, int W, float shift, float eps,
                                    int variant, cudaStream_t stream)
 {
 #define V(id, TW, TH, U, LEAN) \
     case id: return launch_grid_variant<TW, TH, U, LEAN>(vol, dims, src, tgt, raylen, out, B, H, W, shift, eps, stream);
-#define S0(id, TW, TH, U, SLAB) \
-    case id: return launch_slab_variant<TW, TH, U>(vol, dims, src, tgt, raylen, out, B, H, W, SLAB, shift, eps, stream);
     if (variant > 100 && variant <= 164)  // tuning: 101..164 = that many major-axis pieces, whatever the batch size
         return launch_slab_variant<16, 16, 4, true>(vol, dims, src, tgt, raylen, out, B, H, W, variant - 100, shift, eps, stream);
     if (variant > 200 && variant <= 264)
@@ -982,12 +1029,8 @@ cudaError_t launch_siddon_fwd_grid(const float* vol, VolDims dims, const float* 
         return launch_slab_variant<16, 8, 4, true>(vol, dims, src, tgt, raylen, out, B, H, W, variant - 300, shift, eps, stream);
     if (variant > 400 && variant <= 464)
         return launch_slab_variant<8, 16, 4, true>(vol, dims, src, tgt, raylen, out, B, H, W, variant - 400, shift, eps, stream);
-    if (variant == 0) {
-        const int pieces = small_batch_pieces(dims, B, H, W, false);
-        if (pieces > 0) return launch_slab_variant<16, 16, 4, true>(vol, dims, src, tgt, raylen, out, B, H, W, pieces, shift, eps, stream);
-    }
+    if (variant == 0) return launch_siddon_fwd_grid_default(vol, dims, src, tgt, raylen, out, B, H, W, shift, eps, stream);
     switch (variant) {
-        S0(0, 16, 16, 4, 16)
         V(30, 16, 8, 4, 1)
         V(1, 16, 8, 8, 0)
         V(2, 16, 8, 2, 1)
@@ -1239,15 +1282,29 @@ cudaError_t launch_siddon_bwd_mask(const float* vol, const float* mask, VolDims 
 
 static inline dim3 ray_grid(int B, int64_t N) { return dim3((unsigned)((N + kThreads - 1) / kThreads), (unsigned)B, 1); }
 
+// one thread per ray, default options (reducefn="sum", align_corners=False)
+template <class V>
+cudaError_t launch_siddon_fwd_fast(const V* vol, VolDims dims, const float* src, const float* tgt, const float* raylen, float* out,
+                                   int B, int64_t N, float shift, float eps, cudaStream_t stream)
+{
+    siddon_fwd_fast_kernel<V><<<ray_grid(B, N), kThreads, 0, stream>>>(vol, dims, src, tgt, raylen, out, N, shift, eps);
+    return cudaGetLastError();
+}
+#define B200DRR_FWD_FAST(V)                                                                                                         \
+    template cudaError_t launch_siddon_fwd_fast<V>(const V*, VolDims, const float*, const float*, const float*, float*, int, int64_t, \
+                                                   float, float, cudaStream_t);
+B200DRR_FWD_FAST(VoxF16)
+B200DRR_FWD_FAST(VoxBF16)
+#undef B200DRR_FWD_FAST
+
 cudaError_t launch_siddon_fwd(const float* vol, VolDims dims, const float* src, const float* tgt,
                               const float* raylen, float* out, int B, int64_t N, float shift, float eps, int reduce,
                               int align_corners, cudaStream_t stream)
 {
     if (reduce == 0 && !align_corners)
-        siddon_fwd_fast_kernel<<<ray_grid(B, N), kThreads, 0, stream>>>(vol, dims, src, tgt, raylen, out, N, shift, eps);
-    else
-        siddon_fwd_general_kernel<<<ray_grid(B, N), kThreads, 0, stream>>>(vol, dims, src, tgt, raylen, out, N, shift,
-                                                                          eps, reduce, align_corners);
+        return launch_siddon_fwd_fast(vol, dims, src, tgt, raylen, out, B, N, shift, eps, stream);
+    siddon_fwd_general_kernel<<<ray_grid(B, N), kThreads, 0, stream>>>(vol, dims, src, tgt, raylen, out, N, shift, eps, reduce,
+                                                                      align_corners);
     return cudaGetLastError();
 }
 
@@ -1260,7 +1317,8 @@ cudaError_t launch_siddon_visits(VolDims dims, const float* src, const float* tg
 
 // Forward with sensitivities for ARBITRARY ray sets (sub-sampled / patched / user rays): one thread per ray over the
 // whole volume, plain stores (no slabs, so no partial sums).  Volumes too large for 32-bit offsets are refused.
-__global__ void __launch_bounds__(kThreads) siddon_sens_kernel(const float* __restrict__ vol, VolDims dims,
+template <class V>
+__global__ void __launch_bounds__(kThreads) siddon_sens_kernel(const V* __restrict__ vol, VolDims dims,
                                                                const float* __restrict__ src, const float* __restrict__ tgt,
                                                                const float* __restrict__ raylen, float* __restrict__ out,
                                                                float* __restrict__ sens, int64_t N, float shift, float eps)
@@ -1294,8 +1352,8 @@ __global__ void __launch_bounds__(kThreads) siddon_sens_kernel(const float* __re
 // pose is simply thread i, so the 32 lanes of a warp walk 32 spatial neighbours and share 128-byte lines exactly like
 // the 8 x 4 pixel bundles of the detector-grid kernels.  Same slab decomposition, same per-ray math, same atomics.
 // ---------------------------------------------------------------------------------------------------
-template <int THREADS, int U>
-__global__ void __launch_bounds__(THREADS) siddon_fwd_slab_linear_kernel(const float* __restrict__ vol, VolDims dims,
+template <int THREADS, int U, class V>
+__global__ void __launch_bounds__(THREADS) siddon_fwd_slab_linear_kernel(const V* __restrict__ vol, VolDims dims,
                                                                          const float* __restrict__ src,
                                                                          const float* __restrict__ tgt,
                                                                          const float* __restrict__ raylen,
@@ -1319,9 +1377,9 @@ __global__ void __launch_bounds__(THREADS) siddon_fwd_slab_linear_kernel(const f
     if (part != 0.0f) red_add(out + r, __ldg(raylen + r) * part);
 }
 
-template <int THREADS, int U>
+template <int THREADS, int U, class V>
 __global__ void __launch_bounds__(THREADS, 2048 / THREADS / 4) siddon_sens_slab_linear_kernel(
-    const float* __restrict__ vol, VolDims dims, const float* __restrict__ src, const float* __restrict__ tgt,
+    const V* __restrict__ vol, VolDims dims, const float* __restrict__ src, const float* __restrict__ tgt,
     const float* __restrict__ raylen, float* __restrict__ out, float* __restrict__ sens, int B, int64_t N, int slab, float shift,
     float eps)
 {
@@ -1357,7 +1415,8 @@ __global__ void __launch_bounds__(THREADS, 2048 / THREADS / 4) siddon_sens_slab_
     }
 }
 
-cudaError_t launch_siddon_fwd_sorted(const float* vol, VolDims dims, const float* src, const float* tgt, const float* raylen,
+template <class V>
+cudaError_t launch_siddon_fwd_sorted(const V* vol, VolDims dims, const float* src, const float* tgt, const float* raylen,
                                      float* out, int B, int64_t N, float shift, float eps, cudaStream_t stream)
 {
     constexpr int T = 128, SLAB = 32;
@@ -1368,11 +1427,12 @@ cudaError_t launch_siddon_fwd_sorted(const float* vol, VolDims dims, const float
     if (blocks > INT32_MAX) return cudaErrorInvalidValue;
     cudaError_t e = cudaMemsetAsync(out, 0, sizeof(float) * (size_t)B * N, stream);
     if (e != cudaSuccess) return e;
-    siddon_fwd_slab_linear_kernel<T, 4><<<(unsigned)blocks, T, 0, stream>>>(vol, dims, src, tgt, raylen, out, B, N, slab, shift, eps);
+    siddon_fwd_slab_linear_kernel<T, 4, V><<<(unsigned)blocks, T, 0, stream>>>(vol, dims, src, tgt, raylen, out, B, N, slab, shift, eps);
     return cudaGetLastError();
 }
 
-cudaError_t launch_siddon_fwd_sens_sorted(const float* vol, VolDims dims, const float* src, const float* tgt, const float* raylen,
+template <class V>
+cudaError_t launch_siddon_fwd_sens_sorted(const V* vol, VolDims dims, const float* src, const float* tgt, const float* raylen,
                                           float* out, float* sens, int B, int64_t N, float shift, float eps, cudaStream_t stream)
 {
     constexpr int T = 128, SLAB = 48;
@@ -1384,18 +1444,30 @@ cudaError_t launch_siddon_fwd_sens_sorted(const float* vol, VolDims dims, const 
     cudaError_t e = cudaMemsetAsync(out, 0, sizeof(float) * (size_t)B * N, stream);
     if (e == cudaSuccess) e = cudaMemsetAsync(sens, 0, sizeof(float) * 8 * (size_t)B * N, stream);
     if (e != cudaSuccess) return e;
-    siddon_sens_slab_linear_kernel<T, 8><<<(unsigned)blocks, T, 0, stream>>>(vol, dims, src, tgt, raylen, out, sens, B, N, slab, shift,
+    siddon_sens_slab_linear_kernel<T, 8, V><<<(unsigned)blocks, T, 0, stream>>>(vol, dims, src, tgt, raylen, out, sens, B, N, slab, shift,
                                                                             eps);
     return cudaGetLastError();
 }
 
-cudaError_t launch_siddon_fwd_sens(const float* vol, VolDims dims, const float* src, const float* tgt, const float* raylen,
+template <class V>
+cudaError_t launch_siddon_fwd_sens(const V* vol, VolDims dims, const float* src, const float* tgt, const float* raylen,
                                    float* out, float* sens, int B, int64_t N, float shift, float eps, cudaStream_t stream)
 {
     if ((int64_t)dims.d[0] * dims.d[1] * dims.d[2] >= (int64_t)INT32_MAX) return cudaErrorInvalidValue;
-    siddon_sens_kernel<<<ray_grid(B, N), kThreads, 0, stream>>>(vol, dims, src, tgt, raylen, out, sens, N, shift, eps);
+    siddon_sens_kernel<V><<<ray_grid(B, N), kThreads, 0, stream>>>(vol, dims, src, tgt, raylen, out, sens, N, shift, eps);
     return cudaGetLastError();
 }
+#define B200DRR_ARBITRARY_RAYS(V)                                                                                                   \
+    template cudaError_t launch_siddon_fwd_sorted<V>(const V*, VolDims, const float*, const float*, const float*, float*, int,     \
+                                                     int64_t, float, float, cudaStream_t);                                         \
+    template cudaError_t launch_siddon_fwd_sens_sorted<V>(const V*, VolDims, const float*, const float*, const float*, float*,     \
+                                                          float*, int, int64_t, float, float, cudaStream_t);                      \
+    template cudaError_t launch_siddon_fwd_sens<V>(const V*, VolDims, const float*, const float*, const float*, float*, float*,    \
+                                                   int, int64_t, float, float, cudaStream_t);
+B200DRR_ARBITRARY_RAYS(float)
+B200DRR_ARBITRARY_RAYS(VoxF16)
+B200DRR_ARBITRARY_RAYS(VoxBF16)
+#undef B200DRR_ARBITRARY_RAYS
 
 cudaError_t launch_siddon_bwd(const float* vol, VolDims dims, const float* src, const float* tgt,
                               const float* raylen, const float* gout, float* g_src, float* g_tgt, float* g_raylen,

@@ -19,6 +19,7 @@
 #include <cuda.h>  // CUtensorMap + enums only; the encoder is fetched through cudaGetDriverEntryPoint (no -lcuda)
 
 #include <mutex>
+#include <type_traits>
 
 #include "brick.cuh"
 #include "kernels.h"
@@ -103,18 +104,26 @@ struct StShared {
 #ifndef B200DRR_FWD_SWIZZLE
 #define B200DRR_FWD_SWIZZLE 0
 #endif
-struct LdShared {
+// V = the staged voxel type: fp32, or a 16-bit VoxF16 / VoxBF16 (ld.shared.u16, widened by vox16_to_f32; unswizzled).
+template <class V>
+struct LdSharedT {
     uint32_t base_addr;
-    static constexpr int kScale = 4;
+    static constexpr int kScale = (int)sizeof(V);
     __device__ __forceinline__ int base() const { return (int)base_addr; }
     __device__ __forceinline__ float operator()(int off) const
     {
-        float v;
+        if constexpr (sizeof(V) == 4) {
+            float v;
 #if B200DRR_FWD_SWIZZLE
-        off ^= (off >> 3) & 0x70;
+            off ^= (off >> 3) & 0x70;
 #endif
-        asm volatile("ld.shared.f32 %0, [%1];" : "=f"(v) : "r"(off));
-        return v;
+            asm volatile("ld.shared.f32 %0, [%1];" : "=f"(v) : "r"(off));
+            return v;
+        } else {
+            unsigned short h;
+            asm volatile("ld.shared.u16 %0, [%1];" : "=h"(h) : "r"(off));
+            return vox16_to_f32(h, std::is_same<V, VoxBF16>::value);
+        }
     }
 };
 
@@ -218,12 +227,12 @@ struct BrickGrid {
     int nb0, nb1, nb2;  // bricks per axis
 };
 
-template <int BX, int BY, int BZ, int STAGES, int THREADS, int K, int U, int CTAS, int PIPE, int RAYS = 1>
+template <int BX, int BY, int BZ, int STAGES, int THREADS, int K, int U, int CTAS, int PIPE, int RAYS = 1, class V = float>
 struct BrickCfg {
     // 4-row tile bands per pose chunk (a chunk takes as many poses as fit); the two-CTA-per-SM shape has less room
     static constexpr int kRowCap = CTAS == 1 ? 512 : 256;
     static constexpr int kBrickElems = BX * BY * BZ;
-    static constexpr int kBrickBytes = kBrickElems * 4;
+    static constexpr int kBrickBytes = kBrickElems * (int)sizeof(V);  // 16-bit voxels: half the bytes, same shape
     static constexpr int kWarps = THREADS / 32;
     static constexpr int kCap = kWarps * K * 32;  // items per round (every candidate of a round may hit)
     static constexpr int kPB = kBrickPoseChunk;
@@ -251,7 +260,8 @@ struct BrickCfg {
 // SENS = 1: training-step mode (full detector grids).  Every pair rebuilds its ray, runs the exact-frame sensitivities walk over
 // the staged brick (brick_pair_sens) and flushes like siddon_sens_slab_kernel: two red.global.add.v4 into sa.sens (dI/dt, S,
 // dI/ds) and L * S into out, nothing for an all-zero pair.  The work list is sorted by major axis first (sens_bin).
-template <int BX, int BY, int BZ, int STAGES, int THREADS, int K, int U, int CTAS, int PIPE, int RAYS, int BWD = 0, int SENS = 0>
+template <int BX, int BY, int BZ, int STAGES, int THREADS, int K, int U, int CTAS, int PIPE, int RAYS, int BWD = 0, int SENS = 0,
+          class V = float>
 __global__ void __launch_bounds__(THREADS, CTAS)
     siddon_fwd_brick_kernel(const __grid_constant__ CUtensorMap tmap, VolDims dims, BrickGrid bg,
                             const float4* __restrict__ raytab, const float* __restrict__ ltab,
@@ -259,8 +269,10 @@ __global__ void __launch_bounds__(THREADS, CTAS)
                             const int* __restrict__ pix_index /* [H*W] pixel -> ray index, -1 = no ray; nullptr = full grid */,
                             int Nr /* rays per pose */, int B, int H, int W, float shift, SensArgs sa)
 {
-    using Cfg = BrickCfg<BX, BY, BZ, STAGES, THREADS, K, U, CTAS, PIPE, RAYS>;
+    using Cfg = BrickCfg<BX, BY, BZ, STAGES, THREADS, K, U, CTAS, PIPE, RAYS, V>;
+    using LdShared = LdSharedT<V>;
     static_assert(BWD == 0 || (STAGES == 1 && RAYS == 1), "volume-gradient mode: single stage, one pair per thread");
+    static_assert(BWD == 0 || sizeof(V) == 4, "the volume gradient is fp32");
     static_assert(SENS == 0 || (BWD == 0 && RAYS == 1), "sensitivities mode: forward walk, one pair per thread");
     constexpr int kRowCap = Cfg::kRowCap;
     extern __shared__ __align__(1024) unsigned char smem[];
@@ -845,29 +857,38 @@ EncodeTiledFn get_encoder()
     return fn;
 }
 
-bool make_volume_map(CUtensorMap* map, const float* vol, VolDims dims, int BX, int BY, int BZ, bool swizzle128 = false)
+template <class V> constexpr CUtensorMapDataType tmap_type() { return CU_TENSOR_MAP_DATA_TYPE_FLOAT32; }
+template <> constexpr CUtensorMapDataType tmap_type<VoxF16>() { return CU_TENSOR_MAP_DATA_TYPE_FLOAT16; }
+template <> constexpr CUtensorMapDataType tmap_type<VoxBF16>() { return CU_TENSOR_MAP_DATA_TYPE_BFLOAT16; }
+
+// Out-of-bounds elements are zero-filled (+0.0 in every element type).  The global strides must be multiples of 16 bytes:
+// D2 % 4 == 0 for fp32 voxels, D2 % 8 == 0 for 16-bit ones (siddon_brick_supported).
+template <class V>
+bool make_volume_map(CUtensorMap* map, const V* vol, VolDims dims, int BX, int BY, int BZ, bool swizzle128 = false)
 {
     EncodeTiledFn enc = get_encoder();
     if (!enc) return false;
+    constexpr cuuint64_t es = sizeof(V);
     const cuuint64_t gdim[3] = {(cuuint64_t)dims.d[2], (cuuint64_t)dims.d[1], (cuuint64_t)dims.d[0]};
-    const cuuint64_t gstride[2] = {(cuuint64_t)dims.d[2] * 4, (cuuint64_t)dims.d[2] * dims.d[1] * 4};
+    const cuuint64_t gstride[2] = {(cuuint64_t)dims.d[2] * es, (cuuint64_t)dims.d[2] * dims.d[1] * es};
     const cuuint32_t box[3] = {(cuuint32_t)BZ, (cuuint32_t)BY, (cuuint32_t)BX};
     const cuuint32_t estr[3] = {1, 1, 1};
-    return enc(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, const_cast<float*>(vol), gdim, gstride, box, estr,
-               CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle128 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_NONE,
+    return enc(map, tmap_type<V>(), 3, const_cast<V*>(vol), gdim, gstride, box, estr,
+               CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle128 && es == 4 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_NONE,
                CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
                CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
 
 size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
 
-template <int BX, int BY, int BZ, int STAGES, int THREADS, int K, int U, int CTAS, int PIPE, int RAYS = 1, int BWD = 0, int SENS = 0>
+template <int BX, int BY, int BZ, int STAGES, int THREADS, int K, int U, int CTAS, int PIPE, int RAYS = 1, int BWD = 0, int SENS = 0,
+          class V = float>
 cudaError_t launch_brick_variant(const CUtensorMap& map, VolDims dims, const float4* raytab, const float* ltab,
                                  const PoseGeo* geo, float* out, unsigned* counter, const int* pix_index, int Nr, int B, int H,
                                  int W, float shift, cudaStream_t stream, const SensArgs& sa = SensArgs{})
 {
-    using Cfg = BrickCfg<BX, BY, BZ, STAGES, THREADS, K, U, CTAS, PIPE, RAYS>;
-    auto kern = siddon_fwd_brick_kernel<BX, BY, BZ, STAGES, THREADS, K, U, CTAS, PIPE, RAYS, BWD, SENS>;
+    using Cfg = BrickCfg<BX, BY, BZ, STAGES, THREADS, K, U, CTAS, PIPE, RAYS, V>;
+    auto kern = siddon_fwd_brick_kernel<BX, BY, BZ, STAGES, THREADS, K, U, CTAS, PIPE, RAYS, BWD, SENS, V>;
     static bool configured = false;
     if (!configured) {
         cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes);
@@ -896,22 +917,23 @@ size_t siddon_brick_workspace_bytes(int B, int H, int W)
     return 256 + align_up(sizeof(PoseGeo) * (size_t)B, 256) + (sizeof(float4) + sizeof(float)) * (size_t)B * H * W;
 }
 
-bool siddon_brick_supported(VolDims dims, int H, int W)
+bool siddon_brick_supported(VolDims dims, int H, int W, int elem_bytes)
 {
-    return dims.d[2] % 4 == 0 && H <= kBrickMaxSide && W <= kBrickMaxSide && H >= 2 && W >= 2 && get_encoder() != nullptr;
+    return ((int64_t)dims.d[2] * elem_bytes) % 16 == 0 && H <= kBrickMaxSide && W <= kBrickMaxSide && H >= 2 && W >= 2 && get_encoder() != nullptr;
 }
 
 // pix_index / corners / Nsub describe a ray SUBSET of the H x W grid (all nullptr / 0 for the full grid): tgt, raylen and out
 // are then (B, Nsub) arrays, pix_index [H*W] maps a pixel to its ray (-1: none), corners [B][3][3] are the voxel-space
 // targets of the full grid's pixels (0,0), (0,W-1), (H-1,0).
-cudaError_t launch_siddon_fwd_brick(const float* vol, VolDims dims, const float* src, const float* tgt, const float* raylen,
+template <class V>
+cudaError_t launch_siddon_fwd_brick(const V* vol, VolDims dims, const float* src, const float* tgt, const float* raylen,
                                     const float* G, const float* Wd, const float* rows, const float* cols, float* out,
                                     void* workspace, size_t workspace_bytes, int B, int H, int W, float shift, float eps,
                                     int variant, cudaStream_t stream, const int* pix_index, const float* corners, int64_t Nsub)
 {
     const bool subset = pix_index != nullptr;
     const int64_t Nr = subset ? Nsub : (int64_t)H * W;
-    if (!siddon_brick_supported(dims, H, W) || ((uintptr_t)vol & 15u) != 0 || (int64_t)B * Nr >= ((int64_t)1 << 31) || Nr <= 0 ||
+    if (!siddon_brick_supported(dims, H, W, (int)sizeof(V)) || ((uintptr_t)vol & 15u) != 0 || (int64_t)B * Nr >= ((int64_t)1 << 31) || Nr <= 0 ||
         Nr > (int64_t)H * W || (subset && (corners == nullptr || G != nullptr)))
         return cudaErrorNotSupported;
     const size_t need = 256 + align_up(sizeof(PoseGeo) * (size_t)B, 256) + (sizeof(float4) + sizeof(float)) * (size_t)B * Nr;
@@ -931,18 +953,24 @@ cudaError_t launch_siddon_fwd_brick(const float* vol, VolDims dims, const float*
 #define BV(id, BX, BY, BZ, STAGES, THREADS, K, U, CTAS, PIPE)                                                            \
     case id:                                                                                                             \
         if (!make_volume_map(&map, vol, dims, BX, BY, BZ, B200DRR_FWD_SWIZZLE != 0 && BZ == 32)) return cudaErrorNotSupported;                                 \
-        return launch_brick_variant<BX, BY, BZ, STAGES, THREADS, K, U, CTAS, PIPE>(map, dims, raytab, ltab, geo, out, counter, \
+        return launch_brick_variant<BX, BY, BZ, STAGES, THREADS, K, U, CTAS, PIPE, 1, 0, 0, V>(map, dims, raytab, ltab, geo, out, counter, \
                                                                                    pix_index, (int)Nr, B, H, W, shift, stream);
 #define BV3(id, BX, BY, BZ, STAGES, THREADS, K, U, CTAS)                                                                 \
     case id:                                                                                                             \
         if (!make_volume_map(&map, vol, dims, BX, BY, BZ, B200DRR_FWD_SWIZZLE != 0 && BZ == 32)) return cudaErrorNotSupported;                                 \
-        return launch_brick_variant<BX, BY, BZ, STAGES, THREADS, K, U, CTAS, 0, 3>(map, dims, raytab, ltab, geo, out, counter, \
+        return launch_brick_variant<BX, BY, BZ, STAGES, THREADS, K, U, CTAS, 0, 3, 0, 0, V>(map, dims, raytab, ltab, geo, out, counter, \
                                                                                    pix_index, (int)Nr, B, H, W, shift, stream);
 #define BV2(id, BX, BY, BZ, STAGES, THREADS, K, U, CTAS)                                                                 \
     case id:                                                                                                             \
         if (!make_volume_map(&map, vol, dims, BX, BY, BZ, B200DRR_FWD_SWIZZLE != 0 && BZ == 32)) return cudaErrorNotSupported;                                 \
-        return launch_brick_variant<BX, BY, BZ, STAGES, THREADS, K, U, CTAS, 0, 2>(map, dims, raytab, ltab, geo, out, counter, \
+        return launch_brick_variant<BX, BY, BZ, STAGES, THREADS, K, U, CTAS, 0, 2, 0, 0, V>(map, dims, raytab, ltab, geo, out, counter, \
                                                                                    pix_index, (int)Nr, B, H, W, shift, stream);
+    if constexpr (sizeof(V) != 4) {  // 16-bit volumes: the production shape only (the tuning variants are fp32-only)
+        if (variant != 0) return cudaErrorInvalidValue;
+        if (!make_volume_map(&map, vol, dims, 24, 32, 32)) return cudaErrorNotSupported;
+        return launch_brick_variant<24, 32, 32, 1, 512, 4, 2, 2, 0, 1, 0, 0, V>(map, dims, raytab, ltab, geo, out, counter, pix_index,
+                                                                                (int)Nr, B, H, W, shift, stream);
+    } else {
     switch (variant) {
         BV(0, 24, 32, 32, 1, 512, 4, 2, 2, 0)    // two CTAs per SM, one 96 KB brick each (production shape)
         BV(7, 24, 32, 32, 2, 1024, 4, 2, 1, 1)   // one CTA per SM with a two-stage TMA + mbarrier pipeline (slower: CTA-wide barriers)
@@ -969,10 +997,21 @@ cudaError_t launch_siddon_fwd_brick(const float* vol, VolDims dims, const float*
 #endif
         default: return cudaErrorInvalidValue;
     }
+    }
 #undef BV
 #undef BV2
 #undef BV3
 }
+template cudaError_t launch_siddon_fwd_brick<float>(const float*, VolDims, const float*, const float*, const float*, const float*,
+                                                    const float*, const float*, const float*, float*, void*, size_t, int, int, int,
+                                                    float, float, int, cudaStream_t, const int*, const float*, int64_t);
+template cudaError_t launch_siddon_fwd_brick<VoxF16>(const VoxF16*, VolDims, const float*, const float*, const float*, const float*,
+                                                     const float*, const float*, const float*, float*, void*, size_t, int, int, int,
+                                                     float, float, int, cudaStream_t, const int*, const float*, int64_t);
+template cudaError_t launch_siddon_fwd_brick<VoxBF16>(const VoxBF16*, VolDims, const float*, const float*, const float*,
+                                                      const float*, const float*, const float*, const float*, float*, void*, size_t,
+                                                      int, int, int, float, float, int, cudaStream_t, const int*, const float*,
+                                                      int64_t);
 
 // Volume gradient of the full-grid Siddon render through the brick kernel's BWD mode: g_vol [D0][D1][D2] is OVERWRITTEN with
 // sum over poses and rays of gout * raylen * chord length (what autograd gives for renderers.py:40-76 w.r.t. the volume).
@@ -982,7 +1021,7 @@ cudaError_t launch_siddon_bwd_vol_brick(const float* gout, VolDims dims, const f
                                         cudaStream_t stream)
 {
     const int64_t Nr = (int64_t)H * W;
-    if (!siddon_brick_supported(dims, H, W) || ((uintptr_t)g_vol & 15u) != 0 || (int64_t)B * Nr >= ((int64_t)1 << 31))
+    if (!siddon_brick_supported(dims, H, W, 4) || ((uintptr_t)g_vol & 15u) != 0 || (int64_t)B * Nr >= ((int64_t)1 << 31))
         return cudaErrorNotSupported;
     const size_t need = siddon_brick_workspace_bytes(B, H, W);
     if (workspace == nullptr || workspace_bytes < need || ((uintptr_t)workspace & 255u) != 0) return cudaErrorInvalidValue;
@@ -1028,13 +1067,13 @@ constexpr int kSensBrickMinBatch = 4;
 // the dynamic queue of 2 x 132 resident CTAs to balance (>= 2048 bricks of 24 x 32 x 32), the rays are sparse (detector pixels at
 // most half the voxels of a volume cross-section, as the module's forward routing requires: dense rays share L1 sectors and the
 // slab-major gather wins) and the batch is big enough for the staged bricks to be shared.
-bool siddon_sens_brick_route(VolDims dims, int B, int H, int W, const float* vol, const float* sens)
+bool siddon_sens_brick_route(VolDims dims, int B, int H, int W, const void* vol, const float* sens, int elem_bytes)
 {
     const int64_t n_bricks = (int64_t)((dims.d[0] + 23) / 24) * ((dims.d[1] + 31) / 32) * ((dims.d[2] + 31) / 32);
     const double nvox = (double)dims.d[0] * dims.d[1] * dims.d[2];
     const bool sparse = (double)H * W <= 0.5 * pow(nvox, 2.0 / 3.0);
     return B >= kSensBrickMinBatch && n_bricks >= 2048 && sparse && (int64_t)B * H * W < ((int64_t)1 << 31) &&
-           ((uintptr_t)vol & 15u) == 0 && ((uintptr_t)sens & 15u) == 0 && siddon_brick_supported(dims, H, W);
+           ((uintptr_t)vol & 15u) == 0 && ((uintptr_t)sens & 15u) == 0 && siddon_brick_supported(dims, H, W, elem_bytes);
 }
 
 // Scratch pool of the sensitivities mode, one per device.  Its release threshold is unlimited: memory freed into it stays
@@ -1065,12 +1104,13 @@ static cudaMemPool_t sens_scratch_pool(int dev)
 }
 
 // out [B][H*W] and sens [B][H*W][8] are overwritten (zero-filled by brick_prep_kernel, then summed into by the pairs).
-cudaError_t launch_siddon_fwd_sens_brick(const float* vol, VolDims dims, const float* src, const float* tgt, const float* raylen,
+template <class V>
+cudaError_t launch_siddon_fwd_sens_brick(const V* vol, VolDims dims, const float* src, const float* tgt, const float* raylen,
                                          const float* G, const float* Wd, const float* rows, const float* cols, float* out,
                                          float* sens, int B, int H, int W, float shift, float eps, cudaStream_t stream)
 {
     const int64_t Nr = (int64_t)H * W;
-    if (!siddon_brick_supported(dims, H, W) || ((uintptr_t)vol & 15u) != 0 || ((uintptr_t)sens & 15u) != 0 ||
+    if (!siddon_brick_supported(dims, H, W, (int)sizeof(V)) || ((uintptr_t)vol & 15u) != 0 || ((uintptr_t)sens & 15u) != 0 ||
         (int64_t)B * Nr >= ((int64_t)1 << 31))
         return cudaErrorNotSupported;
     CUtensorMap map;
@@ -1108,11 +1148,19 @@ cudaError_t launch_siddon_fwd_sens_brick(const float* vol, VolDims dims, const f
     }
     if (e == cudaSuccess) {
         const SensArgs sa{src, tgt, raylen, pr, sens, eps};
-        e = launch_brick_variant<24, 32, 32, 1, 512, 4, B200DRR_SENS_U, 2, 0, 1, 0, 1>(map, dims, raytab, ltab, geo, out, counter,
+        e = launch_brick_variant<24, 32, 32, 1, 512, 4, B200DRR_SENS_U, 2, 0, 1, 0, 1, V>(map, dims, raytab, ltab, geo, out, counter,
                                                                                       nullptr, (int)Nr, B, H, W, shift, stream, sa);
     }
     const cudaError_t ef = cudaFreeAsync(ws, stream);
     return e != cudaSuccess ? e : ef;
 }
+#define B200DRR_SENS_BRICK(V)                                                                                                      \
+    template cudaError_t launch_siddon_fwd_sens_brick<V>(const V*, VolDims, const float*, const float*, const float*, const float*, \
+                                                         const float*, const float*, const float*, float*, float*, int, int, int,   \
+                                                         float, float, cudaStream_t);
+B200DRR_SENS_BRICK(float)
+B200DRR_SENS_BRICK(VoxF16)
+B200DRR_SENS_BRICK(VoxBF16)
+#undef B200DRR_SENS_BRICK
 
 }  // namespace b200drr

@@ -7,7 +7,8 @@ namespace b200drr {
 
 constexpr int kThreads = 128;
 
-__global__ void __launch_bounds__(kThreads) trilinear_fwd_kernel(const float* __restrict__ vol, VolDims dims,
+template <class V>
+__global__ void __launch_bounds__(kThreads) trilinear_fwd_kernel(const V* __restrict__ vol, VolDims dims,
                                                                  const float* __restrict__ src,
                                                                  const float* __restrict__ tgt,
                                                                  const float* __restrict__ raylen,
@@ -78,8 +79,8 @@ __global__ void __launch_bounds__(kThreads) trilinear_bwd_kernel(
 // plane-synchronous by construction (every lane is at the same alpha in the same iteration), so the ray bundle of a
 // warp shares sectors among its 8 corner gathers.
 // ---------------------------------------------------------------------------------------------------
-template <int TW, int TH>
-__global__ void __launch_bounds__(TW* TH) trilinear_fwd_grid_kernel(const float* __restrict__ vol, VolDims dims,
+template <int TW, int TH, class V>
+__global__ void __launch_bounds__(TW* TH) trilinear_fwd_grid_kernel(const V* __restrict__ vol, VolDims dims,
                                                                     const float* __restrict__ src,
                                                                     const float* __restrict__ tgt,
                                                                     const float* __restrict__ raylen,
@@ -152,8 +153,8 @@ __global__ void __launch_bounds__(TW* TH) trilinear_bwd_grid_kernel(
 // Forward / backward from the packed-corner copy of the volume (ray_math.cuh: GatherPacked): one aligned 32-byte read
 // per sample instead of 8 scalar gathers.  ncu: the scalar-gather kernel is 99 % L1-bound; this one reaches 65 % of the
 // HBM roofline on BASELINE config 3's shape.
-template <int TW, int TH>
-__global__ void __launch_bounds__(TW* TH) trilinear_fwd_packed_kernel(const float4* __restrict__ packed, VolDims dims,
+template <int TW, int TH, class PK>
+__global__ void __launch_bounds__(TW* TH) trilinear_fwd_packed_kernel(const PK* __restrict__ packed, VolDims dims,
                                                                       const float* __restrict__ src,
                                                                       const float* __restrict__ tgt,
                                                                       const float* __restrict__ raylen,
@@ -226,9 +227,9 @@ __global__ void __launch_bounds__(TW* TH) trilinear_bwd_packed_kernel(
 // voxels along axis 0 (slab * (D1+1)*(D2+1)*32 bytes of the packed copy, sized to sit in L2), so the poses of a batch
 // share the packed cells through L2 instead of each streaming the 8x volume from HBM.  Partial sums are combined
 // with red.global.add (outputs zero-filled by the launcher).
-template <int TW, int TH>
+template <int TW, int TH, class PK>
 __global__ void __launch_bounds__(TW* TH) trilinear_fwd_packed_slab_kernel(
-    const float4* __restrict__ packed, VolDims dims, const float* __restrict__ src, const float* __restrict__ tgt,
+    const PK* __restrict__ packed, VolDims dims, const float* __restrict__ src, const float* __restrict__ tgt,
     const float* __restrict__ raylen, float* __restrict__ out, int B, int H, int W, int slab, float shift, float eps, int P,
     const float* __restrict__ alpha_range)
 {
@@ -327,9 +328,41 @@ cudaError_t launch_pack_corners(const float* vol, VolDims dims, float* packed, c
     return cudaGetLastError();
 }
 
-cudaError_t launch_trilinear_fwd_packed(const float* packed, VolDims dims, const float* src, const float* tgt,
-                                        const float* raylen, float* out, int B, int H, int W, float shift, float eps,
-                                        int n_points, const float* alpha_range, int slab, cudaStream_t stream)
+// 16-bit volumes: the same cells with the corners kept in the volume's own 16-bit type, 16 bytes each (ray_math.cuh: Cell16);
+// the zero padding is +0.0 (all bits clear) in both formats.
+template <class V>
+__global__ void __launch_bounds__(256) pack_corners16_kernel(const V* __restrict__ vol, VolDims dims, uint4* __restrict__ packed)
+{
+    const int64_t n1 = dims.d[1] + 1, n2 = dims.d[2] + 1;
+    const int64_t cells = (int64_t)(dims.d[0] + 1) * n1 * n2;
+    const unsigned short* bits = reinterpret_cast<const unsigned short*>(vol);
+    for (int64_t c = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; c < cells; c += (int64_t)gridDim.x * blockDim.x) {
+        const int i2 = (int)(c % n2) - 1, i1 = (int)((c / n2) % n1) - 1, i0 = (int)(c / (n2 * n1)) - 1;
+        uint32_t h[8];
+#pragma unroll
+        for (int k = 0; k < 8; ++k) {
+            const int x = i0 + (k & 1), y = i1 + ((k >> 1) & 1), z = i2 + ((k >> 2) & 1);
+            const bool inb = (unsigned)x < (unsigned)dims.d[0] && (unsigned)y < (unsigned)dims.d[1] &&
+                             (unsigned)z < (unsigned)dims.d[2];
+            h[k] = inb ? (uint32_t)__ldg(bits + ((int64_t)x * dims.d[1] + y) * dims.d[2] + z) : 0u;
+        }
+        packed[c] = make_uint4(h[0] | (h[1] << 16), h[2] | (h[3] << 16), h[4] | (h[5] << 16), h[6] | (h[7] << 16));
+    }
+}
+
+template <class V>
+cudaError_t launch_pack_corners16(const V* vol, VolDims dims, Cell16<V>* packed, cudaStream_t stream)
+{
+    pack_corners16_kernel<V><<<current_sm_count() * 16, 256, 0, stream>>>(vol, dims, reinterpret_cast<uint4*>(packed));
+    return cudaGetLastError();
+}
+template cudaError_t launch_pack_corners16<VoxF16>(const VoxF16*, VolDims, Cell16<VoxF16>*, cudaStream_t);
+template cudaError_t launch_pack_corners16<VoxBF16>(const VoxBF16*, VolDims, Cell16<VoxBF16>*, cudaStream_t);
+
+template <class PK>
+cudaError_t launch_trilinear_fwd_packed_t(const PK* packed, VolDims dims, const float* src, const float* tgt,
+                                          const float* raylen, float* out, int B, int H, int W, float shift, float eps,
+                                          int n_points, const float* alpha_range, int slab, cudaStream_t stream)
 {
     if (slab > 0) {
         const int n_slabs = (dims.d[0] + 1 + slab - 1) / slab;
@@ -337,14 +370,28 @@ cudaError_t launch_trilinear_fwd_packed(const float* packed, VolDims dims, const
         if (blocks > INT32_MAX) return cudaErrorInvalidValue;
         cudaError_t e = cudaMemsetAsync(out, 0, sizeof(float) * (size_t)B * H * W, stream);
         if (e != cudaSuccess) return e;
-        trilinear_fwd_packed_slab_kernel<16, 16><<<(unsigned)blocks, 256, 0, stream>>>(
-            (const float4*)packed, dims, src, tgt, raylen, out, B, H, W, slab, shift, eps, n_points, alpha_range);
+        trilinear_fwd_packed_slab_kernel<16, 16, PK><<<(unsigned)blocks, 256, 0, stream>>>(
+            packed, dims, src, tgt, raylen, out, B, H, W, slab, shift, eps, n_points, alpha_range);
         return cudaGetLastError();
     }
     const dim3 grid((unsigned)(((W + 15) / 16) * ((H + 15) / 16)), (unsigned)B, 1);
-    trilinear_fwd_packed_kernel<16, 16><<<grid, 256, 0, stream>>>((const float4*)packed, dims, src, tgt, raylen, out, H, W,
-                                                                   shift, eps, n_points, alpha_range);
+    trilinear_fwd_packed_kernel<16, 16, PK><<<grid, 256, 0, stream>>>(packed, dims, src, tgt, raylen, out, H, W, shift, eps,
+                                                                       n_points, alpha_range);
     return cudaGetLastError();
+}
+template cudaError_t launch_trilinear_fwd_packed_t<Cell16<VoxF16>>(const Cell16<VoxF16>*, VolDims, const float*, const float*,
+                                                                   const float*, float*, int, int, int, float, float, int,
+                                                                   const float*, int, cudaStream_t);
+template cudaError_t launch_trilinear_fwd_packed_t<Cell16<VoxBF16>>(const Cell16<VoxBF16>*, VolDims, const float*, const float*,
+                                                                    const float*, float*, int, int, int, float, float, int,
+                                                                    const float*, int, cudaStream_t);
+
+cudaError_t launch_trilinear_fwd_packed(const float* packed, VolDims dims, const float* src, const float* tgt,
+                                        const float* raylen, float* out, int B, int H, int W, float shift, float eps,
+                                        int n_points, const float* alpha_range, int slab, cudaStream_t stream)
+{
+    return launch_trilinear_fwd_packed_t((const float4*)packed, dims, src, tgt, raylen, out, B, H, W, shift, eps, n_points,
+                                         alpha_range, slab, stream);
 }
 
 cudaError_t launch_trilinear_bwd_packed(const float* packed, VolDims dims, const float* src, const float* tgt,
@@ -384,9 +431,9 @@ cudaError_t launch_trilinear_bwd_packed(const float* packed, VolDims dims, const
 //   out[r] = L * step * sum V     and     sens[r] = { dI/dtgt[3], step*sum V | dI/dsrc[3], dI/dalphamin | dI/dalphamax, 0, 0, 0 }
 // and the backward pass is the elementwise trilinear_sens_bwd_kernel.
 // ---------------------------------------------------------------------------------------------------
-template <int TW, int TH, bool SLAB>
+template <int TW, int TH, bool SLAB, class PK>
 __global__ void __launch_bounds__(TW* TH) trilinear_sens_packed_kernel(
-    const float4* __restrict__ packed, VolDims dims, const float* __restrict__ src, const float* __restrict__ tgt,
+    const PK* __restrict__ packed, VolDims dims, const float* __restrict__ src, const float* __restrict__ tgt,
     const float* __restrict__ raylen, float* __restrict__ out, float* __restrict__ sens, int B, int H, int W, int slab,
     float shift, float eps, int P, const float* __restrict__ alpha_range, PoseRays pr)
 {
@@ -428,7 +475,8 @@ __global__ void __launch_bounds__(TW* TH) trilinear_sens_packed_kernel(
 // Forward with sensitivities from the PLAIN volume (8 scalar gathers per sample): arbitrary ray sets (H == 0: ray n of
 // pose b, one thread per ray in row order) or the full detector grid (H > 0: 16x16 pixel tiles, 8x4 ray bundle per warp).
 // Same sens layout as the packed kernel; align_corners supported (arbitrary-ray form only).
-__global__ void __launch_bounds__(256) trilinear_sens_kernel(const float* __restrict__ vol, VolDims dims,
+template <class V>
+__global__ void __launch_bounds__(256) trilinear_sens_kernel(const V* __restrict__ vol, VolDims dims,
                                                              const float* __restrict__ src, const float* __restrict__ tgt,
                                                              const float* __restrict__ raylen, float* __restrict__ out,
                                                              float* __restrict__ sens, int64_t N, int H, int W, float shift,
@@ -462,18 +510,26 @@ __global__ void __launch_bounds__(256) trilinear_sens_kernel(const float* __rest
     out[r] = tg.sumV * (L * step);  // bitwise the forward kernels' expression
 }
 
-cudaError_t launch_trilinear_fwd_sens(const float* vol, VolDims dims, const float* src, const float* tgt, const float* raylen,
+template <class V>
+cudaError_t launch_trilinear_fwd_sens(const V* vol, VolDims dims, const float* src, const float* tgt, const float* raylen,
                                       float* out, float* sens, int B, int64_t N, int H, int W, float shift, float eps,
                                       int n_points, const float* alpha_range, int align_corners, cudaStream_t stream)
 {
     if (H > 0 && ((int64_t)H * W != N || align_corners)) return cudaErrorInvalidValue;
     const int64_t blocks = H > 0 ? (int64_t)((W + 15) / 16) * ((H + 15) / 16) : (N + 255) / 256;
     if (blocks > INT32_MAX || B > 65535) return cudaErrorInvalidValue;
-    trilinear_sens_kernel<<<dim3((unsigned)blocks, (unsigned)B), 256, 0, stream>>>(vol, dims, src, tgt, raylen, out, sens, N, H,
-                                                                                 W, shift, eps, n_points, alpha_range,
-                                                                                 align_corners);
+    trilinear_sens_kernel<V><<<dim3((unsigned)blocks, (unsigned)B), 256, 0, stream>>>(vol, dims, src, tgt, raylen, out, sens, N,
+                                                                                    H, W, shift, eps, n_points, alpha_range,
+                                                                                    align_corners);
     return cudaGetLastError();
 }
+#define B200DRR_TRI_SENS(V)                                                                                                         \
+    template cudaError_t launch_trilinear_fwd_sens<V>(const V*, VolDims, const float*, const float*, const float*, float*, float*, \
+                                                      int, int64_t, int, int, float, float, int, const float*, int, cudaStream_t);
+B200DRR_TRI_SENS(float)
+B200DRR_TRI_SENS(VoxF16)
+B200DRR_TRI_SENS(VoxBF16)
+#undef B200DRR_TRI_SENS
 
 // mask_to_channels backward (autograd of renderers.py:242-252): gout [B][C][N]; sample m carries the gradient of the
 // channel its nearest label routed it to.  g_alpha_range accumulated into (caller zero-fills).
@@ -536,7 +592,8 @@ cudaError_t launch_trilinear_bwd_mask(const float* vol, const float* mask, VolDi
     return cudaGetLastError();
 }
 
-static cudaError_t launch_sens_packed(const float* packed, VolDims dims, const float* src, const float* tgt,
+template <class PK>
+static cudaError_t launch_sens_packed(const PK* packed, VolDims dims, const float* src, const float* tgt,
                                       const float* raylen, float* out, float* sens, int B, int H, int W, float shift,
                                       float eps, int n_points, const float* alpha_range, int slab, cudaStream_t stream,
                                       PoseRays pr)
@@ -550,13 +607,13 @@ static cudaError_t launch_sens_packed(const float* packed, VolDims dims, const f
         cudaError_t e = cudaMemsetAsync(out, 0, sizeof(float) * n, stream);
         if (e == cudaSuccess) e = cudaMemsetAsync(sens, 0, sizeof(float) * 12 * n, stream);
         if (e != cudaSuccess) return e;
-        trilinear_sens_packed_kernel<16, 16, true><<<(unsigned)blocks, 256, 0, stream>>>(
-            (const float4*)packed, dims, src, tgt, raylen, out, sens, B, H, W, slab, shift, eps, n_points, alpha_range, pr);
+        trilinear_sens_packed_kernel<16, 16, true, PK><<<(unsigned)blocks, 256, 0, stream>>>(
+            packed, dims, src, tgt, raylen, out, sens, B, H, W, slab, shift, eps, n_points, alpha_range, pr);
         return cudaGetLastError();
     }
     if (tiles * B > INT32_MAX) return cudaErrorInvalidValue;
-    trilinear_sens_packed_kernel<16, 16, false><<<(unsigned)(tiles * B), 256, 0, stream>>>(
-        (const float4*)packed, dims, src, tgt, raylen, out, sens, B, H, W, 0, shift, eps, n_points, alpha_range, pr);
+    trilinear_sens_packed_kernel<16, 16, false, PK><<<(unsigned)(tiles * B), 256, 0, stream>>>(
+        packed, dims, src, tgt, raylen, out, sens, B, H, W, 0, shift, eps, n_points, alpha_range, pr);
     return cudaGetLastError();
 }
 
@@ -565,9 +622,27 @@ cudaError_t launch_trilinear_fwd_sens_packed(const float* packed, VolDims dims, 
                                              float eps, int n_points, const float* alpha_range, int slab,
                                              cudaStream_t stream)
 {
-    return launch_sens_packed(packed, dims, src, tgt, raylen, out, sens, B, H, W, shift, eps, n_points, alpha_range, slab, stream,
-                              PoseRays{nullptr, nullptr, nullptr, nullptr});
+    return launch_sens_packed((const float4*)packed, dims, src, tgt, raylen, out, sens, B, H, W, shift, eps, n_points, alpha_range,
+                              slab, stream, PoseRays{nullptr, nullptr, nullptr, nullptr});
 }
+
+template <class V>
+cudaError_t launch_trilinear_fwd_sens_packed16(const Cell16<V>* packed, VolDims dims, const float* src, const float* tgt,
+                                               const float* raylen, const float* G, const float* Wd, const float* rows,
+                                               const float* cols, float* out, float* sens, int B, int H, int W, float shift,
+                                               float eps, int n_points, const float* alpha_range, int slab, cudaStream_t stream)
+{
+    return launch_sens_packed(packed, dims, src, tgt, raylen, out, sens, B, H, W, shift, eps, n_points, alpha_range, slab, stream,
+                              PoseRays{G, Wd, rows, cols});
+}
+#define B200DRR_SENS_PACKED16(V)                                                                                                    \
+    template cudaError_t launch_trilinear_fwd_sens_packed16<V>(const Cell16<V>*, VolDims, const float*, const float*,              \
+                                                               const float*, const float*, const float*, const float*,            \
+                                                               const float*, float*, float*, int, int, int, float, float, int,   \
+                                                               const float*, int, cudaStream_t);
+B200DRR_SENS_PACKED16(VoxF16)
+B200DRR_SENS_PACKED16(VoxBF16)
+#undef B200DRR_SENS_PACKED16
 
 // ---- pose-in entry (SURVEY 8f-2 for the trilinear renderer) -----------------------------------------------------------------
 // The batch-global sampling range of renderers.py:217-222 (min over ALL rays of the slab-entry alpha, max of the slab-exit
@@ -653,8 +728,8 @@ cudaError_t launch_trilinear_fwd_sens_pose(const float* packed, VolDims dims, co
                                            float shift, float eps, int n_points, const float* alpha_range, int slab,
                                            cudaStream_t stream)
 {
-    return launch_sens_packed(packed, dims, src, nullptr, nullptr, out, sens, B, H, W, shift, eps, n_points, alpha_range, slab,
-                              stream, PoseRays{G, Wd, rows, cols});
+    return launch_sens_packed((const float4*)packed, dims, src, nullptr, nullptr, out, sens, B, H, W, shift, eps, n_points,
+                              alpha_range, slab, stream, PoseRays{G, Wd, rows, cols});
 }
 
 // gradients of the pose-in form reduced to the per-pose matrices (the trilinear twin of sens_bwd_pose_kernel, siddon.cu):
@@ -785,13 +860,13 @@ cudaError_t launch_trilinear_bwd_sens(const float* sens, const float* gout, floa
     return cudaGetLastError();
 }
 
-template <int TW, int TH>
-static cudaError_t tri_fwd_grid(const float* vol, VolDims dims, const float* src, const float* tgt, const float* raylen,
+template <int TW, int TH, class V>
+static cudaError_t tri_fwd_grid(const V* vol, VolDims dims, const float* src, const float* tgt, const float* raylen,
                                 float* out, int B, int H, int W, float shift, float eps, int P, const float* ar,
                                 cudaStream_t stream)
 {
     const dim3 grid((unsigned)(((W + TW - 1) / TW) * ((H + TH - 1) / TH)), (unsigned)B, 1);
-    trilinear_fwd_grid_kernel<TW, TH><<<grid, TW * TH, 0, stream>>>(vol, dims, src, tgt, raylen, out, H, W, shift, eps, P, ar);
+    trilinear_fwd_grid_kernel<TW, TH, V><<<grid, TW * TH, 0, stream>>>(vol, dims, src, tgt, raylen, out, H, W, shift, eps, P, ar);
     return cudaGetLastError();
 }
 
@@ -810,7 +885,8 @@ static cudaError_t tri_bwd_grid(const float* vol, VolDims dims, const float* src
     return cudaGetLastError();
 }
 
-cudaError_t launch_trilinear_fwd_grid(const float* vol, VolDims dims, const float* src, const float* tgt,
+template <class V>
+cudaError_t launch_trilinear_fwd_grid(const V* vol, VolDims dims, const float* src, const float* tgt,
                                       const float* raylen, float* out, int B, int H, int W, float shift, float eps,
                                       int n_points, const float* alpha_range, int variant, cudaStream_t stream)
 {
@@ -822,6 +898,13 @@ cudaError_t launch_trilinear_fwd_grid(const float* vol, VolDims dims, const floa
         default: return cudaErrorInvalidValue;
     }
 }
+#define B200DRR_TRI_GRID(V)                                                                                                         \
+    template cudaError_t launch_trilinear_fwd_grid<V>(const V*, VolDims, const float*, const float*, const float*, float*, int,    \
+                                                      int, int, float, float, int, const float*, int, cudaStream_t);
+B200DRR_TRI_GRID(float)
+B200DRR_TRI_GRID(VoxF16)
+B200DRR_TRI_GRID(VoxBF16)
+#undef B200DRR_TRI_GRID
 
 cudaError_t launch_trilinear_bwd_grid(const float* vol, VolDims dims, const float* src, const float* tgt,
                                       const float* raylen, const float* gout, float* g_src, float* g_tgt,
@@ -876,15 +959,23 @@ cudaError_t launch_trilinear_fwd_mask(const float* vol, const float* mask, VolDi
 
 static inline dim3 ray_grid(int B, int64_t N) { return dim3((unsigned)((N + kThreads - 1) / kThreads), (unsigned)B, 1); }
 
-cudaError_t launch_trilinear_fwd(const float* vol, VolDims dims, const float* src, const float* tgt,
+template <class V>
+cudaError_t launch_trilinear_fwd(const V* vol, VolDims dims, const float* src, const float* tgt,
                                  const float* raylen, float* out, int B, int64_t N, float shift, float eps,
                                  int n_points, const float* alpha_range, int reduce, int align_corners,
                                  cudaStream_t stream)
 {
-    trilinear_fwd_kernel<<<ray_grid(B, N), kThreads, 0, stream>>>(vol, dims, src, tgt, raylen, out, N, shift, eps,
-                                                                  n_points, alpha_range, reduce, align_corners);
+    trilinear_fwd_kernel<V><<<ray_grid(B, N), kThreads, 0, stream>>>(vol, dims, src, tgt, raylen, out, N, shift, eps,
+                                                                     n_points, alpha_range, reduce, align_corners);
     return cudaGetLastError();
 }
+#define B200DRR_TRI_FWD(V)                                                                                                          \
+    template cudaError_t launch_trilinear_fwd<V>(const V*, VolDims, const float*, const float*, const float*, float*, int, int64_t, \
+                                                 float, float, int, const float*, int, int, cudaStream_t);
+B200DRR_TRI_FWD(float)
+B200DRR_TRI_FWD(VoxF16)
+B200DRR_TRI_FWD(VoxBF16)
+#undef B200DRR_TRI_FWD
 
 cudaError_t launch_trilinear_bwd(const float* vol, VolDims dims, const float* src, const float* tgt,
                                  const float* raylen, const float* gout, float* g_src, float* g_tgt, float* g_raylen,

@@ -107,7 +107,8 @@ class DRR(nn.Module):
 
     @property
     def dtype(self):
-        return self.density.dtype
+        """The dtype poses and rays are built in: the density's, or fp32 for a density stored in 16 bits (DESIGN.md 4.5)."""
+        return torch.float32 if self.density.dtype in (torch.float16, torch.bfloat16) else self.density.dtype
 
     def reshape_transform(self, img, batch_size):
         if not self.reshape:
@@ -161,8 +162,8 @@ class DRR(nn.Module):
                 and not r.filter_intersections_outside_volume and not mask_to_channels
                 and not kwargs.get("align_corners", False) and kwargs.get("mask") is None
                 and self.detector.n_subsample is None and self.patch_size is None
-                and self.density.is_cuda and self.density.dtype == torch.float32 and self.density.dim() == 3
-                and self.density.numel() < 2**31 - 1)
+                and self.density.is_cuda and self.density.dim() == 3 and self.density.numel() < 2**31 - 1
+                and self.density.dtype in (torch.float32, torch.float16, torch.bfloat16))
 
     def _pose_in_trilinear_ok(self, mask_to_channels, kwargs, args) -> bool:
         """True when pose -> rays -> trilinear march can run with in-kernel ray generation: the TRAINING step (pose gradients
@@ -171,7 +172,8 @@ class DRR(nn.Module):
         if not (isinstance(r, Trilinear) and r.mode == "bilinear" and r.reducefn == "sum" and _TRILINEAR_POSE_IN
                 and not mask_to_channels and set(kwargs) <= {"n_points"}
                 and self.detector.n_subsample is None and self.patch_size is None and torch.is_grad_enabled()
-                and self.density.is_cuda and self.density.dtype == torch.float32 and self.density.dim() == 3
+                and self.density.is_cuda and self.density.dim() == 3
+                and self.density.dtype in (torch.float32, torch.float16, torch.bfloat16)
                 and not self.density.requires_grad):
             return False
         wants_grad = any((a.matrix if isinstance(a, RigidTransform) else a).requires_grad
@@ -280,7 +282,7 @@ class DRR(nn.Module):
             pick(sdd, d.sdd), pick(height, d.height), pick(width, d.width), pick(delx, d.delx), pick(dely, d.dely),
             pick(x0, -d.x0), pick(y0, -d.y0),  # the x0/y0 properties are negated (quirk Q9): undo it
             self.subject.reorient, pick(n_subsample, d.n_subsample), pick(reverse_x_axis, d.reverse_x_axis),
-        ).to(self.density)
+        ).to(device=self.density.device, dtype=self.dtype)  # fp32 geometry for a 16-bit density
         # the fused path caches Q = reorient . calibration per detector: a NEW detector must never find the old constants
         # (its buffers can land on the freed addresses of a previous one; ADVICE r1)
         object.__setattr__(self, "_pose_consts", None)

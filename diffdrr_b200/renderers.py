@@ -8,7 +8,8 @@ kernel (no saved activations: `checkpoint_gradients` is a no-op by construction)
 needed the forward kernel also writes each ray's end-point sensitivities (32-48 B per ray) and the backward is elementwise.
 
 There is no CPU / PyTorch fallback: tensors must be CUDA fp32 (tuned kernels) or CUDA fp64 (reference-literal kernels of
-csrc/literal.cu, which also serve a callable `reducefn`), otherwise the call raises.
+csrc/literal.cu, which also serve a callable `reducefn`), otherwise the call raises.  The volume may also be STORED in fp16 or
+bf16 with fp32 rays (DESIGN.md 4.5): the same kernels read it through a widening load; options outside that contract raise.
 """
 from __future__ import annotations
 
@@ -30,12 +31,16 @@ _PACKED_SLAB_SENS = 0   # forward+sensitivities march: unslabbed (its registers 
 _PACKED_SLAB_MIN_BATCH = 8
 
 
-def _check_inputs(volume, source, target, img, dtype=torch.float32):
+# 16-bit volume storage (include/b200drr.h: B200DRR_VOL_F16 / B200DRR_VOL_BF16; DESIGN.md 4.5)
+_VOL16 = {torch.float16: 1, torch.bfloat16: 2}
+
+
+def _check_inputs(volume, source, target, img, dtype=torch.float32, vol16=False):
     for name, t in (("volume", volume), ("source", source), ("target", target), ("img", img)):
         if not t.is_cuda:
             raise _lib.B200DRRError(
                 f"diffdrr_b200 renderers run on CUDA devices only ({name} is on {t.device}); there is no CPU fallback")
-        if t.dtype != dtype:
+        if t.dtype != dtype and not (vol16 and t is volume and t.dtype in _VOL16):
             raise NotImplementedError(
                 f"diffdrr_b200 kernels take fp32 tensors, or fp64 tensors throughout ({name} is {t.dtype}, volume is {volume.dtype})")
     if volume.dim() != 3:
@@ -50,6 +55,30 @@ def _check_inputs(volume, source, target, img, dtype=torch.float32):
 
 def _ptr(t):
     return None if t is None else ctypes.c_void_p(t.data_ptr())
+
+
+def _vol_entry(lib, name, vol, data=None):
+    """(entry point, its leading volume arguments, its name): the fp32 entry point `name`, or for a 16-bit volume its twin
+    `name`_v16, which takes the voxel type after the pointer (include/b200drr.h).  `data` (default: the volume) is the array
+    passed, e.g. the volume's packed-corner copy."""
+    data = vol if data is None else data
+    code = _VOL16.get(vol.dtype)
+    if code is None:
+        return getattr(lib, name), (_ptr(data),), name
+    return getattr(lib, name + "_v16"), (_ptr(data), code), name + "_v16"
+
+
+def _check_vol16(volume, source, target=None):
+    """A 16-bit volume is a STATIC density read by the default-option kernels; refuse the rest before any launch."""
+    if volume.requires_grad:
+        raise NotImplementedError(
+            f"a {volume.dtype} volume cannot require grad: 16-bit volumes are static densities (ray and pose gradients are "
+            "supported; optimise an fp32 volume for volume gradients)")
+    for name, t in (("source", source), ("target", target)):
+        if t is not None and t.dtype != torch.float32:
+            raise NotImplementedError(
+                f"a {volume.dtype} volume is rendered with fp32 rays and poses ({name} is {t.dtype}): convert only the density, "
+                "e.g. drr.density = drr.density.to(torch.bfloat16), not the whole module")
 
 
 def _stream():
@@ -77,7 +106,9 @@ def _brick_ok(vol, B, H, W, check_density: bool = True) -> bool:
     # >= ~1.4 voxels apart): dense rays share 32-byte sectors in L1 and the slab-major gather wins (at 512^3 -> 1024^2;
     # at 512^3 -> 256^2 the other way round)
     sparse = (not check_density) or H * W <= _BRICK_MAX_RAY_DENSITY * float(vol.numel()) ** (2.0 / 3.0)
-    return (B >= _BRICK_MIN_BATCH and n_bricks >= _BRICK_MIN_BRICKS and sparse and vol.shape[2] % 4 == 0 and 2 <= H <= 2048
+    # the TMA map needs 16-byte row strides: D2 % 4 == 0 for fp32 voxels, D2 % 8 == 0 for 16-bit ones
+    aligned = vol.shape[2] % (16 // vol.element_size()) == 0
+    return (B >= _BRICK_MIN_BATCH and n_bricks >= _BRICK_MIN_BRICKS and sparse and aligned and 2 <= H <= 2048
             and 2 <= W <= 2048 and B * H * W < 2**31 and vol.data_ptr() % 16 == 0 and vol.numel() < 2**31 - 1)
 
 
@@ -156,7 +187,7 @@ class _SiddonFunction(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, volume, source, target, img, voxel_shift, eps, reduce, align_corners, stop_grad, grid, subset=None):
-        B, N = _check_inputs(volume, source, target, img)
+        B, N = _check_inputs(volume, source, target, img, vol16=True)
         vol = volume.contiguous()
         src = source.reshape(B, 3).contiguous()
         tgt = target.contiguous()
@@ -172,6 +203,8 @@ class _SiddonFunction(torch.autograd.Function):
         if (_FUSED_SENSITIVITIES and _wants_sens(ctx.needs_input_grad, stop_grad) and reduce == 0 and not align_corners
                 and vol.numel() < 2**31 - 1):
             sens = torch.empty(B, N, 8, dtype=torch.float32, device=vol.device)
+        if vol.dtype in _VOL16 and sens is None and any(ctx.needs_input_grad[1:4]):
+            raise NotImplementedError(f"ray gradients from a {vol.dtype} volume come from the fused sensitivities walk only")
         with torch.cuda.device(vol.device):
             fast = reduce == 0 and not align_corners and vol.numel() < 2**31 - 1
             if (grid is None and fast and sens is None and subset is not None and subset[0].numel() == subset[2] * subset[3]
@@ -181,10 +214,10 @@ class _SiddonFunction(torch.autograd.Function):
                 need = int(lib.b200drr_siddon_brick_workspace_bytes(B, 1, N))
                 ws = _brick_workspace(vol.device, B, 1, N)
                 assert ws.numel() >= need
-                _lib.check(lib.b200drr_siddon_fwd_brick_subset(_ptr(vol), *vol.shape, _ptr(src), _ptr(tgt), _ptr(raylen),
-                                                               ctypes.c_void_p(pix.data_ptr()), _ptr(corners.contiguous().float()),
-                                                               _ptr(out), ctypes.c_void_p(ws.data_ptr()), ws.numel(), B, Hs, Ws, N,
-                                                               voxel_shift, eps, 0, _stream()), "b200drr_siddon_fwd_brick_subset")
+                fn, head, name = _vol_entry(lib, "b200drr_siddon_fwd_brick_subset", vol)
+                _lib.check(fn(*head, *vol.shape, _ptr(src), _ptr(tgt), _ptr(raylen), ctypes.c_void_p(pix.data_ptr()),
+                              _ptr(corners.contiguous().float()), _ptr(out), ctypes.c_void_p(ws.data_ptr()), ws.numel(), B, Hs, Ws,
+                              N, voxel_shift, eps, 0, _stream()), name)
             elif grid is None and fast and N >= _SORT_MIN_RAYS:
                 # arbitrary ray set, big enough to be worth ordering: sort for locality, walk slab-major, un-sort the results
                 perm = _locality_order(tgt)
@@ -193,37 +226,37 @@ class _SiddonFunction(torch.autograd.Function):
                 out_s = torch.empty_like(out)
                 if sens is not None:
                     sens_s = torch.empty_like(sens)
-                    _lib.check(lib.b200drr_siddon_fwd_sens_sorted(_ptr(vol), *vol.shape, _ptr(src), _ptr(tgt_s), _ptr(len_s),
-                                                                  _ptr(out_s), _ptr(sens_s), B, N, voxel_shift, eps, _stream()),
-                               "b200drr_siddon_fwd_sens_sorted")
+                    fn, head, name = _vol_entry(lib, "b200drr_siddon_fwd_sens_sorted", vol)
+                    _lib.check(fn(*head, *vol.shape, _ptr(src), _ptr(tgt_s), _ptr(len_s), _ptr(out_s), _ptr(sens_s), B, N,
+                                  voxel_shift, eps, _stream()), name)
                     sens.scatter_(1, perm.unsqueeze(-1).expand(-1, -1, 8), sens_s)
                 else:
-                    _lib.check(lib.b200drr_siddon_fwd_sorted(_ptr(vol), *vol.shape, _ptr(src), _ptr(tgt_s), _ptr(len_s),
-                                                             _ptr(out_s), B, N, voxel_shift, eps, _stream()),
-                               "b200drr_siddon_fwd_sorted")
+                    fn, head, name = _vol_entry(lib, "b200drr_siddon_fwd_sorted", vol)
+                    _lib.check(fn(*head, *vol.shape, _ptr(src), _ptr(tgt_s), _ptr(len_s), _ptr(out_s), B, N, voxel_shift, eps,
+                                  _stream()), name)
                 out.scatter_(1, perm, out_s)
             elif sens is not None and grid is None:   # small arbitrary ray set (one thread per ray)
-                _lib.check(lib.b200drr_siddon_fwd_sens(_ptr(vol), *vol.shape, _ptr(src), _ptr(tgt), _ptr(raylen), _ptr(out),
-                                                       _ptr(sens), B, N, voxel_shift, eps, _stream()),
-                           "b200drr_siddon_fwd_sens")
+                fn, head, name = _vol_entry(lib, "b200drr_siddon_fwd_sens", vol)
+                _lib.check(fn(*head, *vol.shape, _ptr(src), _ptr(tgt), _ptr(raylen), _ptr(out), _ptr(sens), B, N, voxel_shift,
+                              eps, _stream()), name)
             elif sens is not None:
-                _lib.check(lib.b200drr_siddon_fwd_sens_grid(_ptr(vol), *vol.shape, _ptr(src), _ptr(tgt), _ptr(raylen),
-                                                            _ptr(out), _ptr(sens), B, grid[0], grid[1], voxel_shift, eps, 0,
-                                                            _stream()), "b200drr_siddon_fwd_sens_grid")
+                fn, head, name = _vol_entry(lib, "b200drr_siddon_fwd_sens_grid", vol)
+                _lib.check(fn(*head, *vol.shape, _ptr(src), _ptr(tgt), _ptr(raylen), _ptr(out), _ptr(sens), B, grid[0], grid[1],
+                              voxel_shift, eps, 0, _stream()), name)
             elif grid is not None and _brick_full_grid_ok(vol, B, grid[0], grid[1]):
                 ws = _brick_workspace(vol.device, B, grid[0], grid[1])
-                _lib.check(lib.b200drr_siddon_fwd_brick(_ptr(vol), *vol.shape, _ptr(src), _ptr(tgt), _ptr(raylen), None, None,
-                                                        None, None, _ptr(out), ctypes.c_void_p(ws.data_ptr()), ws.numel(), B,
-                                                        grid[0], grid[1], voxel_shift, eps, 0, _stream()),
-                           "b200drr_siddon_fwd_brick")
+                fn, head, name = _vol_entry(lib, "b200drr_siddon_fwd_brick", vol)
+                _lib.check(fn(*head, *vol.shape, _ptr(src), _ptr(tgt), _ptr(raylen), None, None, None, None, _ptr(out),
+                              ctypes.c_void_p(ws.data_ptr()), ws.numel(), B, grid[0], grid[1], voxel_shift, eps, 0, _stream()),
+                           name)
             elif grid is not None:
-                _lib.check(lib.b200drr_siddon_fwd_grid(_ptr(vol), *vol.shape, _ptr(src), _ptr(tgt), _ptr(raylen), _ptr(out),
-                                                       B, grid[0], grid[1], voxel_shift, eps, 0, _stream()),
-                           "b200drr_siddon_fwd_grid")
+                fn, head, name = _vol_entry(lib, "b200drr_siddon_fwd_grid", vol)
+                _lib.check(fn(*head, *vol.shape, _ptr(src), _ptr(tgt), _ptr(raylen), _ptr(out), B, grid[0], grid[1], voxel_shift,
+                              eps, 0, _stream()), name)
             else:
-                _lib.check(lib.b200drr_siddon_fwd(_ptr(vol), *vol.shape, _ptr(src), _ptr(tgt), _ptr(raylen), _ptr(out), B,
-                                                  N, voxel_shift, eps, reduce, int(align_corners), _stream()),
-                           "b200drr_siddon_fwd")
+                fn, head, name = _vol_entry(lib, "b200drr_siddon_fwd", vol)
+                _lib.check(fn(*head, *vol.shape, _ptr(src), _ptr(tgt), _ptr(raylen), _ptr(out), B, N, voxel_shift, eps, reduce,
+                              int(align_corners), _stream()), name)
         if sens is not None:
             ctx.save_for_backward(sens)
         else:
@@ -348,25 +381,26 @@ class _SiddonPoseFunction(torch.autograd.Function):
         out = torch.empty(B, H * W, dtype=torch.float32, device=vol.device)
         ctx.fused = _FUSED_SENSITIVITIES and _wants_sens(ctx.needs_input_grad, stop_grad)
         ctx.cfg = (voxel_shift, eps, stop_grad)
+        if vol.dtype in _VOL16 and not ctx.fused and any(ctx.needs_input_grad[1:4]):
+            raise NotImplementedError(f"pose gradients from a {vol.dtype} volume come from the fused sensitivities walk only")
+        lib = _lib.load()
         with torch.cuda.device(vol.device):
             if ctx.fused:  # one walk: image + per-ray sensitivities; backward is elementwise
                 sens = torch.empty(B, H * W, 8, dtype=torch.float32, device=vol.device)
-                _lib.check(_lib.load().b200drr_siddon_fwd_sens_pose(_ptr(vol), *vol.shape, _ptr(src), _ptr(G), _ptr(Wd),
-                                                                    _ptr(rows), _ptr(cols), _ptr(out), _ptr(sens), B, H, W,
-                                                                    voxel_shift, eps, _stream()),
-                           "b200drr_siddon_fwd_sens_pose")
+                fn, head, name = _vol_entry(lib, "b200drr_siddon_fwd_sens_pose", vol)
+                _lib.check(fn(*head, *vol.shape, _ptr(src), _ptr(G), _ptr(Wd), _ptr(rows), _ptr(cols), _ptr(out), _ptr(sens), B,
+                              H, W, voxel_shift, eps, _stream()), name)
                 ctx.save_for_backward(sens, Wd, rows, cols)
                 return out.view(B, 1, H * W)
             if _brick_full_grid_ok(vol, B, H, W):
                 ws = _brick_workspace(vol.device, B, H, W)
-                _lib.check(_lib.load().b200drr_siddon_fwd_brick(_ptr(vol), *vol.shape, _ptr(src), None, None, _ptr(G), _ptr(Wd),
-                                                                _ptr(rows), _ptr(cols), _ptr(out),
-                                                                ctypes.c_void_p(ws.data_ptr()), ws.numel(), B, H, W,
-                                                                voxel_shift, eps, 0, _stream()), "b200drr_siddon_fwd_brick")
+                fn, head, name = _vol_entry(lib, "b200drr_siddon_fwd_brick", vol)
+                _lib.check(fn(*head, *vol.shape, _ptr(src), None, None, _ptr(G), _ptr(Wd), _ptr(rows), _ptr(cols), _ptr(out),
+                              ctypes.c_void_p(ws.data_ptr()), ws.numel(), B, H, W, voxel_shift, eps, 0, _stream()), name)
             else:
-                _lib.check(_lib.load().b200drr_siddon_fwd_pose(_ptr(vol), *vol.shape, _ptr(src), _ptr(G), _ptr(Wd), _ptr(rows),
-                                                               _ptr(cols), _ptr(out), B, H, W, voxel_shift, eps, _stream()),
-                           "b200drr_siddon_fwd_pose")
+                fn, head, name = _vol_entry(lib, "b200drr_siddon_fwd_pose", vol)
+                _lib.check(fn(*head, *vol.shape, _ptr(src), _ptr(G), _ptr(Wd), _ptr(rows), _ptr(cols), _ptr(out), B, H, W,
+                              voxel_shift, eps, _stream()), name)
         ctx.save_for_backward(vol, src, G, Wd, rows, cols)
         return out.view(B, 1, H * W)
 
@@ -428,7 +462,7 @@ class _TrilinearFunction(torch.autograd.Function):
     @staticmethod
     def forward(ctx, volume, source, target, img, alpha_range, voxel_shift, eps, n_points, reduce, align_corners, grid,
                 packed):
-        B, N = _check_inputs(volume, source, target, img)
+        B, N = _check_inputs(volume, source, target, img, vol16=True)
         if grid is not None and (grid[0] * grid[1] != N or reduce != 0 or align_corners):
             grid = None
         if grid is None:
@@ -445,32 +479,32 @@ class _TrilinearFunction(torch.autograd.Function):
         sens = None
         if _FUSED_SENSITIVITIES and reduce == 0 and any(ctx.needs_input_grad[1:5]) and not ctx.needs_input_grad[0]:
             sens = torch.empty(B, N, 12, dtype=torch.float32, device=vol.device)
+        if vol.dtype in _VOL16 and sens is None and any(ctx.needs_input_grad[1:5]):
+            raise NotImplementedError(f"ray gradients from a {vol.dtype} volume come from the fused sensitivities march only")
         with torch.cuda.device(vol.device):
             if sens is not None and packed is None:   # plain volume: arbitrary ray sets, or the grid without a packed copy
                 h, w_ = grid if grid is not None else (0, 0)
-                _lib.check(lib.b200drr_trilinear_fwd_sens(_ptr(vol), *vol.shape, _ptr(src), _ptr(tgt), _ptr(raylen), _ptr(out),
-                                                          _ptr(sens), B, N, h, w_, voxel_shift, eps, n_points, _ptr(arange),
-                                                          int(align_corners), _stream()), "b200drr_trilinear_fwd_sens")
+                fn, head, name = _vol_entry(lib, "b200drr_trilinear_fwd_sens", vol)
+                _lib.check(fn(*head, *vol.shape, _ptr(src), _ptr(tgt), _ptr(raylen), _ptr(out), _ptr(sens), B, N, h, w_,
+                              voxel_shift, eps, n_points, _ptr(arange), int(align_corners), _stream()), name)
             elif sens is not None:
-                _lib.check(lib.b200drr_trilinear_fwd_sens_packed(_ptr(packed), *vol.shape, _ptr(src), _ptr(tgt), _ptr(raylen),
-                                                                 _ptr(out), _ptr(sens), B, grid[0], grid[1], voxel_shift, eps,
-                                                                 n_points, _ptr(arange),
-                                                                 _PACKED_SLAB_SENS if B >= _PACKED_SLAB_MIN_BATCH else 0,
-                                                                 _stream()), "b200drr_trilinear_fwd_sens_packed")
+                fn, head, name = _vol_entry(lib, "b200drr_trilinear_fwd_sens_packed", vol, packed)
+                _lib.check(fn(*head, *vol.shape, _ptr(src), _ptr(tgt), _ptr(raylen), _ptr(out), _ptr(sens), B, grid[0], grid[1],
+                              voxel_shift, eps, n_points, _ptr(arange),
+                              _PACKED_SLAB_SENS if B >= _PACKED_SLAB_MIN_BATCH else 0, _stream()), name)
             elif packed is not None:
-                _lib.check(lib.b200drr_trilinear_fwd_packed(_ptr(packed), *vol.shape, _ptr(src), _ptr(tgt), _ptr(raylen),
-                                                            _ptr(out), B, grid[0], grid[1], voxel_shift, eps, n_points,
-                                                            _ptr(arange),
-                                                            _PACKED_SLAB_FWD if B >= _PACKED_SLAB_MIN_BATCH else 0, _stream()),
-                           "b200drr_trilinear_fwd_packed")
+                fn, head, name = _vol_entry(lib, "b200drr_trilinear_fwd_packed", vol, packed)
+                _lib.check(fn(*head, *vol.shape, _ptr(src), _ptr(tgt), _ptr(raylen), _ptr(out), B, grid[0], grid[1], voxel_shift,
+                              eps, n_points, _ptr(arange), _PACKED_SLAB_FWD if B >= _PACKED_SLAB_MIN_BATCH else 0, _stream()),
+                           name)
             elif grid is not None:
-                _lib.check(lib.b200drr_trilinear_fwd_grid(_ptr(vol), *vol.shape, _ptr(src), _ptr(tgt), _ptr(raylen), _ptr(out),
-                                                          B, grid[0], grid[1], voxel_shift, eps, n_points, _ptr(arange), 1,
-                                                          _stream()), "b200drr_trilinear_fwd_grid")
+                fn, head, name = _vol_entry(lib, "b200drr_trilinear_fwd_grid", vol)
+                _lib.check(fn(*head, *vol.shape, _ptr(src), _ptr(tgt), _ptr(raylen), _ptr(out), B, grid[0], grid[1], voxel_shift,
+                              eps, n_points, _ptr(arange), 1, _stream()), name)
             else:
-                _lib.check(lib.b200drr_trilinear_fwd(_ptr(vol), *vol.shape, _ptr(src), _ptr(tgt), _ptr(raylen), _ptr(out), B, N,
-                                                     voxel_shift, eps, n_points, _ptr(arange), reduce, int(align_corners),
-                                                     _stream()), "b200drr_trilinear_fwd")
+                fn, head, name = _vol_entry(lib, "b200drr_trilinear_fwd", vol)
+                _lib.check(fn(*head, *vol.shape, _ptr(src), _ptr(tgt), _ptr(raylen), _ptr(out), B, N, voxel_shift, eps, n_points,
+                              _ptr(arange), reduce, int(align_corners), _stream()), name)
         ctx.fused = sens is not None
         if ctx.fused:
             ctx.save_for_backward(sens)
@@ -541,7 +575,7 @@ class _TrilinearPoseFunction(torch.autograd.Function):
     gradients come back as matrices + the two range partials, no (B,N,3) tensors exist."""
 
     @staticmethod
-    def forward(ctx, packed, dims, src, G, Wd, rows, cols, alpha_range, voxel_shift, eps, n_points):
+    def forward(ctx, packed, dims, src, G, Wd, rows, cols, alpha_range, voxel_shift, eps, n_points, vol_dtype=torch.float32):
         B, H, W = G.shape[0], rows.numel(), cols.numel()
         src, G, Wd = src.contiguous().float(), G.contiguous().float(), Wd.contiguous().float()
         rows, cols = rows.contiguous().float(), cols.contiguous().float()
@@ -549,11 +583,12 @@ class _TrilinearPoseFunction(torch.autograd.Function):
         out = torch.empty(B, H * W, dtype=torch.float32, device=packed.device)
         sens = torch.empty(B, H * W, 12, dtype=torch.float32, device=packed.device)
         with torch.cuda.device(packed.device):
-            _lib.check(_lib.load().b200drr_trilinear_fwd_sens_pose(_ptr(packed), *dims, _ptr(src), _ptr(G), _ptr(Wd), _ptr(rows),
-                                                                   _ptr(cols), _ptr(out), _ptr(sens), B, H, W, voxel_shift, eps,
-                                                                   n_points, _ptr(arange),
-                                                                   _PACKED_SLAB_SENS if B >= _PACKED_SLAB_MIN_BATCH else 0,
-                                                                   _stream()), "b200drr_trilinear_fwd_sens_pose")
+            lib, code = _lib.load(), _VOL16.get(vol_dtype)
+            fn = lib.b200drr_trilinear_fwd_sens_pose if code is None else lib.b200drr_trilinear_fwd_sens_pose_v16
+            head = (_ptr(packed),) if code is None else (_ptr(packed), code)
+            _lib.check(fn(*head, *dims, _ptr(src), _ptr(G), _ptr(Wd), _ptr(rows), _ptr(cols), _ptr(out), _ptr(sens), B, H, W,
+                          voxel_shift, eps, n_points, _ptr(arange), _PACKED_SLAB_SENS if B >= _PACKED_SLAB_MIN_BATCH else 0,
+                          _stream()), fn.__name__)
         ctx.save_for_backward(sens, Wd, rows, cols)
         return out.view(B, 1, H * W)
 
@@ -572,13 +607,15 @@ class _TrilinearPoseFunction(torch.autograd.Function):
             _lib.check(_lib.load().b200drr_trilinear_bwd_sens_pose(_ptr(sens), _ptr(gout), _ptr(Wd), _ptr(rows), _ptr(cols),
                                                                    _ptr(g_src), _ptr(g_G), _ptr(g_Wd), _ptr(g_ar), B, H, W,
                                                                    _stream()), "b200drr_trilinear_bwd_sens_pose")
-        return None, None, g_src, g_G, g_Wd, None, None, g_ar, None, None, None
+        return None, None, g_src, g_G, g_Wd, None, None, g_ar, None, None, None, None
 
 
 def trilinear_pose_render(renderer, volume, packed, src, G, Wd, rows, cols, n_points):
     """Fused pose-in rendering for a `Trilinear` module with default options and a packed static volume (used by DRR.forward
     when pose gradients are wanted); -> (B, 1, H*W).  The batch-global sampling range (reference renderers.py:217-222) is found
     by a reduction kernel over the in-kernel rays, then rebuilt differentiably in torch from the TWO rays that attain it."""
+    if volume.dtype in _VOL16:
+        _check_vol16(volume, src, G)
     B, H, W = G.shape[0], rows.numel(), cols.numel()
     dev = volume.device
     src_c, G_c, Wd_c = src.detach().contiguous().float(), G.detach().contiguous().float(), Wd.detach().contiguous().float()
@@ -601,7 +638,7 @@ def trilinear_pose_render(renderer, volume, packed, src, G, Wd, rows, cols, n_po
     amin, amax = _get_alpha_minmax(src2, tgt2, dims, renderer.voxel_shift, renderer.eps)
     alpha_range = torch.stack([amin[0, 0, 0], amax[1, 0, 0]])
     return _TrilinearPoseFunction.apply(packed, tuple(volume.shape), src, G, Wd, rows, cols, alpha_range,
-                                        float(renderer.voxel_shift), float(renderer.eps), int(n_points))
+                                        float(renderer.voxel_shift), float(renderer.eps), int(n_points), volume.dtype)
 
 
 class _SiddonFunction64(torch.autograd.Function):
@@ -885,6 +922,13 @@ class Siddon(torch.nn.Module):
             # the reference crashes on this flag (renderers.py:118 calls _get_alpha_minmax with too few arguments)
             raise NotImplementedError("filter_intersections_outside_volume=True is broken in the reference and "
                                       "unnecessary here: the fused walk already clips to the volume")
+        if volume.dtype in _VOL16:  # 16-bit volume storage (DESIGN.md 4.5): default options only
+            if (mask is not None or self.mode != "nearest" or not isinstance(self.reducefn, str) or self.reducefn != "sum"
+                    or align_corners):
+                raise NotImplementedError(
+                    f"a {volume.dtype} volume is rendered with the default Siddon options only (mode='nearest', reducefn='sum', "
+                    "align_corners=False, no mask_to_channels); use an fp32 volume for the others")
+            _check_vol16(volume, source, target)
         if _reduce_code(self.reducefn) == 2:  # callable: it receives the (B, N, M-1) segment tensor (renderers.py:175-183)
             if mask is not None or self.mode != "nearest":
                 raise NotImplementedError("a callable reducefn is implemented for mode='nearest' without mask_to_channels")
@@ -915,6 +959,8 @@ class Siddon(torch.nn.Module):
 
 def siddon_pose_render(renderer, volume, src, G, Wd, rows, cols):
     """Fused pose-in rendering for a `Siddon` module with default options (used by DRR.forward); -> (B, 1, H*W)."""
+    if volume.dtype in _VOL16:
+        _check_vol16(volume, src, G)
     return _SiddonPoseFunction.apply(volume, src, G, Wd, rows, cols, float(renderer.voxel_shift), float(renderer.eps),
                                      bool(renderer.stop_gradients_through_grid_sample))
 
@@ -958,27 +1004,29 @@ class Trilinear(torch.nn.Module):
         self._packed, self._packed_key, self._packed_src = None, None, None
 
     def _packed_volume(self, volume):
-        if (not self.pack_corners or volume.requires_grad or not volume.is_cuda or volume.dtype != torch.float32
-                or volume.dim() != 3):
+        if (not self.pack_corners or volume.requires_grad or not volume.is_cuda or volume.dim() != 3
+                or volume.dtype not in (torch.float32, *_VOL16)):
             return None
         lib = _lib.load()
-        n = int(lib.b200drr_packed_volume_floats(*volume.shape))
-        if n * 4 > self.pack_corners_max_bytes:
+        n = int(lib.b200drr_packed_volume_floats(*volume.shape))   # 8 corners per cell, in the volume's own type
+        if n * volume.element_size() > self.pack_corners_max_bytes:
             return None
         # The cache is tied to the tensor OBJECT (weak reference) and its in-place version counter: a temporary volume that
         # the caching allocator re-creates at the same address must not find a stale packed copy (ADVICE r1).  Writes
         # through `.data` bypass the version counter -- call `invalidate_packed()` after those.
-        key = (volume._version, tuple(volume.shape), volume.device)
+        key = (volume._version, tuple(volume.shape), volume.device, volume.dtype)
         src = self._packed_src() if self._packed_src is not None else None
         if self._packed is None or src is not volume or self._packed_key != key:
             vol = volume.contiguous()
             try:
-                packed = torch.empty(n, dtype=torch.float32, device=vol.device)
+                # fp32: 32 B per cell; 16-bit: the corners stay 16-bit, 16 B per cell (include/b200drr.h: _v16 twins)
+                packed = torch.empty(n * volume.element_size() // 4, dtype=torch.float32, device=vol.device)
             except torch.cuda.OutOfMemoryError:
                 self._packed, self._packed_key, self._packed_src = None, None, None
                 return None  # no room for the 8x copy: the gather kernels read the volume as stored
             with torch.cuda.device(vol.device):
-                _lib.check(lib.b200drr_pack_corners(_ptr(vol), *vol.shape, _ptr(packed), _stream()), "b200drr_pack_corners")
+                fn, head, name = _vol_entry(lib, "b200drr_pack_corners", vol)
+                _lib.check(fn(*head, *vol.shape, _ptr(packed), _stream()), name)
             self._packed, self._packed_key, self._packed_src = packed, key, weakref.ref(volume)
         return self._packed
 
@@ -986,6 +1034,12 @@ class Trilinear(torch.nn.Module):
                 alphamax=None):
         if self.mode != "bilinear":
             raise NotImplementedError("Trilinear kernels implement mode='bilinear' (the reference default) only")
+        if volume.dtype in _VOL16:  # 16-bit volume storage (DESIGN.md 4.5): default options only
+            if mask is not None or not isinstance(self.reducefn, str) or self.reducefn != "sum" or align_corners:
+                raise NotImplementedError(
+                    f"a {volume.dtype} volume is rendered with the default Trilinear options only (reducefn='sum', "
+                    "align_corners=False, no mask_to_channels); use an fp32 volume for the others")
+            _check_vol16(volume, source, target)
         if mask is not None and _reduce_code(self.reducefn) != 0:
             raise NotImplementedError("mask_to_channels is implemented for reducefn='sum'")
         if alphamin is None or alphamax is None:

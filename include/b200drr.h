@@ -525,6 +525,79 @@ int b200drr_mi_fwd(const float *x1, const float *x2, int B, int64_t N, const flo
 int b200drr_mi_bwd(const float *x1, const float *x2, const float *bins, const float *sigma, const float *stats, const float *gscore,
                    float *g_x1, float *g_x2, int B, int64_t N, int num_bins, void *stream);
 
+/*
+ * 16-bit volumes (DESIGN.md 4.5): twins of the Siddon forward entry points for a volume stored as IEEE binary16
+ * (vol_type = B200DRR_VOL_F16) or bfloat16 (B200DRR_VOL_BF16).  Only the voxels are 16 bits: every voxel read is widened to
+ * fp32 exactly, and the rays, alphas, lengths, sums, outputs and sensitivities are fp32 as in the fp32 entry points, whose
+ * arguments follow vol_type unchanged.  Each twin runs the kernel the fp32 call selects with variant 0 / default options, on the
+ * widened voxels, so its results equal the fp32 call on the up-cast volume.  The brick kernels need D2 % 8 == 0 (16-byte TMA
+ * strides; D2 % 4 for fp32).  Any other vol_type, a nonzero reduce / align_corners or a null pointer returns B200DRR_EINVAL
+ * without touching CUDA; so does a variant other than 0 (the tuning variants are fp32-only).  The backward of these forwards is
+ * b200drr_siddon_bwd_sens / _bwd_sens_pose (sensitivities only).
+ */
+#define B200DRR_VOL_F16 1
+#define B200DRR_VOL_BF16 2
+int b200drr_siddon_fwd_v16(const void *vol, int vol_type, int D0, int D1, int D2, const float *src, const float *tgt,
+                           const float *raylen, float *out, int B, int64_t N, float voxel_shift, float eps, int reduce,
+                           int align_corners, void *stream);
+int b200drr_siddon_fwd_sens_v16(const void *vol, int vol_type, int D0, int D1, int D2, const float *src, const float *tgt,
+                                const float *raylen, float *out, float *sens, int B, int64_t N, float voxel_shift, float eps,
+                                void *stream);
+int b200drr_siddon_fwd_sorted_v16(const void *vol, int vol_type, int D0, int D1, int D2, const float *src, const float *tgt,
+                                  const float *raylen, float *out, int B, int64_t N, float voxel_shift, float eps, void *stream);
+int b200drr_siddon_fwd_sens_sorted_v16(const void *vol, int vol_type, int D0, int D1, int D2, const float *src, const float *tgt,
+                                       const float *raylen, float *out, float *sens, int B, int64_t N, float voxel_shift, float eps,
+                                       void *stream);
+int b200drr_siddon_fwd_grid_v16(const void *vol, int vol_type, int D0, int D1, int D2, const float *src, const float *tgt,
+                                const float *raylen, float *out, int B, int H, int W, float voxel_shift, float eps, int variant,
+                                void *stream);
+int b200drr_siddon_fwd_sens_grid_v16(const void *vol, int vol_type, int D0, int D1, int D2, const float *src, const float *tgt,
+                                     const float *raylen, float *out, float *sens, int B, int H, int W, float voxel_shift, float eps,
+                                     int variant, void *stream);
+int b200drr_siddon_fwd_brick_v16(const void *vol, int vol_type, int D0, int D1, int D2, const float *src, const float *tgt,
+                                 const float *raylen, const float *G, const float *Wd, const float *rows, const float *cols,
+                                 float *out, void *workspace, int64_t workspace_bytes, int B, int H, int W, float voxel_shift,
+                                 float eps, int variant, void *stream);
+int b200drr_siddon_fwd_brick_subset_v16(const void *vol, int vol_type, int D0, int D1, int D2, const float *src, const float *tgt,
+                                        const float *raylen, const int32_t *pix_index, const float *corners, float *out,
+                                        void *workspace, int64_t workspace_bytes, int B, int H, int W, int64_t Nsub,
+                                        float voxel_shift, float eps, int variant, void *stream);
+int b200drr_siddon_fwd_pose_v16(const void *vol, int vol_type, int D0, int D1, int D2, const float *src, const float *G,
+                                const float *Wd, const float *rows, const float *cols, float *out, int B, int H, int W,
+                                float voxel_shift, float eps, void *stream);
+int b200drr_siddon_fwd_sens_pose_v16(const void *vol, int vol_type, int D0, int D1, int D2, const float *src, const float *G,
+                                     const float *Wd, const float *rows, const float *cols, float *out, float *sens, int B, int H,
+                                     int W, float voxel_shift, float eps, void *stream);
+
+/*
+ * 16-bit volumes, Trilinear (DESIGN.md 4.5): twins of the trilinear entry points with the same fp32 arguments after vol_type.
+ * b200drr_pack_corners_v16 writes the packed-corner copy with the 8 corners of each cell in the volume's own 16-bit type:
+ * b200drr_packed_volume_floats(D0, D1, D2) * 2 bytes (16 B per base voxel, 16-byte aligned); the *_packed_v16 / _sens_pose_v16
+ * twins read that copy (`packed`) and take the volume's vol_type.  reduce and align_corners must be 0; B200DRR_EINVAL otherwise, for
+ * a bad vol_type and for null pointers, without touching CUDA.  fwd_grid_v16 takes the fp32 call's tile variants.
+ */
+int b200drr_pack_corners_v16(const void *vol, int vol_type, int D0, int D1, int D2, void *packed, void *stream);
+int b200drr_trilinear_fwd_v16(const void *vol, int vol_type, int D0, int D1, int D2, const float *src, const float *tgt,
+                              const float *raylen, float *out, int B, int64_t N, float voxel_shift, float eps, int n_points,
+                              const float *alpha_range, int reduce, int align_corners, void *stream);
+int b200drr_trilinear_fwd_grid_v16(const void *vol, int vol_type, int D0, int D1, int D2, const float *src, const float *tgt,
+                                   const float *raylen, float *out, int B, int H, int W, float voxel_shift, float eps, int n_points,
+                                   const float *alpha_range, int variant, void *stream);
+int b200drr_trilinear_fwd_sens_v16(const void *vol, int vol_type, int D0, int D1, int D2, const float *src, const float *tgt,
+                                   const float *raylen, float *out, float *sens, int B, int64_t N, int H, int W, float voxel_shift,
+                                   float eps, int n_points, const float *alpha_range, int align_corners, void *stream);
+int b200drr_trilinear_fwd_packed_v16(const void *packed, int vol_type, int D0, int D1, int D2, const float *src, const float *tgt,
+                                     const float *raylen, float *out, int B, int H, int W, float voxel_shift, float eps, int n_points,
+                                     const float *alpha_range, int slab, void *stream);
+int b200drr_trilinear_fwd_sens_packed_v16(const void *packed, int vol_type, int D0, int D1, int D2, const float *src,
+                                          const float *tgt, const float *raylen, float *out, float *sens, int B, int H, int W,
+                                          float voxel_shift, float eps, int n_points, const float *alpha_range, int slab,
+                                          void *stream);
+int b200drr_trilinear_fwd_sens_pose_v16(const void *packed, int vol_type, int D0, int D1, int D2, const float *src, const float *G,
+                                        const float *Wd, const float *rows, const float *cols, float *out, float *sens, int B, int H,
+                                        int W, float voxel_shift, float eps, int n_points, const float *alpha_range, int slab,
+                                        void *stream);
+
 #ifdef __cplusplus
 }
 #endif

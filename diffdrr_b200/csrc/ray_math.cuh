@@ -540,7 +540,7 @@ B200_HD float siddon_ray_fast_ilp(const float* vol, const VolDims& dims, const R
 //     contribute nothing), which removes the else-chain;
 //   * the final crossing (anext == a_out) is not taken, so `off` never leaves the volume and the U loads of
 //     a group can be issued unconditionally.
-// Needs D0*D1*D2 < 2^31 (32-bit element offsets); the launcher falls back to siddon_ray_fast_ilp otherwise.
+// Needs D0*D1*D2 < 2^31 (32-bit element offsets); siddon_ray_fast_ilp has no such limit.
 // ---------------------------------------------------------------------------------------------------
 B200_HD float min3f(float a, float b, float c)
 {

@@ -1,7 +1,5 @@
 // siddon.cu -- Siddon exact-path DRR kernels for sm_90a (forward, backward, visit counter).
 // One thread walks one ray (ray_math.cuh); blockIdx.y is the pose, blockIdx.x tiles the rays of that pose.
-#include <stdlib.h>
-
 #include "kernels.h"
 #ifdef B200DRR_EXPERIMENTS
 #include "psync.cuh"  // rejected experiments live only in the opt-in experimental build (build.py)
@@ -113,34 +111,11 @@ __global__ void __launch_bounds__(kThreads) siddon_bwd_kernel(const float* __res
 }
 
 // ---------------------------------------------------------------------------------------------------
-// Detector-grid kernel: the rays of a pose are the full H x W detector (n = h*W + w).  A CTA owns a
+// Detector-grid kernels: the rays of a pose are the full H x W detector (n = h*W + w).  A CTA owns a
 // TW x TH pixel tile and every warp an 8 x 4 sub-tile, so the 32 lanes of a warp walk a compact ray
 // bundle (~16 x 8 voxels across) and their gathers share 128-byte lines / 32-byte sectors in L1.
 // U = voxel loads kept in flight per thread.
-// ---------------------------------------------------------------------------------------------------
-template <int TW, int TH, int U, int LEAN>
-__global__ void __launch_bounds__(TW* TH) siddon_fwd_grid_kernel(const float* __restrict__ vol, VolDims dims,
-                                                                 const float* __restrict__ src,
-                                                                 const float* __restrict__ tgt,
-                                                                 const float* __restrict__ raylen,
-                                                                 float* __restrict__ out, int H, int W, float shift,
-                                                                 float eps)
-{
-    constexpr int WX = TW / 8;  // warps per tile row
-    const int tiles_x = (W + TW - 1) / TW;
-    const int tile_x = blockIdx.x % tiles_x, tile_y = blockIdx.x / tiles_x;
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int px = tile_x * TW + (warp % WX) * 8 + (lane & 7);
-    const int py = tile_y * TH + (warp / WX) * 4 + (lane >> 3);
-    if (px >= W || py >= H) return;
-    const int b = blockIdx.y;
-    const int64_t r = ((int64_t)b * H + py) * W + px;
-    const Ray ray = load_ray(src, tgt, b, r, eps);
-    out[r] = __ldg(raylen + r) *
-             (LEAN ? siddon_ray_lean<U>(vol, dims, ray, shift) : siddon_ray_fast_ilp<U>(vol, dims, ray, shift));
-}
-
-// ---------------------------------------------------------------------------------------------------
+//
 // Slab-major detector-grid kernel.  The volume is cut into slabs of `slab` planes along axis 0 (the
 // slowest axis: a slab is one contiguous chunk of memory sized to stay resident in the 50 MB L2).
 // blockIdx.x enumerates (slab, pose, tile) with the slab SLOWEST, so the CTAs in flight at any time --
@@ -451,39 +426,10 @@ cudaError_t launch_siddon_bwd_grid(const float* vol, VolDims dims, const float* 
                                    float* g_vol, int B, int H, int W, float shift, float eps, int stop_grad, int variant,
                                    cudaStream_t stream)
 {
-#define BV(id, TW, TH, U, SLAB, MINB)                                                                                    \
-    case id:                                                                                                             \
-        return launch_bwd_slab_variant<TW, TH, U, MINB>(vol, dims, src, tgt, raylen, gout, g_src, g_tgt, g_raylen, g_vol, B, \
-                                                        H, W, SLAB, shift, eps, stop_grad, stream);
-    switch (variant) {
-        BV(0, 16, 8, 4, 64, 8)
-        BV(10, 16, 16, 4, 32, 1)
-        BV(1, 16, 8, 4, 32, 1)
-        BV(2, 16, 16, 2, 32, 1)
-        BV(3, 16, 16, 4, 64, 1)
-        BV(4, 16, 16, 4, 64, 4)
-        BV(5, 16, 16, 2, 64, 4)
-        BV(6, 16, 8, 4, 64, 8)
-        BV(7, 16, 8, 2, 64, 8)
-        BV(8, 16, 16, 4, 128, 4)
-        BV(9, 16, 8, 4, 64, 6)
-        default: return cudaErrorInvalidValue;
-    }
-#undef BV
-}
-
-template <int TW, int TH, int U, int LEAN>
-static cudaError_t launch_grid_variant(const float* vol, VolDims dims, const float* src, const float* tgt,
-                                       const float* raylen, float* out, int B, int H, int W, float shift, float eps,
-                                       cudaStream_t stream)
-{
-    const dim3 grid((unsigned)(((W + TW - 1) / TW) * ((H + TH - 1) / TH)), (unsigned)B, 1);
-    if (LEAN && (int64_t)dims.d[0] * dims.d[1] * dims.d[2] >= (int64_t)INT32_MAX)  // 32-bit offsets would overflow
-        siddon_fwd_grid_kernel<TW, TH, U, 0><<<grid, TW * TH, 0, stream>>>(vol, dims, src, tgt, raylen, out, H, W, shift, eps);
-    else
-        siddon_fwd_grid_kernel<TW, TH, U, LEAN><<<grid, TW * TH, 0, stream>>>(vol, dims, src, tgt, raylen, out, H, W, shift,
-                                                                              eps);
-    return cudaGetLastError();
+    if (variant != 0) return cudaErrorInvalidValue;
+    // 16 x 8 tiles, 4 loads in flight, 64-plane slabs, at least 8 CTAs per SM (the same kernel as launch_siddon_bwd_pose)
+    return launch_bwd_slab_variant<16, 8, 4, 8>(vol, dims, src, tgt, raylen, gout, g_src, g_tgt, g_raylen, g_vol, B, H, W, 64, shift,
+                                                eps, stop_grad, stream);
 }
 
 // ---------------------------------------------------------------------------------------------------
@@ -746,16 +692,9 @@ cudaError_t launch_x_siddon_sens_chunk(const float* volT, VolDims dims, int axis
 // both) and the sensitivities walk up to 6, both with K = 16; the slab-major kernels keep the bigger batches, with 16-plane slabs.
 // `load` = B * H * W in units of 256^2 rays.  Pieces thinner than ~24 planes only add set-up; volumes below 384^3 were not measured
 // at batch sizes > 4 (the slab-major tuning of BASELINE config 2 stands there), volumes below 96 voxels keep one thread per ray.
-// Returns K, 0 = not used.
-// B200DRR_MAJOR_PIECES / B200DRR_MAJOR_MAXB override it for kernel A/B runs (K for every batch up to MAXB poses).
+// Returns K, 0 = not used.  Kernel A/B runs pick K explicitly with variants 101..164 of the grid entry points.
 int small_batch_pieces(const VolDims& dims, int B, int H, int W, bool sens)
 {
-    static const int env_k = [] { const char* e = getenv("B200DRR_MAJOR_PIECES"); return e ? atoi(e) : -1; }();
-    static const int env_b = [] { const char* e = getenv("B200DRR_MAJOR_MAXB"); return e ? atoi(e) : -1; }();
-    if (env_k >= 0 || env_b >= 0) {
-        if (B > (env_b >= 0 ? env_b : 2)) return 0;
-        if (env_k >= 0) return env_k > 64 ? 64 : env_k;
-    }
     const int dmax = dims.d[0] > dims.d[1] ? (dims.d[0] > dims.d[2] ? dims.d[0] : dims.d[2]) : (dims.d[1] > dims.d[2] ? dims.d[1] : dims.d[2]);
     if (dmax < 96) return 0;  // tiny volumes: a launch is latency-bound whatever the decomposition
     const double load = (double)B * H * W / 65536.0;
@@ -795,10 +734,6 @@ cudaError_t launch_siddon_fwd_sens_grid(const float* vol, VolDims dims, const fl
                                         const float* raylen, float* out, float* sens, int B, int H, int W, float shift,
                                         float eps, int variant, cudaStream_t stream)
 {
-#define SV(id, TW, TH, U, SLAB, MINB)                                                                                   \
-    case id:                                                                                                             \
-        return launch_sens_slab_variant<TW, TH, U, MINB>(vol, dims, src, tgt, raylen, out, sens, B, H, W, SLAB, shift, eps, \
-                                                         stream);
     if (variant == 0) return launch_siddon_fwd_sens_grid_default(vol, dims, src, tgt, raylen, out, sens, B, H, W, shift, eps, stream);
     if (variant == 42)  // brick-major (siddon_brick.cu)
         return launch_siddon_fwd_sens_brick(vol, dims, src, tgt, raylen, nullptr, nullptr, nullptr, nullptr, out, sens, B, H, W, shift,
@@ -806,55 +741,23 @@ cudaError_t launch_siddon_fwd_sens_grid(const float* vol, VolDims dims, const fl
     if (variant > 100 && variant <= 164)  // tuning: 101..164 = that many major-axis pieces, whatever the batch size
         return launch_sens_slab_variant<8, 16, 8, 8, true>(vol, dims, src, tgt, raylen, out, sens, B, H, W, variant - 100, shift, eps,
                                                            stream);
-    if (variant > 300 && variant <= 364)
-        return launch_sens_slab_variant<16, 8, 8, 8, true>(vol, dims, src, tgt, raylen, out, sens, B, H, W, variant - 300, shift, eps,
-                                                           stream);
-    if (variant > 400 && variant <= 464)
-        return launch_sens_slab_variant<8, 16, 4, 8, true>(vol, dims, src, tgt, raylen, out, sens, B, H, W, variant - 400, shift, eps,
-                                                           stream);
     switch (variant) {
-        SV(38, 8, 16, 8, 48, 8)
-        SV(32, 16, 8, 8, 48, 8)
-        SV(33, 8, 16, 8, 128, 8)
-        SV(34, 8, 16, 8, 512, 8)
-        SV(35, 8, 16, 8, 96, 8)
-        SV(36, 8, 16, 8, 256, 8)
-        SV(37, 8, 16, 8, 64, 8)
-        SV(22, 16, 8, 4, 64, 8)
-        SV(1, 16, 8, 4, 32, 8)
-        SV(2, 16, 16, 4, 64, 4)
-        SV(3, 16, 16, 4, 32, 4)
-        SV(4, 16, 8, 2, 64, 8)
-        SV(5, 16, 8, 4, 64, 6)
-        SV(6, 16, 16, 4, 128, 4)
-        SV(7, 16, 8, 4, 128, 8)
-        SV(8, 16, 8, 6, 64, 6)
-        SV(9, 16, 8, 8, 64, 4)
-        SV(10, 8, 8, 4, 64, 16)
-        SV(11, 16, 16, 2, 64, 4)
-        SV(12, 16, 8, 4, 64, 10)
-        SV(13, 16, 8, 8, 32, 4)
-        SV(14, 16, 8, 8, 32, 8)
-        SV(15, 16, 8, 6, 32, 8)
-        SV(16, 16, 8, 8, 16, 8)
-        SV(17, 16, 16, 8, 32, 4)
-        SV(18, 16, 8, 12, 32, 4)
-        SV(20, 16, 16, 8, 32, 3)
-        SV(24, 32, 4, 8, 48, 8)
-        SV(25, 16, 8, 8, 40, 8)
-        SV(26, 16, 8, 8, 56, 8)
-        SV(27, 16, 4, 8, 48, 16)
-        SV(28, 8, 8, 8, 48, 16)
-        SV(29, 16, 8, 6, 48, 8)
-        SV(30, 16, 8, 10, 48, 6)
-        SV(31, 32, 8, 8, 48, 4)
-        SV(21, 8, 8, 8, 32, 16)
-        SV(39, 8, 16, 8, 32, 8)
-        SV(40, 8, 16, 8, 24, 8)
-        SV(41, 8, 16, 8, 16, 8)  // the default kernel by an explicit id, for batches whose default is the major-axis pieces
+// benchmarking: the default's slab-major kernel with a fixed slab height, whatever the batch size
+#define S(id, SLAB)                                                                                                        \
+    case id:                                                                                                               \
+        return launch_sens_slab_variant<8, 16, 8, 8>(vol, dims, src, tgt, raylen, out, sens, B, H, W, SLAB, shift, eps, stream);
+        S(33, 128)
+        S(34, 512)
+        S(35, 96)
+        S(36, 256)
+        S(37, 64)
+        S(38, 48)
+        S(39, 32)
+        S(40, 24)
+        S(41, 16)  // the default kernel by an explicit id, for batches whose default is the major-axis pieces
+#undef S
         default: return cudaErrorInvalidValue;
     }
-#undef SV
 }
 
 template <class V>
@@ -1019,48 +922,16 @@ cudaError_t launch_siddon_fwd_grid(const float* vol, VolDims dims, const float* 
                                    const float* raylen, float* out, int B, int H, int W, float shift, float eps,
                                    int variant, cudaStream_t stream)
 {
-#define V(id, TW, TH, U, LEAN) \
-    case id: return launch_grid_variant<TW, TH, U, LEAN>(vol, dims, src, tgt, raylen, out, B, H, W, shift, eps, stream);
+    if (variant == 0) return launch_siddon_fwd_grid_default(vol, dims, src, tgt, raylen, out, B, H, W, shift, eps, stream);
     if (variant > 100 && variant <= 164)  // tuning: 101..164 = that many major-axis pieces, whatever the batch size
         return launch_slab_variant<16, 16, 4, true>(vol, dims, src, tgt, raylen, out, B, H, W, variant - 100, shift, eps, stream);
-    if (variant > 200 && variant <= 264)
-        return launch_slab_variant<8, 16, 8, true>(vol, dims, src, tgt, raylen, out, B, H, W, variant - 200, shift, eps, stream);
-    if (variant > 300 && variant <= 364)
-        return launch_slab_variant<16, 8, 4, true>(vol, dims, src, tgt, raylen, out, B, H, W, variant - 300, shift, eps, stream);
-    if (variant > 400 && variant <= 464)
-        return launch_slab_variant<8, 16, 4, true>(vol, dims, src, tgt, raylen, out, B, H, W, variant - 400, shift, eps, stream);
-    if (variant == 0) return launch_siddon_fwd_grid_default(vol, dims, src, tgt, raylen, out, B, H, W, shift, eps, stream);
     switch (variant) {
-        V(30, 16, 8, 4, 1)
-        V(1, 16, 8, 8, 0)
-        V(2, 16, 8, 2, 1)
-        V(3, 16, 8, 8, 1)
-        V(4, 16, 16, 4, 1)
-        V(5, 32, 8, 4, 1)
-        V(6, 8, 8, 4, 1)
-        V(7, 8, 16, 4, 1)
-        V(8, 16, 8, 6, 1)
-        V(9, 8, 8, 8, 1)
-#define S(id, TW, TH, U, SLAB) \
-    case id: return launch_slab_variant<TW, TH, U>(vol, dims, src, tgt, raylen, out, B, H, W, SLAB, shift, eps, stream);
-        S(10, 16, 8, 4, 32)
-        S(11, 16, 8, 4, 16)
-        S(12, 16, 8, 4, 64)
-        S(13, 16, 8, 2, 32)
-        S(14, 16, 8, 8, 32)
-        S(15, 16, 16, 4, 32)
-        S(16, 8, 8, 4, 32)
-        S(17, 16, 8, 4, 8)
-        S(18, 16, 8, 4, 128)
-        S(19, 32, 8, 4, 32)
-        S(40, 8, 16, 4, 32)
-        S(41, 8, 16, 8, 32)
-        S(42, 8, 16, 4, 48)
-        S(43, 16, 8, 8, 48)
-        S(44, 16, 16, 8, 32)
-        S(45, 8, 16, 6, 32)
-        S(46, 16, 16, 4, 16)
-        S(47, 16, 16, 4, 24)
+// benchmarking: the default's slab-major kernel with 32- / 16- / 24-plane slabs, whatever the batch size
+#define S(id, SLAB) \
+    case id: return launch_slab_variant<16, 16, 4>(vol, dims, src, tgt, raylen, out, B, H, W, SLAB, shift, eps, stream);
+        S(15, 32)
+        S(46, 16)
+        S(47, 24)
 #undef S
 #ifdef B200DRR_EXPERIMENTS
 #define P(id, TW, TH, U, SLAB, ALIGN) \
@@ -1080,7 +951,6 @@ cudaError_t launch_siddon_fwd_grid(const float* vol, VolDims dims, const float* 
 
         default: return cudaErrorInvalidValue;
     }
-#undef V
 }
 
 // mask_to_channels forward: out [B][C][N], zero-filled by the launcher; one thread per ray owns out[b][:][n].

@@ -950,6 +950,12 @@ cudaError_t launch_siddon_fwd_brick(const V* vol, VolDims dims, const float* src
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return e;
     CUtensorMap map;
+    if (variant == 0) {  // two CTAs per SM, one 96 KB brick each (production shape); 16-bit bricks are staged unswizzled
+        if (!make_volume_map(&map, vol, dims, 24, 32, 32, B200DRR_FWD_SWIZZLE != 0 && sizeof(V) == 4)) return cudaErrorNotSupported;
+        return launch_brick_variant<24, 32, 32, 1, 512, 4, 2, 2, 0, 1, 0, 0, V>(map, dims, raytab, ltab, geo, out, counter, pix_index,
+                                                                                (int)Nr, B, H, W, shift, stream);
+    }
+#ifdef B200DRR_EXPERIMENTS  // tuning variants, all measured and not chosen; fp32 volumes only, not in the shipped library
 #define BV(id, BX, BY, BZ, STAGES, THREADS, K, U, CTAS, PIPE)                                                            \
     case id:                                                                                                             \
         if (!make_volume_map(&map, vol, dims, BX, BY, BZ, B200DRR_FWD_SWIZZLE != 0 && BZ == 32)) return cudaErrorNotSupported;                                 \
@@ -965,22 +971,15 @@ cudaError_t launch_siddon_fwd_brick(const V* vol, VolDims dims, const float* src
         if (!make_volume_map(&map, vol, dims, BX, BY, BZ, B200DRR_FWD_SWIZZLE != 0 && BZ == 32)) return cudaErrorNotSupported;                                 \
         return launch_brick_variant<BX, BY, BZ, STAGES, THREADS, K, U, CTAS, 0, 2, 0, 0, V>(map, dims, raytab, ltab, geo, out, counter, \
                                                                                    pix_index, (int)Nr, B, H, W, shift, stream);
-    if constexpr (sizeof(V) != 4) {  // 16-bit volumes: the production shape only (the tuning variants are fp32-only)
-        if (variant != 0) return cudaErrorInvalidValue;
-        if (!make_volume_map(&map, vol, dims, 24, 32, 32)) return cudaErrorNotSupported;
-        return launch_brick_variant<24, 32, 32, 1, 512, 4, 2, 2, 0, 1, 0, 0, V>(map, dims, raytab, ltab, geo, out, counter, pix_index,
-                                                                                (int)Nr, B, H, W, shift, stream);
-    } else {
+    if constexpr (sizeof(V) == 4) {
     switch (variant) {
-        BV(0, 24, 32, 32, 1, 512, 4, 2, 2, 0)    // two CTAs per SM, one 96 KB brick each (production shape)
-        BV(7, 24, 32, 32, 2, 1024, 4, 2, 1, 1)   // one CTA per SM with a two-stage TMA + mbarrier pipeline (slower: CTA-wide barriers)
-#ifdef B200DRR_EXPERIMENTS   // tuning variants, all measured and not chosen before the port; not in the shipped library
-        BV(1, 24, 32, 32, 1, 512, 4, 2, 2, 1)    // ... with the software-pipelined walk
+        BV(1, 24, 32, 32, 1, 512, 4, 2, 2, 1)    // the production shape with the software-pipelined walk
         BV(2, 24, 32, 32, 1, 512, 4, 4, 2, 1)
         BV(3, 24, 32, 32, 1, 512, 4, 4, 2, 0)
         BV(4, 22, 32, 32, 1, 512, 8, 2, 2, 1)    // bigger rounds (fewer barriers), slightly smaller brick
         BV(5, 15, 32, 32, 1, 320, 4, 2, 3, 1)    // three CTAs per SM
         BV(6, 15, 32, 32, 1, 320, 4, 2, 3, 0)
+        BV(7, 24, 32, 32, 2, 1024, 4, 2, 1, 1)   // one CTA per SM with a two-stage TMA + mbarrier pipeline (slower: CTA-wide barriers)
         BV(8, 24, 32, 32, 2, 1024, 4, 2, 1, 0)
         BV(9, 12, 32, 32, 2, 512, 4, 2, 2, 1)    // two CTAs per SM, each with a two-stage pipeline of 48 KB bricks
         BV(10, 24, 32, 32, 1, 384, 5, 2, 2, 1)
@@ -994,13 +993,14 @@ cudaError_t launch_siddon_fwd_brick(const V* vol, VolDims dims, const float* src
         BV2(24, 24, 32, 32, 1, 512, 4, 2, 2)     // 1.22 ms
         BV3(30, 24, 32, 32, 1, 512, 4, 2, 2)     // warp-specialised: 4 producer warps (test + sort) / 12 consumer warps (walk): 1.25 ms
         BV3(31, 24, 32, 32, 1, 512, 4, 4, 2)
-#endif
-        default: return cudaErrorInvalidValue;
+        default: break;
     }
     }
 #undef BV
 #undef BV2
 #undef BV3
+#endif
+    return cudaErrorInvalidValue;
 }
 template cudaError_t launch_siddon_fwd_brick<float>(const float*, VolDims, const float*, const float*, const float*, const float*,
                                                     const float*, const float*, const float*, float*, void*, size_t, int, int, int,

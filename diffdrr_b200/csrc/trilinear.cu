@@ -75,7 +75,7 @@ __global__ void __launch_bounds__(kThreads) trilinear_bwd_kernel(
 }
 
 // ---------------------------------------------------------------------------------------------------
-// Detector-grid variants: CTA = TW x TH pixel tile, warp = 8 x 4 sub-tile (see siddon.cu).  Fixed-step marching is
+// Detector-grid kernels: CTA = TW x TH pixel tile, warp = 8 x 4 sub-tile (see siddon.cu).  Fixed-step marching is
 // plane-synchronous by construction (every lane is at the same alpha in the same iteration), so the ray bundle of a
 // warp shares sectors among its 8 corner gathers.
 // ---------------------------------------------------------------------------------------------------
@@ -860,43 +860,19 @@ cudaError_t launch_trilinear_bwd_sens(const float* sens, const float* gout, floa
     return cudaGetLastError();
 }
 
-template <int TW, int TH, class V>
-static cudaError_t tri_fwd_grid(const V* vol, VolDims dims, const float* src, const float* tgt, const float* raylen,
-                                float* out, int B, int H, int W, float shift, float eps, int P, const float* ar,
-                                cudaStream_t stream)
-{
-    const dim3 grid((unsigned)(((W + TW - 1) / TW) * ((H + TH - 1) / TH)), (unsigned)B, 1);
-    trilinear_fwd_grid_kernel<TW, TH, V><<<grid, TW * TH, 0, stream>>>(vol, dims, src, tgt, raylen, out, H, W, shift, eps, P, ar);
-    return cudaGetLastError();
-}
-
-template <int TW, int TH>
-static cudaError_t tri_bwd_grid(const float* vol, VolDims dims, const float* src, const float* tgt, const float* raylen,
-                                const float* gout, float* g_src, float* g_tgt, float* g_raylen, float* g_vol, float* g_ar,
-                                int B, int H, int W, float shift, float eps, int P, const float* ar, cudaStream_t stream)
-{
-    if (g_src) {
-        cudaError_t e = cudaMemsetAsync(g_src, 0, sizeof(float) * 3 * (size_t)B, stream);
-        if (e != cudaSuccess) return e;
-    }
-    const dim3 grid((unsigned)(((W + TW - 1) / TW) * ((H + TH - 1) / TH)), (unsigned)B, 1);
-    trilinear_bwd_grid_kernel<TW, TH><<<grid, TW * TH, 0, stream>>>(vol, dims, src, tgt, raylen, gout, g_src, g_tgt, g_raylen,
-                                                                   g_vol, g_ar, H, W, shift, eps, P, ar);
-    return cudaGetLastError();
-}
+// Full-grid trilinear launchers: 16 x 16 pixel tiles, the one tile shape (variant 1) the renderers launch.
+constexpr int kTriTile = 16;
 
 template <class V>
 cudaError_t launch_trilinear_fwd_grid(const V* vol, VolDims dims, const float* src, const float* tgt,
                                       const float* raylen, float* out, int B, int H, int W, float shift, float eps,
                                       int n_points, const float* alpha_range, int variant, cudaStream_t stream)
 {
-    switch (variant) {
-        case 0: return tri_fwd_grid<16, 8>(vol, dims, src, tgt, raylen, out, B, H, W, shift, eps, n_points, alpha_range, stream);
-        case 1: return tri_fwd_grid<16, 16>(vol, dims, src, tgt, raylen, out, B, H, W, shift, eps, n_points, alpha_range, stream);
-        case 2: return tri_fwd_grid<8, 8>(vol, dims, src, tgt, raylen, out, B, H, W, shift, eps, n_points, alpha_range, stream);
-        case 3: return tri_fwd_grid<32, 8>(vol, dims, src, tgt, raylen, out, B, H, W, shift, eps, n_points, alpha_range, stream);
-        default: return cudaErrorInvalidValue;
-    }
+    if (variant != 1) return cudaErrorInvalidValue;
+    const dim3 grid((unsigned)(((W + kTriTile - 1) / kTriTile) * ((H + kTriTile - 1) / kTriTile)), (unsigned)B, 1);
+    trilinear_fwd_grid_kernel<kTriTile, kTriTile, V><<<grid, kTriTile * kTriTile, 0, stream>>>(vol, dims, src, tgt, raylen, out, H, W,
+                                                                                              shift, eps, n_points, alpha_range);
+    return cudaGetLastError();
 }
 #define B200DRR_TRI_GRID(V)                                                                                                         \
     template cudaError_t launch_trilinear_fwd_grid<V>(const V*, VolDims, const float*, const float*, const float*, float*, int,    \
@@ -911,17 +887,15 @@ cudaError_t launch_trilinear_bwd_grid(const float* vol, VolDims dims, const floa
                                       float* g_raylen, float* g_vol, float* g_alpha_range, int B, int H, int W, float shift,
                                       float eps, int n_points, const float* alpha_range, int variant, cudaStream_t stream)
 {
-#define TB(TW, TH) \
-    tri_bwd_grid<TW, TH>(vol, dims, src, tgt, raylen, gout, g_src, g_tgt, g_raylen, g_vol, g_alpha_range, B, H, W, shift, eps, \
-                         n_points, alpha_range, stream)
-    switch (variant) {
-        case 0: return TB(16, 8);
-        case 1: return TB(16, 16);
-        case 2: return TB(8, 8);
-        case 3: return TB(32, 8);
-        default: return cudaErrorInvalidValue;
+    if (variant != 1) return cudaErrorInvalidValue;
+    if (g_src) {
+        cudaError_t e = cudaMemsetAsync(g_src, 0, sizeof(float) * 3 * (size_t)B, stream);
+        if (e != cudaSuccess) return e;
     }
-#undef TB
+    const dim3 grid((unsigned)(((W + kTriTile - 1) / kTriTile) * ((H + kTriTile - 1) / kTriTile)), (unsigned)B, 1);
+    trilinear_bwd_grid_kernel<kTriTile, kTriTile><<<grid, kTriTile * kTriTile, 0, stream>>>(
+        vol, dims, src, tgt, raylen, gout, g_src, g_tgt, g_raylen, g_vol, g_alpha_range, H, W, shift, eps, n_points, alpha_range);
+    return cudaGetLastError();
 }
 
 __global__ void __launch_bounds__(kThreads) trilinear_fwd_mask_kernel(const float* __restrict__ vol,

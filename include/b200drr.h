@@ -56,10 +56,9 @@ int b200drr_siddon_fwd(const float *vol, int D0, int D1, int D2, const float *sr
  * warps/CTAs for cache locality.  Same result as b200drr_siddon_fwd(reduce=0, align_corners=0).
  * variant: 0 = tuned default -- up to 16 poses of 256^2 rays (volumes >= 384 voxels; smaller ones up to 4) every ray is cut into
  * pieces along its own major axis with a thread per (ray, piece), beyond that the volume is cut into 16-plane slabs that the poses
- * of the batch share through L2 (DESIGN.md 4.1 / 4.1c); other values select kernels for benchmarking: 46 / 47 / 15 = the
- * slab-major kernel with 16- / 24- / 32-plane slabs,
- * 100+K / 200+K / 300+K / 400+K (K = 1..64) = K major-axis pieces with 16x16/U4, 8x16/U8, 16x8/U4, 8x16/U4 tiles, further ids =
- * tile-shape / unroll variants (cudaErrorInvalidValue if unknown).
+ * of the batch share through L2 (DESIGN.md 4.1 / 4.1c).  The other ids run the same kernels for benchmarking, whatever the batch
+ * size: 46 / 47 / 15 = the slab-major kernel with 16- / 24- / 32-plane slabs, 100+K (K = 1..64) = K major-axis pieces.  Any other
+ * id returns cudaErrorInvalidValue.
  */
 int b200drr_siddon_fwd_grid(const float *vol, int D0, int D1, int D2, const float *src, const float *tgt,
                             const float *raylen, float *out, int B, int H, int W, float voxel_shift, float eps,
@@ -85,7 +84,7 @@ int b200drr_siddon_bwd(const float *vol, int D0, int D1, int D2, const float *sr
 /*
  * Siddon backward for a FULL detector grid (see b200drr_siddon_fwd_grid): same outputs and conventions as
  * b200drr_siddon_bwd (g_src / g_tgt / g_raylen overwritten, g_vol accumulated into), computed slab-major with
- * red.global.add partial sums.  align_corners=0 only.
+ * red.global.add partial sums.  align_corners=0 only.  variant: 0 (64-plane slabs); any other id returns cudaErrorInvalidValue.
  */
 int b200drr_siddon_bwd_grid(const float *vol, int D0, int D1, int D2, const float *src, const float *tgt,
                             const float *raylen, const float *gout, float *g_src, float *g_tgt, float *g_raylen,
@@ -126,12 +125,12 @@ int b200drr_siddon_bwd_pose(const float *vol, int D0, int D1, int D2, const floa
  * (use b200drr_siddon_bwd_grid when the volume requires grad).  variant 0 = tuned default: the brick-major kernel (id 42) when
  * the shape allows it -- at least 4 poses, >= 2048 bricks of 24x32x32 voxels, sparse rays (H*W <= half the voxels of a volume
  * cross-section), D2 % 4 == 0, H, W in [2, 2048], 16-byte aligned vol and sens -- else major-axis pieces up to 6 poses of
- * 256^2 rays, 16-plane slabs beyond.  b200drr_siddon_fwd_sens_pose follows the same rule.  41 / 40 / 39 / 38 = the 16- / 24- /
- * 32- / 48-plane-slab kernels (41 = the slab-major kernel by an explicit id); 42 = the brick-major kernel (TMA-staged 24x32x32
- * bricks, the slab kernels' sensitivities walk per (ray, brick); ~20 B per ray of scratch from a stream-ordered memory pool of
- * the library that keeps its memory between calls; cudaErrorNotSupported outside the brick kernel's range); 100+K / 300+K /
- * 400+K = K major-axis pieces (8x16/U8, 16x8/U8, 8x16/U4 tiles); further ids = tile / unroll / slab-height variants for
- * benchmarking.
+ * 256^2 rays, 16-plane slabs beyond.  b200drr_siddon_fwd_sens_pose follows the same rule.  The other ids run the same kernels for
+ * benchmarking, whatever the batch size: 41 / 40 / 39 / 38 / 37 / 35 / 33 / 36 / 34 = the slab-major kernel with 16- / 24- / 32- /
+ * 48- / 64- / 96- / 128- / 256- / 512-plane slabs (41 = the default's slab height); 42 = the brick-major kernel (TMA-staged
+ * 24x32x32 bricks, the slab kernels' sensitivities walk per (ray, brick); ~20 B per ray of scratch from a stream-ordered memory
+ * pool of the library that keeps its memory between calls; cudaErrorNotSupported outside the brick kernel's range); 100+K
+ * (K = 1..64) = K major-axis pieces.  Any other id returns cudaErrorInvalidValue.
  */
 int b200drr_siddon_fwd_sens(const float *vol, int D0, int D1, int D2, const float *src, const float *tgt,
                             const float *raylen, float *out, float *sens, int B, int64_t N, float voxel_shift, float eps,
@@ -197,7 +196,8 @@ int b200drr_trilinear_bwd(const float *vol, int D0, int D1, int D2, const float 
 
 /*
  * Trilinear forward / backward for a FULL detector grid (n = h*W + w), reduce="sum", align_corners=0: same results
- * as b200drr_trilinear_fwd / _bwd with pixel tiles mapped onto warps/CTAs for cache locality.
+ * as b200drr_trilinear_fwd / _bwd with pixel tiles mapped onto warps/CTAs for cache locality.  variant: 1 (16x16 pixel tiles);
+ * any other id returns cudaErrorInvalidValue.
  */
 int b200drr_trilinear_fwd_grid(const float *vol, int D0, int D1, int D2, const float *src, const float *tgt,
                                const float *raylen, float *out, int B, int H, int W, float voxel_shift, float eps,
@@ -406,7 +406,7 @@ int b200drr_siddon_fwd_sens_sorted(const float *vol, int D0, int D1, int D2, con
  *   (G, Wd, rows, cols) as in b200drr_siddon_fwd_pose with tgt = raylen = NULL.
  *   workspace: caller-owned scratch of b200drr_siddon_brick_workspace_bytes(B, H, W) bytes, 256-byte aligned (ray table
  *   {1/d, sum|d|, d, L} = 32 B per ray, per-pose detector geometry, the brick work counter); contents are don't-care.
- *   variant: 0 = tuned default.
+ *   variant: 0 (the production brick shape; the brick_subset form below as well); any other id returns cudaErrorInvalidValue.
  */
 int64_t b200drr_siddon_brick_workspace_bytes(int B, int H, int W);
 int b200drr_siddon_fwd_brick(const float *vol, int D0, int D1, int D2, const float *src, const float *tgt,
@@ -574,7 +574,7 @@ int b200drr_siddon_fwd_sens_pose_v16(const void *vol, int vol_type, int D0, int 
  * b200drr_pack_corners_v16 writes the packed-corner copy with the 8 corners of each cell in the volume's own 16-bit type:
  * b200drr_packed_volume_floats(D0, D1, D2) * 2 bytes (16 B per base voxel, 16-byte aligned); the *_packed_v16 / _sens_pose_v16
  * twins read that copy (`packed`) and take the volume's vol_type.  reduce and align_corners must be 0; B200DRR_EINVAL otherwise, for
- * a bad vol_type and for null pointers, without touching CUDA.  fwd_grid_v16 takes the fp32 call's tile variants.
+ * a bad vol_type and for null pointers, without touching CUDA.  fwd_grid_v16 takes the fp32 call's variant (1).
  */
 int b200drr_pack_corners_v16(const void *vol, int vol_type, int D0, int D1, int D2, void *packed, void *stream);
 int b200drr_trilinear_fwd_v16(const void *vol, int vol_type, int D0, int D1, int D2, const float *src, const float *tgt,

@@ -31,7 +31,7 @@ for dims, H, B in (((50, 72, 64), 40, 3), ((30, 40, 36), 24, 35)):
     ref = torch.empty(B, N, device=dev)
     _lib.check(lib.b200drr_siddon_fwd(_ptr(vol), *dims, _ptr(src), _ptr(tgt), _ptr(raylen), _ptr(ref), B, N, 0.5, 1e-8, 0, 0, _stream()), "fwd")
     ws = torch.empty(lib.b200drr_siddon_brick_workspace_bytes(B, H, H), dtype=torch.uint8, device=dev)
-    for v in (0, 7):
+    for v in (0,):
         out = torch.zeros(B, N, device=dev)
         _lib.check(lib.b200drr_siddon_fwd_brick(_ptr(vol), *dims, _ptr(src), _ptr(tgt), _ptr(raylen), None, None, None, None, _ptr(out),
                                                 _ptr(ws), ws.numel(), B, H, H, 0.5, 1e-8, v, _stream()), "brick")

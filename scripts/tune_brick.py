@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Times the brick-major (TMA) Siddon forward variants on the bench workload and checks them against the slab-major kernel.
 
-  BVARIANTS=0,1,...   brick variants (siddon_brick.cu)        B=16  poses       D=512  H=256
+  BVARIANTS=0,1,...   brick variants (siddon_brick.cu; ids other than 0 need B200DRR_BUILD_EXPERIMENTS=1)   B=16  poses   D=512  H=256
   SMALL=1             also run small / odd-shaped correctness cases first
 """
 import os

@@ -1,9 +1,9 @@
 #!/usr/bin/env python
 """Batches of one or two poses (registration loop, single-DRR inference), 512^3 (VOL) -> 256^2 (DET): the Siddon forward and
 forward-with-sensitivities kernels with every ray cut into K pieces along its own major axis (variants 100+K of
-b200drr_siddon_fwd_grid / b200drr_siddon_fwd_sens_grid; 200+K = the forward with the 8x16 tile / 8 loads in flight) against
-the un-cut kernels, parity against each other.  `--loop` runs the registration loop of BASELINE config 5 (bench.py's set-up)
-with the fused NCC kernels and torch's fused Adam, one CUDA graph per step."""
+b200drr_siddon_fwd_grid / b200drr_siddon_fwd_sens_grid) against the un-cut kernels, parity against each other.  `--loop` runs
+the registration loop of BASELINE config 5 (bench.py's set-up) with the fused NCC kernels and torch's fused Adam, one CUDA graph
+per step."""
 import argparse
 import os
 import sys
@@ -50,8 +50,8 @@ def kernels():
             _lib.check(lib.b200drr_siddon_fwd_sens_grid(_ptr(vol), D, D, D, _ptr(s), _ptr(t), _ptr(l), _ptr(o), _ptr(q), B, H, H,
                                                         0.5, 1e-8, variant, _stream()), "fwd_sens_grid")
 
-        fwd(10, ref_out)      # 32-plane slabs, 16x8 tile (the pre-existing default shape for every batch size)
-        t_f0 = float(np.median(bench._time_events(lambda: fwd(10), 7, warmup=2)))
+        fwd(15, ref_out)      # 32-plane slabs
+        t_f0 = float(np.median(bench._time_events(lambda: fwd(15), 7, warmup=2)))
         sns(34, ref_out, ref_sens)   # one thread per ray (a single 512-plane slab): the pre-existing choice for B <= 2
         t_s0 = float(np.median(bench._time_events(lambda: sns(34), 7, warmup=2)))
         t_s48 = float(np.median(bench._time_events(lambda: sns(35), 7, warmup=2)))
@@ -61,16 +61,13 @@ def kernels():
             fwd(100 + K)
             ef = float((out - ref_out).abs().max() / ref_out.abs().max())
             tf = float(np.median(bench._time_events(lambda: fwd(100 + K), 7, warmup=2)))
-            fwd(200 + K)
-            ef2 = float((out - ref_out).abs().max() / ref_out.abs().max())
-            tf2 = float(np.median(bench._time_events(lambda: fwd(200 + K), 7, warmup=2)))
             sns(100 + K)
             es = float((out - ref_out).abs().max() / ref_out.abs().max())
             eq = float((sens - ref_sens).abs().max() / ref_sens.abs().max())
             ts = float(np.median(bench._time_events(lambda: sns(100 + K), 7, warmup=2)))
-            print(f"  K = {K:2d}: forward 16x16/U4 {tf * 1e3:7.1f} us ({4 * visits / tf * 1e-6 / peak * 100:4.1f} %)  8x16/U8 {tf2 * 1e3:7.1f} us | "
+            print(f"  K = {K:2d}: forward {tf * 1e3:7.1f} us ({4 * visits / tf * 1e-6 / peak * 100:4.1f} %) | "
                   f"sens {ts * 1e3:7.1f} us ({4 * visits / ts * 1e-6 / peak * 100:4.1f} % of HBM peak on visited voxels)   "
-                  f"maxdiff/max fwd {ef:.1e} {ef2:.1e} sens-img {es:.1e} sens {eq:.1e}", flush=True)
+                  f"maxdiff/max fwd {ef:.1e} sens-img {es:.1e} sens {eq:.1e}", flush=True)
         fwd(0)
         sns(0)
         t_fd = float(np.median(bench._time_events(lambda: fwd(0), 7, warmup=2)))
@@ -138,8 +135,8 @@ def loop():
             ms = e0.elapsed_time(e1)
             with torch.no_grad():
                 final = float(1.0 - ncc(target, reg()).mean())
-            print(f"registration loop {D}^3 -> {H}^2, fused NCC {fused_ncc}, fused Adam {fused_adam}, pieces "
-                  f"{os.environ.get('B200DRR_MAJOR_PIECES', 'default')}: {n_it / (ms * 1e-3):8.1f} it/s ({ms / n_it * 1e3:6.1f} us/it)  "
+            print(f"registration loop {D}^3 -> {H}^2, fused NCC {fused_ncc}, fused Adam {fused_adam}: "
+                  f"{n_it / (ms * 1e-3):8.1f} it/s ({ms / n_it * 1e3:6.1f} us/it)  "
                   f"1-ncc {final:.2e} rot err {float((reg.rotation.detach() - true_rot).abs().max()):.4f} "
                   f"xyz err {float((reg.translation.detach() - true_xyz).abs().max()):.3f}", flush=True)
 
@@ -176,23 +173,18 @@ def big():
 
         fwd(15, ref_out)
         pct = lambda tt: 4 * visits / tt * 1e-6 / peak * 100  # noqa: E731
-        t_slab, t_brick, t_sens = ms(lambda: fwd(15)), ms(brick), ms(lambda: sns(32 if False else 0))
+        t_slab, t_brick, t_sens = ms(lambda: fwd(15)), ms(brick), ms(lambda: sns(0))
         print(f"{D}^3 -> {H}^2 x {B} poses ({visits / (B * N):.0f} visits/ray): forward slab-major {t_slab * 1e3:7.1f} us ({pct(t_slab):4.1f} %) | "
-              f"brick {t_brick * 1e3:7.1f} us ({pct(t_brick):4.1f} %) | sens 48-plane slabs {t_sens * 1e3:7.1f} us ({pct(t_sens):4.1f} %)", flush=True)
+              f"brick {t_brick * 1e3:7.1f} us ({pct(t_brick):4.1f} %) | sens default {t_sens * 1e3:7.1f} us ({pct(t_sens):4.1f} %)", flush=True)
         for K in [int(k) for k in args.pieces.split(",")]:
-            row = f"  K = {K:2d}: forward"
-            for base, name in ((100, "16x16/U4"), (200, "8x16/U8"), (300, "16x8/U4"), (400, "8x16/U4")):
-                fwd(base + K)
-                e = float((out - ref_out).abs().max() / ref_out.abs().max())
-                tt = ms(lambda: fwd(base + K))
-                row += f" {name} {tt * 1e3:7.1f} ({pct(tt):4.1f} %, {e:.0e})"
-            row += " | sens"
-            for base, name in ((100, "8x16/U8"), (300, "16x8/U8"), (400, "8x16/U4")):
-                sns(base + K)
-                e = float((out - ref_out).abs().max() / ref_out.abs().max())
-                tt = ms(lambda: sns(base + K))
-                row += f" {name} {tt * 1e3:7.1f} ({pct(tt):4.1f} %, {e:.0e})"
-            print(row, flush=True)
+            fwd(100 + K)
+            e = float((out - ref_out).abs().max() / ref_out.abs().max())
+            tf = ms(lambda: fwd(100 + K))
+            sns(100 + K)
+            es = float((out - ref_out).abs().max() / ref_out.abs().max())
+            ts = ms(lambda: sns(100 + K))
+            print(f"  K = {K:2d}: forward {tf * 1e3:7.1f} ({pct(tf):4.1f} %, {e:.0e}) | sens {ts * 1e3:7.1f} ({pct(ts):4.1f} %, {es:.0e})",
+                  flush=True)
 
 
 if args.loop:

@@ -1,5 +1,10 @@
 #!/usr/bin/env python
-"""Times the trilinear kernels on BASELINE config 3's shape (512^3 -> 512^2, n_points=500) at a reduced batch."""
+"""Times the trilinear kernels on BASELINE config 3's shape (512^3 -> 512^2, n_points=500) at a reduced batch.
+
+  VARIANTS=-1,1,10,...   -1 = one thread per ray (b200drr_trilinear_fwd / _bwd), 1 = the full-grid kernels
+                         (b200drr_trilinear_fwd_grid / _bwd_grid, 16x16 tiles), 10 + S = the packed-corner kernels with
+                         S-plane slabs (0 = whole rays)
+"""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch

@@ -636,13 +636,82 @@ struct BrickLoad {
 };
 
 // A, C accumulated INTO (see siddon_ray_sens_box_m); returns sum v * dalpha over the brick's voxels [lo_v, hi_v).
+// The framed pair starts from the ray's volume frame f (volume_frame), its source s and direction d: what siddon_ray_sens_box
+// does for the ray, without re-deriving the frame.
+template <int U, class Ld>
+B200_HD float brick_pair_sens_framed(const Ld& ld, const VolFrame& f, const float s[3], const float d[3], const VolDims& dims,
+                                     const int lo_v[3], const int hi_v[3], const int org[3], int st0, int st1, int st2, float shift,
+                                     float A[3], float C[3])
+{
+    const int s0 = st0 * Ld::kScale, s1 = st1 * Ld::kScale, s2 = st2 * Ld::kScale;
+    const BrickLoad<Ld> load{ld, ld.base() - (org[0] * s0 + org[1] * s1 + org[2] * s2)};
+    const Walk w = start_walk_in_frame<true>(f, s, d, dims, lo_v, hi_v, shift);
+    const float* vol = nullptr;
+    const float m0 = fabsf(d[0]), m1 = fabsf(d[1]), m2 = fabsf(d[2]);
+    if (m0 >= m1 && m0 >= m2) return siddon_ray_sens_walk_m<U, 0>(vol, w, s0, s1, s2, A, C, load);
+    if (m1 >= m2) return siddon_ray_sens_walk_m<U, 1>(vol, w, s0, s1, s2, A, C, load);
+    return siddon_ray_sens_walk_m<U, 2>(vol, w, s0, s1, s2, A, C, load);
+}
+
 template <int U, class Ld>
 B200_HD float brick_pair_sens(const Ld& ld, const Ray& ray, const VolDims& dims, const int lo_v[3], const int hi_v[3],
                               const int org[3], int st0, int st1, int st2, float shift, float A[3], float C[3])
 {
-    const int s0 = st0 * Ld::kScale, s1 = st1 * Ld::kScale, s2 = st2 * Ld::kScale;
-    const BrickLoad<Ld> load{ld, ld.base() - (org[0] * s0 + org[1] * s1 + org[2] * s2)};
-    return siddon_ray_sens_box<U, BrickLoad<Ld>, true>(static_cast<const float*>(nullptr), dims, lo_v, hi_v, s0, s1, s2, ray, shift, A, C, load);
+    return brick_pair_sens_framed<U>(ld, volume_frame(ray, dims, shift), ray.s, ray.d, dims, lo_v, hi_v, org, st0, st1, st2, shift, A,
+                                     C);
+}
+
+// ---- per-ray frame record of the sensitivities mode ----------------------------------------------------------------------------
+// A ray is cut into ~20-30 (ray, brick) pairs, and every part of a pair's set-up that depends on the ray alone -- rebuilding the
+// ray, its volume frame, its length L -- is the same for all of them.  brick_prep_kernel builds it once per launch into this record,
+// so a pair only clips the frame to its brick (start_walk_in_frame).  The stored values are the ones the pair would compute, so
+// every brick of a ray still sees bit-identical alphas.  32 bytes, one L2 sector: 1/d comes from the ray table, s from the pose,
+// and the frame's entry voxel index i_a (pref_a = i_a + 1 when d_a > 0, else i_a) takes 10 bits per axis -- which limits the
+// volume's sides to kSensFrameMaxSide voxels (larger volumes take the slab kernels, siddon_sens_brick_route).
+//   f0 = (a0[0], a0[1], a0[2], L),   f1 = (d[0], d[1], d[2], bits of i_0 | i_1 << 10 | i_2 << 20 | hit << 30)
+struct SensFrameRec {
+    float4 f0, f1;
+};
+constexpr int kSensFrameMaxSide = 1024;
+
+B200_HD SensFrameRec pack_sens_frame(const VolFrame& f, const float d[3], float L)
+{
+    uint32_t bits = f.hit ? 1u << 30 : 0u;
+#pragma unroll
+    for (int a = 0; a < 3; ++a) bits |= (uint32_t)((int)f.pref[a] - (f.sti[a] > 0 ? 1 : 0)) << (10 * a);
+    SensFrameRec r;
+    r.f0.x = f.a0[0];
+    r.f0.y = f.a0[1];
+    r.f0.z = f.a0[2];
+    r.f0.w = L;
+    r.f1.x = d[0];
+    r.f1.y = d[1];
+    r.f1.z = d[2];
+    r.f1.w = f32_from_bits(bits);
+    return r;
+}
+
+// inv = the ray's 1/d (ray table); d and L are read back from the record
+B200_HD VolFrame unpack_sens_frame(const SensFrameRec& r, const float inv[3], float d[3], float& L)
+{
+    VolFrame f;
+    const uint32_t bits = f32_bits(r.f1.w);
+    const float a0[3] = {r.f0.x, r.f0.y, r.f0.z};
+    d[0] = r.f1.x;
+    d[1] = r.f1.y;
+    d[2] = r.f1.z;
+#pragma unroll
+    for (int a = 0; a < 3; ++a) {
+        f.inv[a] = inv[a];
+        f.da[a] = fabsf(inv[a]);
+        f.sti[a] = d[a] > 0.0f ? 1 : -1;
+        f.a0[a] = a0[a];
+        const int i = (int)((bits >> (10 * a)) & 1023u);
+        f.pref[a] = (float)(f.sti[a] > 0 ? i + 1 : i);
+    }
+    f.hit = ((bits >> 30) & 1u) != 0u;
+    L = r.f0.w;
+    return f;
 }
 
 // Sort key of the sensitivities mode: the walk branches three ways on the ray's major axis M, and a warp's 32 items mix poses,

@@ -61,6 +61,17 @@ B200_HD float f32_from_bits(uint32_t u)
 #endif
 }
 
+B200_HD uint32_t f32_bits(float f)
+{
+#if defined(__CUDA_ARCH__)
+    return __float_as_uint(f);
+#else
+    uint32_t u;
+    __builtin_memcpy(&u, &f, 4);
+    return u;
+#endif
+}
+
 // The one 16-bit -> fp32 conversion (exact: both formats are subsets of fp32).  bf16 is the top half of an fp32; binary16 is
 // decoded by hand on the host (subnormals, infinities and NaN payloads as numpy's float16 -> float32) and by cvt on the device.
 B200_HD float vox16_to_f32(uint16_t h, bool bf16)

@@ -137,6 +137,7 @@ cudaError_t launch_siddon_fwd_sens_sorted(const V* vol, VolDims dims, const floa
 
 // brick-major Siddon forward (siddon_brick.cu): TMA-staged voxel bricks in shared memory; G == nullptr -> rays from tgt/raylen
 size_t siddon_brick_workspace_bytes(int B, int H, int W);
+size_t siddon_sens_brick_scratch_bytes(int B, int H, int W);  // the sensitivities mode's own scratch (+ per-ray frame records)
 bool siddon_brick_supported(VolDims dims, int H, int W, int elem_bytes = 4);  // 16-byte global strides for the TMA map
 template <class V>
 cudaError_t launch_siddon_fwd_brick(const V* vol, VolDims dims, const float* src, const float* tgt, const float* raylen,

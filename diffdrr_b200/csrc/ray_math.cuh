@@ -320,29 +320,38 @@ B200_HD Walk start_walk_box(const Ray& ray, const int lo_v[3], const int hi_v[3]
 // sum of the coefficients still telescopes, their attribution does not -- found as 3-13 rays per 10^6 that run through a voxel
 // edge exactly on a cut, 4e-3 of the largest gradient).  Slabs along axis 0 have no lower axis, so CUT = false is exact for them
 // (and keeps the production slab kernels' code unchanged).
-template <bool CUT = false>
-B200_HD Walk start_walk_frame(const Ray& ray, const VolDims& dims, const int lo_v[3], const int hi_v[3], float shift)
+//
+// start_walk_frame = volume_frame (depends on the ray alone) + start_walk_in_frame (the box): a kernel that cuts one ray into many
+// boxes may build the frame once and keep it (the brick kernel's sensitivities mode, SensFrameRec in brick.cuh).
+struct VolFrame {
+    float inv[3];   // 1/d
+    float da[3];    // |1/d|
+    int sti[3];     // +1 / -1
+    float a0[3];    // alpha of the frame's first plane per axis, plane_alpha_acc(pref)
+    float pref[3];  // index of that plane: the first one crossed after the entry into the volume
+    bool hit;       // the line crosses the volume (av_in < av_out; false for NaN as well)
+};
+
+B200_HD VolFrame volume_frame(const Ray& ray, const VolDims& dims, float shift)
 {
-    Walk w;
-    // ---- frame: entry into the whole volume ----------------------------------------------------------------
+    VolFrame f;
     float vlo[3];
     float av_in = -INFINITY, av_out = INFINITY;
 #pragma unroll
     for (int a = 0; a < 3; ++a) {
-        w.inv[a] = ray.inv[a];
-        w.da[a] = fabsf(ray.inv[a]);
-        w.sti[a] = ray.d[a] > 0.0f ? 1 : -1;
+        f.inv[a] = ray.inv[a];
+        f.da[a] = fabsf(ray.inv[a]);
+        f.sti[a] = ray.d[a] > 0.0f ? 1 : -1;
         const float a0 = plane_alpha_acc(ray, a, 0.0f, shift), a1 = plane_alpha_acc(ray, a, (float)dims.d[a], shift);
         vlo[a] = fminf(a0, a1);
         av_in = fmaxf(av_in, vlo[a]);
         av_out = fminf(av_out, fmaxf(a0, a1));
     }
-    float pref[3];
 #pragma unroll
     for (int a = 0; a < 3; ++a) {
         // straight-line (select-only) version of: floor the entry position, then move one voxel back/forward if the
         // plane behind is not strictly before av_in / the plane ahead is already before it
-        const bool fwd = w.sti[a] > 0;
+        const bool fwd = f.sti[a] > 0;
         const int hi_i = dims.d[a] - 1;
         int i = (int)floorf(fmaf(av_in, ray.d[a], ray.s[a] + shift));
         i = i < 0 ? 0 : (i > hi_i ? hi_i : i);
@@ -350,10 +359,28 @@ B200_HD Walk start_walk_frame(const Ray& ray, const VolDims& dims, const int lo_
         const float a_ahead = plane_alpha_acc(ray, a, (float)(fwd ? i + 1 : i), shift);
         const bool back = (a_behind >= av_in) && (fwd ? i > 0 : i < hi_i);
         const bool ahead = !(a_behind >= av_in) && (a_ahead < av_in) && (fwd ? i < hi_i : i > 0);
-        i += back ? -w.sti[a] : (ahead ? w.sti[a] : 0);
+        i += back ? -f.sti[a] : (ahead ? f.sti[a] : 0);
         i = (vlo[a] >= av_in) ? (fwd ? 0 : hi_i) : i;  // entering through a face of this axis
-        pref[a] = (float)(fwd ? i + 1 : i);
-        w.a0[a] = plane_alpha_acc(ray, a, pref[a], shift);
+        f.pref[a] = (float)(fwd ? i + 1 : i);
+        f.a0[a] = plane_alpha_acc(ray, a, f.pref[a], shift);
+    }
+    f.hit = av_in < av_out;
+    return f;
+}
+
+// The box part: clip to [lo_v, hi_v) with frame alphas, the CUT rules, the start voxel.  s and d are the ray's (for the floor).
+template <bool CUT = false>
+B200_HD Walk start_walk_in_frame(const VolFrame& f, const float s[3], const float d[3], const VolDims& dims, const int lo_v[3],
+                                 const int hi_v[3], float shift)
+{
+    Walk w;
+    const float* pref = f.pref;
+#pragma unroll
+    for (int a = 0; a < 3; ++a) {
+        w.inv[a] = f.inv[a];
+        w.da[a] = f.da[a];
+        w.sti[a] = f.sti[a];
+        w.a0[a] = f.a0[a];
     }
     // ---- clip to the box with frame alphas -----------------------------------------------------------------
     float lo[3];
@@ -372,7 +399,7 @@ B200_HD Walk start_walk_frame(const Ray& ray, const VolDims& dims, const int lo_
         w.a_out = fminf(w.a_out, fmaxf(a0, a1));
     }
     // a_in == a_out is a (zero-length) hit here: the voxel touched still takes part in the crossing bookkeeping
-    w.hit = (av_in < av_out) && (w.a_in <= w.a_out);
+    w.hit = f.hit && (w.a_in <= w.a_out);
     // CUT: the un-cut walk processes the events of one alpha in this order -- entry into the volume, then the crossings lowest
     // axis first, the exit at its axis' turn (tied crossings on higher axes are dropped) -- and a cut on axis M is the M-crossing
     // of that list: everything before it belongs to the box that is left, everything after it to the box that is entered.  So
@@ -406,7 +433,7 @@ B200_HD Walk start_walk_frame(const Ray& ray, const VolDims& dims, const int lo_
         const bool fwd = w.sti[a] > 0;
         const float sg = (float)w.sti[a];
         const int lo_i = lo_v[a], hi_i = hi_v[a] - 1;
-        int i = (int)floorf(fmaf(w.a_in, ray.d[a], ray.s[a] + shift));
+        int i = (int)floorf(fmaf(w.a_in, d[a], s[a] + shift));
         i = i < lo_i ? lo_i : (i > hi_i ? hi_i : i);
         const float a_behind = fmaf(((float)(fwd ? i : i + 1) - pref[a]) * sg, w.da[a], w.a0[a]);
         const float a_ahead = fmaf(((float)(fwd ? i + 1 : i) - pref[a]) * sg, w.da[a], w.a0[a]);
@@ -431,6 +458,12 @@ B200_HD Walk start_walk_frame(const Ray& ray, const VolDims& dims, const int lo_
         w.an[a] = fmaf(w.nf[a], w.da[a], w.a0[a]);
     }
     return w;
+}
+
+template <bool CUT = false>
+B200_HD Walk start_walk_frame(const Ray& ray, const VolDims& dims, const int lo_v[3], const int hi_v[3], float shift)
+{
+    return start_walk_in_frame<CUT>(volume_frame(ray, dims, shift), ray.s, ray.d, dims, lo_v, hi_v, shift);
 }
 
 B200_HD Walk start_walk(const Ray& ray, const VolDims& dims, float shift)
@@ -1009,12 +1042,12 @@ struct LoadChunk {
 // The sensitivities walk of one ray restricted to a box, for a ray whose major axis is M: same walk, tie order and
 // tail as siddon_ray_bwd_lean_box, two accumulated axes + the telescoping identities.  A, C accumulated INTO.
 // `loader` fetches the voxels (a loader with state, e.g. the brick kernel's shared-memory copy, is handed in).
-template <int U, int M, class Load = LoadPlain, bool CUT = false, class V = float>
-B200_HD float siddon_ray_sens_box_m(const V* vol, const VolDims& dims, const int lo_v[3], const int hi_v[3], int st0,
-                                    int st1, int st2, const Ray& ray, float shift, float A[3], float C[3], Load loader = Load())
+// siddon_ray_sens_walk_m takes the walk's start (start_walk_frame<CUT>) ready made.
+template <int U, int M, class Load = LoadPlain, class V = float>
+B200_HD float siddon_ray_sens_walk_m(const V* vol, const Walk& w, int st0, int st1, int st2, float A[3], float C[3],
+                                     Load loader = Load())
 {
     using Ax = MinorAxes<M>;
-    const Walk w = start_walk_frame<CUT>(ray, dims, lo_v, hi_v, shift);
     if (!w.hit) return 0.0f;
     LeanConst k;
     LeanState s;
@@ -1080,6 +1113,13 @@ B200_HD float siddon_ray_sens_box_m(const V* vol, const VolDims& dims, const int
     C[Ax::V] += Cv;
     C[M] -= Cu + Cv;        // sum_a C_a = 0 over the box
     return acc;
+}
+
+template <int U, int M, class Load = LoadPlain, bool CUT = false, class V = float>
+B200_HD float siddon_ray_sens_box_m(const V* vol, const VolDims& dims, const int lo_v[3], const int hi_v[3], int st0,
+                                    int st1, int st2, const Ray& ray, float shift, float A[3], float C[3], Load loader = Load())
+{
+    return siddon_ray_sens_walk_m<U, M>(vol, start_walk_frame<CUT>(ray, dims, lo_v, hi_v, shift), st0, st1, st2, A, C, loader);
 }
 
 // Dispatch on the ray's major axis (uniform per warp except for rays near a 45-degree direction).

@@ -13,7 +13,8 @@
 // The (B, N) ray table {1/d, sum|d|} (+ the ray lengths L) is written once per launch by brick_prep_kernel, which also zero-fills
 // the output and derives the per-pose detector geometry used in step 1.
 // Two more modes of the same kernel: BWD (volume gradient, the staged brick is an accumulator) and SENS (training step: each pair
-// runs the exact-frame sensitivities walk of the slab kernels and adds the ray's image and end-point derivatives).
+// runs the exact-frame sensitivities walk of the slab kernels, from a per-ray frame record the prep kernel writes, and adds the
+// ray's image and end-point derivatives).
 //
 // Replaces reference renderers.py:94-113 (alphas + sort) and 156-169 (grid_sample gather) for full detector grids.
 #include <cuda.h>  // CUtensorMap + enums only; the encoder is fetched through cudaGetDriverEntryPoint (no -lcuda)
@@ -160,15 +161,11 @@ __device__ __forceinline__ Ray make_ray_b(const PoseRaysB& pr, const float* __re
     return ray;
 }
 
-// Sensitivities mode (SENS = 1): what a pair needs to rebuild its ray exactly as siddon_sens_slab_kernel does (make_ray_b: the
-// ray table only serves the hit test) and where it adds its share: sens [B][Nr][8], as b200drr_siddon_fwd_sens_grid lays it out.
+// Sensitivities mode (SENS = 1): the per-ray frame records brick_prep_kernel wrote ([B][Nr], SensFrameRec) and where a pair adds
+// its share: sens [B][Nr][8], as b200drr_siddon_fwd_sens_grid lays it out.
 struct SensArgs {
-    const float* src;
-    const float* tgt;
-    const float* raylen;
-    PoseRaysB pr;
+    const SensFrameRec* frames;
     float* sens;
-    float eps;
 };
 
 // ---- ray table + per-pose geometry + zero fill ----------------------------------------------------------------------
@@ -180,7 +177,9 @@ __global__ void __launch_bounds__(256) brick_prep_kernel(const float* __restrict
                                                          int64_t Nr /* rays per pose */,
                                                          const float* __restrict__ corners /* [B][3][3] or nullptr */,
                                                          const float* __restrict__ gout /* volume-gradient mode, else nullptr */,
-                                                         float* __restrict__ sens = nullptr /* sensitivities mode: zero-filled */)
+                                                         float* __restrict__ sens = nullptr /* sensitivities mode: zero-filled */,
+                                                         SensFrameRec* __restrict__ frames = nullptr /* sensitivities mode */,
+                                                         VolDims dims = VolDims{}, float shift = 0.0f)
 {
     const int64_t n = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     const int b = blockIdx.y;
@@ -197,6 +196,7 @@ __global__ void __launch_bounds__(256) brick_prep_kernel(const float* __restrict
         float4* s4 = reinterpret_cast<float4*>(sens) + 2 * r;
         s4[0] = s4[1] = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
     }
+    if (frames) frames[r] = pack_sens_frame(volume_frame(ray, dims, shift), ray.d, L);
     if (n == 0) {
         float t00[3], t0w[3], th0[3];
         if (corners) {  // targets of the full grid's pixels (0, 0), (0, W-1), (H-1, 0), handed in by the caller
@@ -257,8 +257,9 @@ struct BrickCfg {
 // BWD = 1: volume-gradient mode.  `tmap` then describes g_vol, the staged brick starts as zeros instead of a TMA load, every
 // pair's walk scatters (gout * L) * chord length into it (brick_pair_bwd_lean; ltab holds gout * L), and the finished brick is
 // written with ONE TMA store -- every voxel belongs to exactly one brick, so there is no global atomic and g_vol is overwritten.
-// SENS = 1: training-step mode (full detector grids).  Every pair rebuilds its ray, runs the exact-frame sensitivities walk over
-// the staged brick (brick_pair_sens) and flushes like siddon_sens_slab_kernel: two red.global.add.v4 into sa.sens (dI/dt, S,
+// SENS = 1: training-step mode (full detector grids).  Every pair reads its ray's frame record (SensFrameRec) and 1/d, runs the
+// exact-frame sensitivities walk over the staged brick (brick_pair_sens_framed) and flushes like siddon_sens_slab_kernel: two
+// red.global.add.v4 into sa.sens (dI/dt, S,
 // dI/ds) and L * S into out, nothing for an all-zero pair.  The work list is sorted by major axis first (sens_bin).
 template <int BX, int BY, int BZ, int STAGES, int THREADS, int K, int U, int CTAS, int PIPE, int RAYS, int BWD = 0, int SENS = 0,
           class V = float>
@@ -751,7 +752,7 @@ __global__ void __launch_bounds__(THREADS, CTAS)
                     itw = 0xffffffffu;
                     if (c < n_chunks && i < n_items) {
                         itw = s_items[i];
-                        if constexpr (SENS == 0) {  // the sensitivities walk rebuilds its ray instead
+                        if constexpr (SENS == 0) {  // the sensitivities pair loads its ray table entry with its frame record
                             const unsigned r = (unsigned)(p0 + item_pose(itw)) * (unsigned)Nr + (unsigned)item_ray(itw);
                             q = __ldg(raytab + r);
                             L = __ldg(ltab + r);
@@ -781,18 +782,20 @@ __global__ void __launch_bounds__(THREADS, CTAS)
                                 brick_pair_bwd_lean<U>(StShared{ld.base_addr}, L, s3, inv3, clo3, chi3, lo_v, hi_v, org, BY * BZ, BZ, 1,
                                                        shift);
                         } else if constexpr (SENS != 0) {
-                            const int b = p0 + bl, n = item_ray(itw);
-                            const int64_t r = (int64_t)b * Nr + n;
-                            const int py = n / W, px = n - py * W;
-                            float Lr;
-                            const Ray ray = make_ray_b(sa.pr, sa.src, sa.tgt, sa.raylen, b, r, px, py, sa.eps, Lr);
+                            const size_t r = (size_t)(p0 + bl) * (size_t)Nr + (size_t)item_ray(itw);
+                            const float4* fr = reinterpret_cast<const float4*>(sa.frames + r);
+                            const SensFrameRec rec{__ldg(fr), __ldg(fr + 1)};
+                            const float4 qi = __ldg(raytab + r);
+                            const float inv[3] = {qi.x, qi.y, qi.z};
+                            float d[3], Lr;
+                            const VolFrame f = unpack_sens_frame(rec, inv, d, Lr);
                             float A[3] = {0.0f, 0.0f, 0.0f}, C[3] = {0.0f, 0.0f, 0.0f};
-                            const float S = brick_pair_sens<U>(ld, ray, dims, lo_v, hi_v, org, BY * BZ, BZ, 1, shift, A, C);
+                            const float S = brick_pair_sens_framed<U>(ld, f, s3, d, dims, lo_v, hi_v, org, BY * BZ, BZ, 1, shift, A, C);
                             float jt[3], js[3];
                             bool any = S != 0.0f;
 #pragma unroll
                             for (int a = 0; a < 3; ++a) {
-                                const float k = Lr * ray.inv[a];
+                                const float k = Lr * inv[a];
                                 jt[a] = -k * A[a];
                                 js[a] = k * (A[a] - C[a]);
                                 any = any || jt[a] != 0.0f || js[a] != 0.0f;
@@ -915,6 +918,12 @@ cudaError_t launch_brick_variant(const CUtensorMap& map, VolDims dims, const flo
 size_t siddon_brick_workspace_bytes(int B, int H, int W)
 {
     return 256 + align_up(sizeof(PoseGeo) * (size_t)B, 256) + (sizeof(float4) + sizeof(float)) * (size_t)B * H * W;
+}
+
+// The sensitivities mode's scratch: the forward workspace, then one SensFrameRec per ray (32-byte aligned: one L2 sector each).
+size_t siddon_sens_brick_scratch_bytes(int B, int H, int W)
+{
+    return align_up(siddon_brick_workspace_bytes(B, H, W), 256) + sizeof(SensFrameRec) * (size_t)B * H * W;
 }
 
 bool siddon_brick_supported(VolDims dims, int H, int W, int elem_bytes)
@@ -1055,24 +1064,30 @@ cudaError_t launch_siddon_bwd_vol_brick(const float* gout, VolDims dims, const f
 
 // ---- training step: image + per-ray sensitivities through the SENS mode ---------------------------------------------------------
 #ifndef B200DRR_SENS_U
-#define B200DRR_SENS_U 8  // walk steps per group: fits the 64 registers of 2 CTAs x 512 threads without spills (U = 4 spills 8 B)
+// Walk steps per group.  Each walk pads its last group to U steps, so a smaller U wastes fewer steps per pair (a pair walks ~30
+// voxels) and a larger one keeps more shared-memory loads in flight.  H100 80GB HBM3, 700 W, bench.py, sensitivities launch at 16
+// poses: U = 4 2.037 ms, 5 2.023, 6 2.000, 7 2.034, 8 2.044.  All fit the 64 registers of 2 CTAs x 512 threads without spills.
+#define B200DRR_SENS_U 6
 #endif
-// Batches of at least this many poses take the brick path.  H100 SXM, 700 W, 512^3 -> 256^2 (scripts/sens_brick_sweep.py --block 20,
-// median us per launch, brick / best of the others): 2 poses 384 / 391 (pieces), 4: 583 / 627, 8: 1098 / 1266, 16: 2115 / 2394,
-// 32: 4144 / 4487 (slab-major) -- from 4 poses on the brick kernel wins by 7-15 %; at 2 the margin is inside the noise.
+// Batches of at least this many poses take the brick path.  H100 80GB HBM3, 700 W, 512^3 -> 256^2 (scripts/sens_brick_sweep.py
+// --block 20, median us per launch, brick / best of the others), with the per-ray frame record: 2 poses 373 / 391 (pieces),
+// 4: 565 / 628, 8: 1061 / 1268, 16: 2041 / 2396, 32: 4003 / 4491 (slab-major) -- from 4 poses on the brick kernel wins by 11-17 %;
+// the 5 % at 2 poses is one sweep (2 % before the record, inside the noise), not yet enough to move the threshold.
 constexpr int kSensBrickMinBatch = 4;
 
 // The one routing rule of the training step (b200drr_siddon_fwd_sens_grid variant 0 and b200drr_siddon_fwd_sens_pose): the brick
 // kernel can take the shape (siddon_brick_supported, 16-byte aligned volume and sensitivities), the volume has enough bricks for
 // the dynamic queue of 2 x 132 resident CTAs to balance (>= 2048 bricks of 24 x 32 x 32), the rays are sparse (detector pixels at
 // most half the voxels of a volume cross-section, as the module's forward routing requires: dense rays share L1 sectors and the
-// slab-major gather wins) and the batch is big enough for the staged bricks to be shared.
+// slab-major gather wins), the batch is big enough for the staged bricks to be shared and no side of the volume is longer than the
+// per-ray frame record can index (kSensFrameMaxSide).
 bool siddon_sens_brick_route(VolDims dims, int B, int H, int W, const void* vol, const float* sens, int elem_bytes)
 {
     const int64_t n_bricks = (int64_t)((dims.d[0] + 23) / 24) * ((dims.d[1] + 31) / 32) * ((dims.d[2] + 31) / 32);
     const double nvox = (double)dims.d[0] * dims.d[1] * dims.d[2];
     const bool sparse = (double)H * W <= 0.5 * pow(nvox, 2.0 / 3.0);
-    return B >= kSensBrickMinBatch && n_bricks >= 2048 && sparse && (int64_t)B * H * W < ((int64_t)1 << 31) &&
+    const bool indexable = dims.d[0] <= kSensFrameMaxSide && dims.d[1] <= kSensFrameMaxSide && dims.d[2] <= kSensFrameMaxSide;
+    return B >= kSensBrickMinBatch && n_bricks >= 2048 && sparse && indexable && (int64_t)B * H * W < ((int64_t)1 << 31) &&
            ((uintptr_t)vol & 15u) == 0 && ((uintptr_t)sens & 15u) == 0 && siddon_brick_supported(dims, H, W, elem_bytes);
 }
 
@@ -1111,14 +1126,16 @@ cudaError_t launch_siddon_fwd_sens_brick(const V* vol, VolDims dims, const float
 {
     const int64_t Nr = (int64_t)H * W;
     if (!siddon_brick_supported(dims, H, W, (int)sizeof(V)) || ((uintptr_t)vol & 15u) != 0 || ((uintptr_t)sens & 15u) != 0 ||
-        (int64_t)B * Nr >= ((int64_t)1 << 31))
+        (int64_t)B * Nr >= ((int64_t)1 << 31) || dims.d[0] > kSensFrameMaxSide || dims.d[1] > kSensFrameMaxSide ||
+        dims.d[2] > kSensFrameMaxSide)
         return cudaErrorNotSupported;
     CUtensorMap map;
     if (!make_volume_map(&map, vol, dims, 24, 32, 32, B200DRR_FWD_SWIZZLE != 0)) return cudaErrorNotSupported;
-    // Scratch (claim counter, per-pose geometry, ray table: ~21 MB at 16 poses of 256^2) from the stream-ordered allocator: no
-    // workspace argument, nothing shared across streams, no device-wide sync.  Eager calls take it from sens_scratch_pool; inside
-    // CUDA-graph capture the allocation becomes a pair of allocation / free nodes whose memory the graph itself keeps.
-    const size_t bytes = siddon_brick_workspace_bytes(B, H, W);
+    // Scratch (claim counter, per-pose geometry, ray table, frame records: ~55 MB at 16 poses of 256^2) from the stream-ordered
+    // allocator: no workspace argument, nothing shared across streams, no device-wide sync.  Eager calls take it from
+    // sens_scratch_pool; inside CUDA-graph capture the allocation becomes a pair of allocation / free nodes whose memory the graph
+    // itself keeps.
+    const size_t bytes = siddon_sens_brick_scratch_bytes(B, H, W);
     cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
     cudaError_t e = cudaStreamIsCapturing(stream, &cap);
     if (e != cudaSuccess) return e;
@@ -1139,15 +1156,16 @@ cudaError_t launch_siddon_fwd_sens_brick(const V* vol, VolDims dims, const float
     PoseGeo* geo = reinterpret_cast<PoseGeo*>(w8 + 256);
     float4* raytab = reinterpret_cast<float4*>(w8 + 256 + align_up(sizeof(PoseGeo) * (size_t)B, 256));
     float* ltab = reinterpret_cast<float*>(raytab + (size_t)B * Nr);
+    SensFrameRec* frames = reinterpret_cast<SensFrameRec*>(w8 + align_up(siddon_brick_workspace_bytes(B, H, W), 256));
     const PoseRaysB pr{G, Wd, rows, cols};
-    if (((uintptr_t)ws & 15u) != 0) e = cudaErrorInvalidValue;
+    if (((uintptr_t)ws & 255u) != 0) e = cudaErrorInvalidValue;
     if (e == cudaSuccess) {
         brick_prep_kernel<<<dim3((unsigned)((Nr + 255) / 256), (unsigned)B), 256, 0, stream>>>(
-            src, tgt, raylen, pr, raytab, ltab, geo, out, counter, H, W, eps, Nr, nullptr, nullptr, sens);
+            src, tgt, raylen, pr, raytab, ltab, geo, out, counter, H, W, eps, Nr, nullptr, nullptr, sens, frames, dims, shift);
         e = cudaGetLastError();
     }
     if (e == cudaSuccess) {
-        const SensArgs sa{src, tgt, raylen, pr, sens, eps};
+        const SensArgs sa{frames, sens};
         e = launch_brick_variant<24, 32, 32, 1, 512, 4, B200DRR_SENS_U, 2, 0, 1, 0, 1, V>(map, dims, raytab, ltab, geo, out, counter,
                                                                                       nullptr, (int)Nr, B, H, W, shift, stream, sa);
     }

@@ -1360,14 +1360,20 @@ B200_HD void sample_range(const PixLine& pl, const VolDims& dims, float amin, fl
 // Narrow [m_lo, m_hi] to the samples whose BASE voxel along axis 0 (floor(pix0)) can lie in [s_lo, s_hi): the
 // slab-major trilinear kernels cut the volume into such slabs; the loop re-checks every sample exactly, so each
 // sample is counted by exactly one slab.  One sample of slack on both sides.
+// The loop tests the ROUNDED pix0 = fmaf(alpha, dp0, p0).  A line that runs within round-off of a slab face (|dp0| so
+// small that a whole march moves pix0 by less than an ulp) can have every sample on the other side of the face than the
+// exact line, so the cut is widened by a bound on that round-off (pix0's rounding and the face's alpha):
+// the candidates are then a superset of the samples the loop accepts.
 B200_HD void sample_range_slab(const PixLine& pl, float amin, float range, int P, float s_lo, float s_hi, int& m_lo,
                                int& m_hi)
 {
-    if (!(range > 0.0f) || m_lo > m_hi) return;
+    // dp0 == 0: pix0 == p0 at every sample, the loop's test alone decides (the face alphas would be 0 * inf = NaN)
+    if (!(range > 0.0f) || m_lo > m_hi || pl.dp[0] == 0.0f) return;
+    const float tol = 2e-6f * (fabsf(pl.p0[0]) + fabsf(s_lo) + fabsf(s_hi) + 1.0f);
     const float inv = 1.0f / pl.dp[0];
-    const float a0 = (s_lo - pl.p0[0]) * inv, a1 = (s_hi - pl.p0[0]) * inv;
+    const float a0 = ((s_lo - tol) - pl.p0[0]) * inv, a1 = ((s_hi + tol) - pl.p0[0]) * inv;
     const float lo = fminf(a0, a1), hi = fmaxf(a0, a1);
-    if (!(lo <= hi)) return;  // dp0 == 0 (NaN): the ray runs inside one slab, keep the whole range
+    if (!(lo <= hi)) return;
     const float scale = (float)(P - 1) / range;
     const float f_lo = floorf((lo - amin) * scale) - 1.0f, f_hi = ceilf((hi - amin) * scale) + 1.0f;
     const int n_lo = (int)fmaxf(0.0f, fminf(f_lo, (float)P)), n_hi = (int)fminf((float)(P - 1), fmaxf(f_hi, -1.0f));

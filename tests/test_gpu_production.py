@@ -17,13 +17,14 @@ pytestmark = pytest.mark.gpu
 IMG_TOL = 1e-4  # north_star: <= 1e-4 relative error
 
 
-def _setup(D, H, B, seed=0, kind="rand"):
+def _setup(D, H, B, seed=0, kind="rand", W=None):
+    """Volume D (int or 3-tuple) and the rays of B rotated poses on an H x W (default H x H) detector, in voxel space."""
     from diffdrr_b200 import DRR, synthetic
     from diffdrr_b200.pose import convert
     vol_np = synthetic.make_volume(D, kind, seed=seed)
     subj = synthetic.make_subject(torch.zeros(1, 1, 1, 1))
     subj.volume.affine = synthetic.make_affine(D)
-    drr = DRR(subj, **synthetic.detector_kwargs(H)).to(DEV)
+    drr = DRR(subj, **synthetic.detector_kwargs(H, W)).to(DEV)
     rot, xyz = synthetic.make_poses(max(B, 2), seed=seed)
     rot, xyz = rot[:B], xyz[:B]
     with torch.no_grad():

@@ -240,7 +240,8 @@ def test_trilinear_packed_corner_path():
         drr.density.mul_(2.0)  # in-place update bumps the tensor version -> the packed copy is rebuilt
         after = drr(rot0.to(DEV), xyz0.to(DEV), parameterization="euler_angles", convention="ZXY", n_points=180)
     assert relerr(after.cpu().numpy(), 2.0 * before.cpu().numpy()) < 1e-6
-    # reconstruction mode: the volume is a parameter -> gather path, volume gradient present
+    # reconstruction mode: the volume is a parameter -> gather path, volume gradient present (its VALUES are pinned to the fp64
+    # oracle by tests/test_gpu_trilinear_oracle.py::test_every_launch_vs_oracle, bwd_grid / bwd with g_vol)
     from diffdrr_b200.pose import convert
     dens = drr.density.clone().requires_grad_(True)
     src, tgt = drr.detector(convert(rot0.to(DEV), xyz0.to(DEV), parameterization="euler_angles", convention="ZXY"), None)

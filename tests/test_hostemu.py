@@ -255,7 +255,37 @@ def test_trilinear_packed_slab_cut_counts_every_sample_once(slab):
     assert abs(gb["g_alphamin"] - ga["g_alphamin"]) < 1e-4 * abs(ga["g_alphamin"])
 
 
-@pytest.mark.parametrize("seed,shape", [(0, (40, 56, 48)), (1, (7, 5, 9)), (2, (64, 64, 64)), (3, (1, 1, 1)), (4, (2, 33, 3)),
+@pytest.mark.parametrize("eps", [1e-8, 0.0])
+def test_trilinear_packed_slab_cut_keeps_rays_that_run_along_a_slab_face(eps):
+    """Rays at pix0 = 15 (the face between the first two 16-plane slabs) whose axis-0 direction is 0 or one ulp of 15 either
+    way: the rounded pix0 of every sample sits on the face although the exact line is just off it.  The cut used to drop
+    ~90 % of such a ray (the exact line put its samples in slab 0, the loop's test on the rounded pix0 in slab 1) and, with
+    eps = 0, the whole ray (0 * inf = NaN face alphas)."""
+    vol = synthetic_volume((40, 30, 20))
+    x0 = np.float32(15.0)
+    src = np.array([[[x0, -50.0, 10.3]]], np.float32)
+    tgt = np.array([[[t0, 90.0, z] for t0 in (x0, np.nextafter(x0, np.float32(0)), np.nextafter(x0, np.float32(99)))
+                     for z in (3.0, 10.3, 17.0)]], np.float32)
+    raylen = np.linalg.norm(tgt - src, axis=-1).reshape(1, 1, -1).astype(np.float32)
+    w = np.linspace(0.5, 1.5, 9, dtype=np.float32).reshape(1, 1, 9)
+    ref = oracle.trilinear_fwd(vol, src, tgt, raylen, n_points=77, alphamin=0.3, alphamax=0.6, eps=eps, dtype=np.float64)
+    a, ga = emu.trilinear_packed(vol, src, tgt, raylen, w, 77, 0.3, 0.6, eps=eps)
+    assert relerr(a, ref) < IMG_TOL
+    for slab in (16, 8, 5):
+        b, gb = emu.trilinear_packed(vol, src, tgt, raylen, w, 77, 0.3, 0.6, eps=eps, slab=slab)
+        assert relerr(b, a) < 2e-6, slab
+        for key in ("g_target", "g_source", "g_raylen"):
+            assert relerr(gb[key], ga[key]) < 2e-5, (slab, key)
+
+
+def synthetic_volume(shape):
+    import sys
+    sys.path.insert(0, ROOT)
+    from diffdrr_b200 import synthetic
+    return synthetic.make_volume(shape, "smooth", seed=1)
+
+
+@pytest.mark.parametrize("seed,shape",[(0, (40, 56, 48)), (1, (7, 5, 9)), (2, (64, 64, 64)), (3, (1, 1, 1)), (4, (2, 33, 3)),
                                         (5, (33, 2, 4)), (6, (3, 4, 37))])
 @pytest.mark.parametrize("slab", [0, 3])
 def test_sensitivities_walk_random_rays(seed, shape, slab):

@@ -89,6 +89,12 @@ _SIGNATURES = {
     "b200drr_trilinear_bwd_sens_pose": (ctypes.c_int, [
         _c_float_p, _c_float_p, _c_float_p, _c_float_p, _c_float_p, _c_float_p, _c_float_p, _c_float_p, _c_float_p,
         ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_void_p]),
+    "b200drr_siddon_jac_sens_pose": (ctypes.c_int, [
+        _c_float_p, _c_float_p, _c_float_p, _c_float_p, _c_float_p, _c_float_p, _c_float_p, _c_float_p, ctypes.c_int,
+        ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_void_p]),
+    "b200drr_trilinear_jac_sens_pose": (ctypes.c_int, [
+        _c_float_p, _c_float_p, _c_float_p, _c_float_p, _c_float_p, _c_float_p, _c_float_p, _c_float_p, _c_float_p,
+        ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_void_p]),
     "b200drr_euler_pose_fwd": (ctypes.c_int, [
         _c_float_p, _c_float_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_float, _c_float_p, ctypes.c_int,
         ctypes.c_void_p]),

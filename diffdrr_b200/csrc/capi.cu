@@ -456,6 +456,26 @@ int b200drr_trilinear_bwd_sens_pose(const float* sens, const float* gout, const 
                                               (cudaStream_t)stream));
 }
 
+int b200drr_siddon_jac_sens_pose(const float* sens, const float* dsrc, const float* dG, const float* dWd, const float* Wd,
+                                 const float* rows, const float* cols, float* J, int B, int H, int W, int P, int stop_grad,
+                                 void* stream)
+{
+    if (!sens || !dsrc || !dG || !dWd || !Wd || !rows || !cols || !J || H <= 0 || W <= 0 || bad_rays(B, (int64_t)H * W) || P < 1 ||
+        P > 16)
+        return B200DRR_EINVAL;
+    return ret(launch_siddon_jac_sens_pose(sens, dsrc, dG, dWd, Wd, rows, cols, J, B, H, W, P, stop_grad != 0, (cudaStream_t)stream));
+}
+
+int b200drr_trilinear_jac_sens_pose(const float* sens, const float* dsrc, const float* dG, const float* dWd, const float* Wd,
+                                    const float* rows, const float* cols, const float* drange, float* J, int B, int H, int W, int P,
+                                    void* stream)
+{
+    if (!sens || !dsrc || !dG || !dWd || !Wd || !rows || !cols || !drange || !J || H <= 0 || W <= 0 ||
+        bad_rays(B, (int64_t)H * W) || P < 1 || P > 16)
+        return B200DRR_EINVAL;
+    return ret(launch_trilinear_jac_sens_pose(sens, dsrc, dG, dWd, Wd, rows, cols, drange, J, B, H, W, P, (cudaStream_t)stream));
+}
+
 static bool bad_axes(int c0, int c1, int c2)
 {
     return c0 < 0 || c0 > 2 || c1 < 0 || c1 > 2 || c2 < 0 || c2 > 2 || c1 == c0 || c1 == c2;

@@ -221,6 +221,14 @@ cudaError_t launch_trilinear_bwd_packed(const float* packed, VolDims dims, const
                                         float* g_raylen, float* g_alpha_range, int B, int H, int W, float shift, float eps,
                                         int n_points, const float* alpha_range, int slab, cudaStream_t stream);
 
+// per-pixel pose Jacobians from the saved sensitivities (jacobian.cu)
+cudaError_t launch_siddon_jac_sens_pose(const float* sens, const float* dsrc, const float* dG, const float* dWd, const float* Wd,
+                                        const float* rows, const float* cols, float* J, int B, int H, int W, int P, int stop_grad,
+                                        cudaStream_t stream);
+cudaError_t launch_trilinear_jac_sens_pose(const float* sens, const float* dsrc, const float* dG, const float* dWd, const float* Wd,
+                                           const float* rows, const float* cols, const float* drange, float* J, int B, int H, int W,
+                                           int P, cudaStream_t stream);
+
 // image similarity of the registration loop (ncc.cu)
 int64_t ncc_workspace_bytes(int B, int C, int64_t N);
 cudaError_t launch_ncc_fwd(const float* x1, const float* x2, int B, int C, int64_t N, float eps, void* workspace, float* stats,

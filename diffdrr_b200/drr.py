@@ -154,6 +154,22 @@ class DRR(nn.Module):
             img = self.render(self.density, source, target, mask_to_channels, **kwargs)
         return self.reshape_transform(img, batch_size=len(pose))
 
+    def jacobian(self, *args, parameterization: str, convention: str = None, degrees: bool = False,
+                 calibration: RigidTransform = None, n_points: int = 500, return_range_terms: bool = False):
+        """(img, J): the image `self(*args, parameterization=...)` renders and its per-pixel Jacobian with respect to each pose's
+        own parameters, J of shape img.shape + (p,) -- the rotation's components first, then the translation's 3 (DESIGN.md 6e).
+
+        Trilinear's sampling range is global over the batch, so with B > 1 pose b's image also depends on the (at most two)
+        poses owning the extreme rays; `return_range_terms=True` adds (dI/dalphamin, dI/dalphamax, drange (B, 2, p)) to build
+        those cross-pose columns: dI_b/dtheta_c = [b == c] J[b] + dI/dalphamin[b] drange[c, 0] + dI/dalphamax[b] drange[c, 1]
+        for c != b.  (None, None, None) for Siddon.  Supported: the fused pose-in paths (Siddon with default options, with or
+        without stop_gradients_through_grid_sample; Trilinear with default options and a packed static volume), fp32 / fp16 /
+        bf16 densities, the full detector; anything else raises before any launch.  Detached results, no host sync of its own."""
+        from .jacobian import drr_jacobian
+
+        return drr_jacobian(self, *args, parameterization=parameterization, convention=convention, degrees=degrees,
+                            calibration=calibration, n_points=n_points, return_range_terms=return_range_terms)
+
     # ---- fused pose-in path (SURVEY.md 8f-2) ------------------------------------------------------------------
     def _pose_in_ok(self, mask_to_channels, kwargs) -> bool:
         """True when the whole pose -> rays -> Siddon chain can run as ONE kernel with in-kernel ray generation."""
@@ -185,23 +201,22 @@ class DRR(nn.Module):
         """detector.forward (detector.py:144-154) + ray lengths / affine_inverse (drr.py:201-205) collapsed into two
         3x4 matrices per pose; the rays themselves are generated inside the CUDA kernel.  `rows=(h0, h1)` renders only
         that block of detector rows (ray sharding across GPUs, parallel.py) -> (B, 1, (h1-h0)*W)."""
+        return self._pose_render(*self._pose_in_inputs(pose, calibration, rows), n_points)
+
+    def _pose_in_inputs(self, pose: RigidTransform, calibration: RigidTransform | None, rows: tuple | None = None):
+        """(src, G, Wd, rows, cols): the inputs of the pose-in kernels for `pose` (see _render_pose_in)."""
         det = self.detector
         if calibration is None and pose.matrix.dtype == torch.float32:
             # the whole composition below as one kernel per direction (include/b200drr.h: b200drr_pose_rays_fwd/_bwd)
             Q, r, Ainv = self._pose_constants()
             src, G, Wd = geometry.pose_rays(pose.matrix, Q, r, Ainv)
-            return self._pose_render(src, G, Wd, *self._grid_axes(rows), n_points)
+            return (src, G, Wd, *self._grid_axes(rows))
         grid = det.target.view(det.height, det.width, 3)
         if rows is not None:
             grid = grid[rows[0]:rows[1]]
         calib = det._calibration if calibration is None else calibration.matrix
-        M = pose.matrix @ det._reorient            # canonical C-arm frame -> world   (reorient.compose(extrinsic))
-        T = M @ calib                              # ... including the intrinsic scaling of the detector plane
-        A_inv = self._affine_inverse               # world -> voxel index
-        G = (A_inv @ T)[:, :3, :]
-        src = (A_inv @ M)[:, :3, 3]                # the canonical source is the origin
-        Wd = torch.cat([T[:, :3, :3], (T[:, :3, 3] - M[:, :3, 3]).unsqueeze(-1)], dim=-1)  # target - source, world
-        return self._pose_render(src, G, Wd, grid[:, 0, 1], grid[0, :, 0], n_points)
+        src, G, Wd = pose_in_matrices(pose.matrix, det._reorient, calib, self._affine_inverse)
+        return src, G, Wd, grid[:, 0, 1], grid[0, :, 0]
 
     def _pose_render(self, src, G, Wd, rows, cols, n_points):
         if isinstance(self.renderer, Trilinear):
@@ -318,6 +333,17 @@ class DRR(nn.Module):
         homog = torch.nn.functional.pad(pts, (0, 1), value=1)
         x = self.detector.sdd * (homog @ self.detector.intrinsic.inverse().mT)
         return self.detector.reorient.compose(pose)(x)
+
+
+def pose_in_matrices(P: torch.Tensor, reorient: torch.Tensor, calib: torch.Tensor, A_inv: torch.Tensor):
+    """Pose matrices P (B, 4, 4) -> the pose-in kernels' (src (B, 3), G (B, 3, 4), Wd (B, 3, 4)): detector.forward
+    (detector.py:144-154) + ray lengths / affine_inverse (drr.py:201-205) collapsed into two 3x4 matrices per pose."""
+    M = P @ reorient                           # canonical C-arm frame -> world   (reorient.compose(extrinsic))
+    T = M @ calib                              # ... including the intrinsic scaling of the detector plane
+    G = (A_inv @ T)[:, :3, :]                  # A_inv: world -> voxel index
+    src = (A_inv @ M)[:, :3, 3]                # the canonical source is the origin
+    Wd = torch.cat([T[:, :3, :3], (T[:, :3, 3] - M[:, :3, 3]).unsqueeze(-1)], dim=-1)  # target - source, world
+    return src, G, Wd
 
 
 def reshape_subsampled_drr(img: torch.Tensor, detector: Detector, batch_size: int):

@@ -616,6 +616,14 @@ def trilinear_pose_render(renderer, volume, packed, src, G, Wd, rows, cols, n_po
     by a reduction kernel over the in-kernel rays, then rebuilt differentiably in torch from the TWO rays that attain it."""
     if volume.dtype in _VOL16:
         _check_vol16(volume, src, G)
+    alpha_range, _ = pose_alpha_range(renderer, volume, src, G, Wd, rows, cols)
+    return _TrilinearPoseFunction.apply(packed, tuple(volume.shape), src, G, Wd, rows, cols, alpha_range,
+                                        float(renderer.voxel_shift), float(renderer.eps), int(n_points), volume.dtype)
+
+
+def pose_alpha_range(renderer, volume, src, G, Wd, rows, cols):
+    """(alpha_range [2], arg [2]): the batch-global sampling range of the in-kernel rays, differentiable in (src, G), and the
+    linear ray index b*H*W + h*W + w of the ray attaining each end (see trilinear_pose_render)."""
     B, H, W = G.shape[0], rows.numel(), cols.numel()
     dev = volume.device
     src_c, G_c, Wd_c = src.detach().contiguous().float(), G.detach().contiguous().float(), Wd.detach().contiguous().float()
@@ -636,9 +644,7 @@ def trilinear_pose_render(renderer, volume, packed, src, G, Wd, rows, cols, n_po
     src2 = src[b].float().unsqueeze(1)                                           # (2, 1, 3)
     dims = _dims_tensor(volume.shape, dev, torch.float32)
     amin, amax = _get_alpha_minmax(src2, tgt2, dims, renderer.voxel_shift, renderer.eps)
-    alpha_range = torch.stack([amin[0, 0, 0], amax[1, 0, 0]])
-    return _TrilinearPoseFunction.apply(packed, tuple(volume.shape), src, G, Wd, rows, cols, alpha_range,
-                                        float(renderer.voxel_shift), float(renderer.eps), int(n_points), volume.dtype)
+    return torch.stack([amin[0, 0, 0], amax[1, 0, 0]]), arg
 
 
 class _SiddonFunction64(torch.autograd.Function):

@@ -273,6 +273,26 @@ int b200drr_trilinear_bwd_sens_pose(const float *sens, const float *gout, const 
                                     int H, int W, void *stream);
 
 /*
+ * Per-pixel pose Jacobians from the sensitivities of a full row-major detector grid (the forward-mode twins of
+ * b200drr_siddon_bwd_sens_pose / b200drr_trilinear_bwd_sens_pose).  sens [B][H*W][8] (Siddon) or [B][H*W][12] (Trilinear) from
+ * any producer of that layout (*_fwd_sens_pose and their _v16 twins, *_fwd_sens_grid / _sens_packed).  The pose has P
+ * parameters (1 <= P <= 16); dsrc [B][P][3], dG [B][P][3][4], dWd [B][P][3][4] are the derivatives of the pose-in inputs src, G,
+ * Wd with respect to each of them, and, with p = (cols[w], rows[h], 1, 1) and dl = Wd.p,
+ *   J [B][H*W][P] (overwritten) = dI/dtgt . dG_k p + S (dl . dWd_k p) / |dl| + dI/dsrc . dsrc_k
+ *                                 [Trilinear: + dI/dalphamin drange[b][0][k] + dI/dalphamax drange[b][1][k]]
+ * The ray-length term is dropped when stop_grad != 0, as in b200drr_siddon_bwd_sens_pose.  drange [B][2][P] is the derivative
+ * of the batch-global sampling range with respect to pose b's parameters: zero for poses that own neither extreme ray.
+ * One thread per pixel; nothing is reduced, so sum_n g_n J[b][n][k] equals the contraction of the *_bwd_sens_pose gradients with
+ * tangent k to fp32 round-off.
+ */
+int b200drr_siddon_jac_sens_pose(const float *sens, const float *dsrc, const float *dG, const float *dWd, const float *Wd,
+                                 const float *rows, const float *cols, float *J, int B, int H, int W, int P, int stop_grad,
+                                 void *stream);
+int b200drr_trilinear_jac_sens_pose(const float *sens, const float *dsrc, const float *dG, const float *dWd, const float *Wd,
+                                    const float *rows, const float *cols, const float *drange, float *J, int B, int H, int W,
+                                    int P, void *stream);
+
+/*
  * mask_to_channels forward (reference renderers.py:77-89 and 242-252): `mask` is the label volume [D0][D1][D2] stored
  * as fp32 (as DRR registers it, drr.py:86-91); every segment / sample contributes to channel label(voxel), sampled
  * nearest with zero padding.  out [B][C][N] is overwritten.  Siddon: reduce="sum", align_corners=0.

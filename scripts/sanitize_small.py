@@ -76,6 +76,14 @@ img = drr(rot, xyz, parameterization="euler_angles", convention="ZXY", n_points=
 img.sum().backward()
 torch.cuda.synchronize()
 print("trilinear pose-in ok", float(img.sum()), float(rot.grad.abs().max()))
+# per-pixel pose Jacobians (jacobian.cu): a ragged last pixel block, 6 and 13 pose parameters, both renderers
+for renderer in ("siddon", "trilinear"):
+    drr = DRR(synthetic.make_subject(vol), **synthetic.detector_kwargs(23), renderer=renderer).to(dev)
+    for par in ("euler_angles", "quaternion_adjugate"):
+        r, x = convert(rot.detach(), xyz.detach(), parameterization="euler_angles", convention="ZXY").convert(par, convention="ZXY")
+        img, J = drr.jacobian(r.contiguous(), x.contiguous(), parameterization=par, convention="ZXY", n_points=64)
+        torch.cuda.synchronize()
+        print(renderer, par, "jacobian ok", tuple(J.shape), float(J.abs().max()))
 # image losses: patch-wise NCC (p = 1, a single window row), blur + Sobel with halos past both image edges and a wide blur
 for shape, losses in (((2, 1, 37, 45), (MultiscaleNormalizedCrossCorrelation2d([None, 5, 1], [0.5, 0.3, 0.2]),
                                         GradientNormalizedCrossCorrelation2d(patch_size=9), GradientNormalizedCrossCorrelation2d(sigma=2.5))),

@@ -1012,6 +1012,27 @@ int b200drr_local_ncc_bwd(const float* x1, const float* x2, const float* stats, 
     return ret(launch_local_ncc_bwd(x1, x2, stats, gscore, g_x1, g_x2, B, C, H, W, p, workspace, (cudaStream_t)stream));
 }
 
+static bool bad_ncc_normal(int B, int C, int H, int W, int p, int P)
+{
+    return B <= 0 || C <= 0 || H <= 0 || W <= 0 || p < 0 || p > H || p > W || P < 1 || P > 16 || (int64_t)B * C > 65535;
+}
+
+int64_t b200drr_ncc_normal_workspace_bytes(int B, int C, int H, int W, int p, int P)
+{
+    if (bad_ncc_normal(B, C, H, W, p, P)) return 0;
+    return ncc_normal_workspace_bytes(B, C, H, W, p, P);
+}
+
+int b200drr_ncc_normal(const float* x, const float* t, const float* J, int64_t sJb, int64_t sJc, int64_t sJk, int64_t sJn, int B,
+                       int C, int H, int W, int p, int P, double eps, double weight, void* workspace, double* A, double* g,
+                       void* stream)
+{
+    if (!x || !t || !J || !workspace || !A || !g || sJb < 0 || sJc < 0 || sJk < 0 || sJn < 0 || !(eps >= 0.0) ||
+        bad_ncc_normal(B, C, H, W, p, P))
+        return B200DRR_EINVAL;
+    return ret(launch_ncc_normal(x, t, J, sJb, sJc, sJk, sJn, B, C, H, W, p, P, eps, weight, workspace, A, g, (cudaStream_t)stream));
+}
+
 // odd kernel size, blur radius below both image sides (reflect padding), shared-memory tiles that fit
 static bool bad_sobel(int B, int H, int W, int ksize)
 {

@@ -243,6 +243,12 @@ cudaError_t launch_local_ncc_fwd(const float* x1, const float* x2, int B, int C,
 cudaError_t launch_local_ncc_bwd(const float* x1, const float* x2, const float* stats, const float* gscore, float* g_x1, float* g_x2,
                                  int B, int C, int H, int W, int p, void* workspace, cudaStream_t stream);
 
+// Gauss-Newton normal equations of the global / patch-wise NCC (ncc_normal.cu); p = 0 is the global NCC
+int64_t ncc_normal_workspace_bytes(int B, int C, int H, int W, int p, int P);
+cudaError_t launch_ncc_normal(const float* x, const float* t, const float* J, int64_t sb, int64_t sc, int64_t sk, int64_t sn, int B,
+                              int C, int H, int W, int p, int P, double eps, double weight, void* workspace, double* A, double* g,
+                              cudaStream_t stream);
+
 // blur + Sobel front end of the gradient NCC (sobel.cu)
 int64_t sobel_workspace_bytes(int B, int H, int W);
 bool sobel_kernel_fits(int k);

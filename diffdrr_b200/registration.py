@@ -42,37 +42,107 @@ class Registration(nn.Module):
         return self._translation
 
 
+def ncc_normal_equations(x, t, J, strides, patch_size, eps, weight, A, g):
+    """A += weight * sum Jz^T Jz, g += weight * sum Jz^T r over every window of every channel of the global (patch_size None) or
+    patch-wise NCC between x and t ((B, C, H, W) fp32 CUDA, contiguous), through b200drr_ncc_normal (csrc/ncc_normal.cu).
+    J: fp32 CUDA tensor whose element (pose b, channel c, parameter k, pixel n) sits at the element strides `strides`
+    (b, c, k, n) from its data pointer; A (B, P, P) and g (B, P) float64.  r = z(x) - z(t) per window, Jz its Jacobian
+    (DESIGN.md 6e)."""
+    from . import _lib
+    B, C, H, W = x.shape
+    P = g.shape[1]
+    p = 0 if patch_size is None else int(patch_size)
+    lib = _lib.load()
+    ws = torch.empty(max(int(lib.b200drr_ncc_normal_workspace_bytes(B, C, H, W, p, P)) // 8, 1), dtype=torch.float64,
+                     device=x.device)
+    _lib.check(lib.b200drr_ncc_normal(x.data_ptr(), t.data_ptr(), J.data_ptr(), *(int(s) for s in strides), B, C, H, W, p, P,
+                                      float(eps), float(weight), ws.data_ptr(), A.data_ptr(), g.data_ptr(),
+                                      torch.cuda.current_stream(x.device).cuda_stream), "b200drr_ncc_normal")
+
+
 class LevenbergMarquardt:
-    """Levenberg-Marquardt steps of a `Registration` towards `target` on the global NCC loss (NormalizedCrossCorrelation2d(),
-    patch_size=None), built on DRR.jacobian (DESIGN.md 6e).
+    """Levenberg-Marquardt steps of a `Registration` towards `target` on an NCC loss, built on DRR.jacobian (DESIGN.md 6e).
 
-    The Gauss-Newton model is the z-normalised residual r = z(img) - z(target), z(x) = (x - mean x) / sqrt(var x + eps)
-    (population variance, as in metrics.py), for which |r|^2 / 2N ~= 1 - NCC.  Each step takes one Jacobian, solves the damped
-    normal equations (A + lambda diag A) delta = -J_z^T r per pose in float64, renders one trial image, and keeps the trial per
-    pose only if its true loss is lower (lambda / 10 on accept, x 10 on reject).  The pose Parameters are updated in place and
-    keep their identity, so an optimizer can take over.  The poses are solved independently (for Trilinear with B > 1 the
-    coupling through the batch-global sampling range is left out of the model; the true loss still decides).  No host sync."""
+    `loss` is a NormalizedCrossCorrelation2d (global or any patch_size), a MultiscaleNormalizedCrossCorrelation2d or a
+    GradientNormalizedCrossCorrelation2d (global or patch-wise, any sigma); None is the global NCC with `eps`.  Mutual
+    information is not a sum of squares and other losses have no such model: they raise here.  The Gauss-Newton model of scale s
+    is the z-normalised residual r_w = z(img_w) - z(target_w) of every window w of every channel, z(x) = (x - mean x) /
+    sqrt(var x + eps) (population variance, as in metrics.py), for which w_s (1 - score_s) ~= w_s / (2 N_s) sum_w |r_w|^2 with
+    N_s = C H' W' p^2 (C H W for the global NCC); the gradient NCC models the blurred Sobel gradients, which are linear in the
+    image, so its J is the loss's own Sobel of the Jacobian planes.  Each step takes one Jacobian, accumulates the normal
+    equations of every scale on the GPU (b200drr_ncc_normal), solves (A + lambda diag A) delta = -g per pose in float64, renders
+    one trial image, and keeps the trial per pose only if its true loss (the module's own forward) is lower (lambda / 10 on
+    accept, x 10 on reject).  The pose Parameters are updated in place and keep their identity, so an optimizer can take over.
+    The poses are solved independently (for Trilinear with B > 1 the coupling through the batch-global sampling range is left
+    out of the model; the true loss still decides).  No host sync."""
 
-    def __init__(self, reg: Registration, target: torch.Tensor, damping: float = 1e-3, eps: float = 1e-5):
-        from .metrics import NormalizedCrossCorrelation2d
+    def __init__(self, reg: Registration, target: torch.Tensor, loss=None, damping: float = 1e-3, eps: float = 1e-5):
+        from .metrics import (GradientNormalizedCrossCorrelation2d, MultiscaleNormalizedCrossCorrelation2d,
+                              NormalizedCrossCorrelation2d)
 
-        self.reg, self.eps = reg, eps
-        self.target = target.detach()
-        self.ncc = NormalizedCrossCorrelation2d(eps=eps)
+        self.sobel = None
+        if loss is None:
+            loss = NormalizedCrossCorrelation2d(eps=eps)
+            scales = [(None, 1.0, eps)]
+        elif type(loss) is NormalizedCrossCorrelation2d:
+            scales = [(loss.patch_size, 1.0, loss.eps)]
+        elif type(loss) is GradientNormalizedCrossCorrelation2d:
+            scales = [(loss.patch_size, 1.0, loss.eps)]
+            self.sobel = loss.sobel
+        elif type(loss) is MultiscaleNormalizedCrossCorrelation2d:
+            scales = [(ncc.patch_size, float(w), ncc.eps) for ncc, w in zip(loss.nccs, loss.patch_weights)]
+        else:
+            raise TypeError(f"LevenbergMarquardt needs a loss that is a sum of squares: NormalizedCrossCorrelation2d, "
+                            f"MultiscaleNormalizedCrossCorrelation2d or GradientNormalizedCrossCorrelation2d, not "
+                            f"{type(loss).__name__} (mutual information has no Gauss-Newton model: use a first-order optimizer)")
+        if not torch.is_tensor(target) or target.dim() != 4 or target.shape[1] != 1:
+            raise ValueError(f"LevenbergMarquardt takes a one-channel target image (B, 1, H, W) like the DRR's, got "
+                             f"{tuple(target.shape) if torch.is_tensor(target) else type(target).__name__}")
         B = reg._rotation.shape[0]
+        Bt, _, H, W = target.shape
+        if Bt not in (1, B):
+            raise ValueError(f"the target's batch ({Bt}) must be 1 or the number of poses ({B})")
+        for p, _, _ in scales:
+            if p is not None and not (isinstance(p, int) and 1 <= p <= min(H, W)):
+                raise ValueError(f"patch_size {p} outside 1 .. min(H, W) = {min(H, W)} of the {H} x {W} images")
+        if self.sobel is not None and self.sobel.kernel_size // 2 >= min(H, W):
+            raise ValueError(f"Sobel(sigma={self.sobel.sigma}): the blur's reflect padding of {self.sobel.kernel_size // 2} "
+                             f"pixels needs images larger than that, got {H} x {W}")
+        if not (target.is_cuda and target.dtype == torch.float32):
+            raise ValueError("LevenbergMarquardt's normal equations run on the GPU: the target must be a CUDA fp32 tensor")
+        self.reg, self.eps, self.loss, self.scales = reg, eps, loss, scales
+        # the losses compare images of one shape: the target repeated for every pose
+        self.target = target.detach().expand(B, *target.shape[1:]).contiguous()
         self.damping = torch.full((B,), float(damping), dtype=torch.float64, device=reg._rotation.device)
-        self._zt = self._znorm(self.target.reshape(self.target.shape[0], -1).double())
-
-    def _znorm(self, x):
-        xc = x - x.mean(dim=1, keepdim=True)
-        s = (xc.square().mean(dim=1, keepdim=True) + self.eps).sqrt()
-        return xc / s
+        with torch.no_grad():
+            self._t = self.target if self.sobel is None else self.sobel(self.target)
 
     def _loss(self, img):
-        return 1.0 - self.ncc(self.target, img)
+        return 1.0 - self.loss(self.target, img)
+
+    def normal_equations(self, img, J):
+        """(A (B, P, P), g (B, P)) float64 of the Gauss-Newton model at the image `img` (B, 1, H, W) with Jacobian J
+        (B, 1, H, W, P): sum over the scales of w_s / N_s times the scale's sum_w Jz^T Jz and sum_w Jz^T r."""
+        B, H, W, P = img.shape[0], img.shape[-2], img.shape[-1], J.shape[-1]
+        if tuple(img.shape[1:]) != (1, H, W) or (H, W) != tuple(self._t.shape[-2:]):
+            raise ValueError(f"the rendered image {tuple(img.shape)} does not match the target {tuple(self.target.shape)}")
+        if self.sobel is None:
+            x, Jv, strides = img.contiguous(), J.contiguous(), (H * W * P, 0, 1, P)
+        else:
+            # blur and Sobel are linear: the Jacobian of the gradient images is the Sobel of the Jacobian planes
+            x = self.sobel(img)
+            Jv = self.sobel(J.reshape(B, H * W, P).transpose(1, 2).reshape(B * P, 1, H, W))
+            strides = (2 * P * H * W, H * W, 2 * H * W, 1)
+        C = x.shape[1]
+        A = torch.zeros(B, P, P, dtype=torch.float64, device=img.device)
+        g = torch.zeros(B, P, dtype=torch.float64, device=img.device)
+        for p, w, eps in self.scales:
+            N = C * H * W if p is None else C * (H - p + 1) * (W - p + 1) * p * p
+            ncc_normal_equations(x, self._t, Jv, strides, p, eps, w / N, A, g)
+        return A, g
 
     def step(self) -> torch.Tensor:
-        """One damped Gauss-Newton step; -> the per-pose 1 - NCC after it."""
+        """One damped Gauss-Newton step; -> the per-pose 1 - loss(target, image) after it."""
         reg = self.reg
         rot, xyz = reg._rotation, reg._translation
         kw = dict(parameterization=reg.parameterization, convention=reg.convention)
@@ -81,17 +151,9 @@ class LevenbergMarquardt:
         with torch.no_grad():
             # the model is of the image itself: the full derivative even if the renderer stops gradients for training
             img, J = drr_jacobian(reg.drr, rot, xyz, stop_grad=False, **kw)
-            B, nr = img.shape[0], rot.shape[1]
-            x = img.reshape(B, -1).double()
-            Jx = J.reshape(B, x.shape[1], -1).double()
-            xc = x - x.mean(dim=1, keepdim=True)
-            s = (xc.square().mean(dim=1, keepdim=True) + self.eps).sqrt()
-            z = xc / s
-            # d z = (dI - mean dI) / s - z mean(z dI) / s
-            Jz = (Jx - Jx.mean(dim=1, keepdim=True) - z.unsqueeze(-1) * (z.unsqueeze(-1) * Jx).mean(dim=1, keepdim=True)) / s.unsqueeze(-1)
-            r = (z - self._zt).unsqueeze(-1)
-            A = Jz.mT @ Jz
-            g = Jz.mT @ r
+            nr = rot.shape[1]
+            A, g = self.normal_equations(img, J)
+            g = g.unsqueeze(-1)
             D = torch.diag_embed(torch.diagonal(A, dim1=-2, dim2=-1).clamp_min(1e-12))
             delta = torch.linalg.solve_ex(A + self.damping[:, None, None] * D, -g)[0].squeeze(-1).to(rot.dtype)
             rot_t, xyz_t = rot + delta[:, :nr], xyz + delta[:, nr:]

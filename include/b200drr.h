@@ -507,6 +507,24 @@ int b200drr_local_ncc_bwd(const float *x1, const float *x2, const float *stats, 
                           int C, int H, int W, int p, void *workspace, void *stream);
 
 /*
+ * Gauss-Newton normal equations of the global (p = 0) or patch-wise (1 <= p <= min(H, W)) NCC between a rendered stack x and a
+ * target t, both [B][C][H][W] (device, contiguous), for the pose Jacobian J: fp32, pixel n = h*W + w of parameter k of (pose b,
+ * channel c) at J[b*sJb + c*sJc + k*sJk + n*sJn] (element strides >= 0: DRR.jacobian's (B, H*W, P) is {H*W*P, 0, 1, P}, the blur +
+ * Sobel of its planes (B, P, 2, H, W) is {2*P*H*W, H*W, 2*H*W, 1}).  1 <= P <= 16, B*C <= 65535, eps >= 0.
+ * Every window w (the whole H x W image when p = 0) of every channel is z-normalised as in b200drr_local_ncc_fwd (mean,
+ * population variance + eps, clamped at 0); with the window's residual r = z(x) - z(t) and its Jacobian Jz (J through z(x)):
+ *   A [B][P][P] += weight * sum_{c,w} sum_q Jz_q Jz_q^T,   g [B][P] += weight * sum_{c,w} sum_q Jz_q r_q   (float64; the caller
+ *   zero-fills, so several calls, e.g. one per scale of a multiscale loss, accumulate into one system).
+ * Evaluated from box sums of the 5 + 3P channels {x, x^2, t, t^2, x t, J, x J, t J} and an adjoint box sum of 1/(var + eps), all in
+ * double, in a fixed order (no atomics: repeated calls give identical bits); nothing of size windows x pixels or pixels x P^2 is
+ * formed.  workspace: b200drr_ncc_normal_workspace_bytes(B, C, H, W, p, P) bytes, 8-byte aligned (0 for bad arguments).
+ */
+int64_t b200drr_ncc_normal_workspace_bytes(int B, int C, int H, int W, int p, int P);
+int b200drr_ncc_normal(const float *x, const float *t, const float *J, int64_t sJb, int64_t sJc, int64_t sJk, int64_t sJn, int B,
+                       int C, int H, int W, int p, int P, double eps, double weight, void *workspace, double *A, double *g,
+                       void *stream);
+
+/*
  * Gaussian blur + Sobel gradients of one-channel images (reference diffdrr/metrics.py:69-93, the Sobel front end of
  * GradientNormalizedCrossCorrelation2d).  x [B][H][W] (device) -> out [B][2][H][W]:
  *   blur   separable, 1-D weights [ksize] (device; torchvision's normalised Gaussian, ksize odd; ksize = 1 with weight 1 is no

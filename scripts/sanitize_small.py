@@ -103,4 +103,15 @@ for shape, nb in (((2, 1, 37, 45), 37), ((1, 1, 9, 70), 100), ((3, 1, 33, 17), 2
     mi(a.detach(), b).sum().backward()
     torch.cuda.synchronize()
     print(shape, nb, "MutualInformation ok", float(a.grad.abs().max()), float(b.grad.abs().max()))
+# NCC normal equations (ncc_normal.cu): partial window tiles and pixel chunks, p = 1, p = min(H, W), global, P = 1 and 16
+from diffdrr_b200.registration import ncc_normal_equations  # noqa: E402
+for (B, C, H, W), P, ps in (((2, 2, 37, 45), 1, (None, 1, 5, 37)), ((1, 1, 9, 70), 16, (None, 3, 9)), ((3, 2, 67, 13), 6, (13, None))):
+    x, t = torch.rand(B, C, H, W, device=dev), torch.rand(B, C, H, W, device=dev)
+    J = torch.randn(B, P, C, H, W, device=dev)
+    for p in ps:
+        A = torch.zeros(B, P, P, dtype=torch.float64, device=dev)
+        g = torch.zeros(B, P, dtype=torch.float64, device=dev)
+        ncc_normal_equations(x, t, J, (P * C * H * W, H * W, C * H * W, 1), p, 1e-5, 1.0, A, g)
+        torch.cuda.synchronize()
+        print((B, C, H, W), P, p, "ncc_normal ok", float(A.abs().max()), float(g.abs().max()))
 print("done")

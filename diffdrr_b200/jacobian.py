@@ -14,8 +14,8 @@ import torch
 
 from . import _lib, geometry
 from .pose import PARAMETERIZATIONS, RigidTransform, convert
-from .renderers import (_PACKED_SLAB_MIN_BATCH, _PACKED_SLAB_SENS, _VOL16, Siddon, Trilinear, _check_vol16, _dims_tensor,
-                        _get_alpha_minmax, _ptr, _stream, _vol_entry, pose_alpha_range)
+from .renderers import (_VOL16, Siddon, Trilinear, _check_vol16, _dims_tensor, _get_alpha_minmax, _ptr, _siddon_sens_pose,
+                        _stream, _trilinear_sens_pose, pose_alpha_range)
 
 
 def pose_in_tangents(rot, xyz, parameterization, convention, degrees, reorient, calib, A_inv):
@@ -148,18 +148,13 @@ def drr_jacobian(drr, *args, parameterization, convention=None, degrees=False, c
         src, G, Wd = src.contiguous().float(), G.contiguous().float(), Wd.contiguous().float()
         rows, cols = rows.contiguous().float(), cols.contiguous().float()
         dev = vol.device
-        out = torch.empty(B, H * W, dtype=torch.float32, device=dev)
         J = torch.empty(B, H * W, P, dtype=torch.float32, device=dev)
         lib = _lib.load()
         if vol.dtype in _VOL16:
             _check_vol16(vol, src, G)
         with torch.cuda.device(dev):
             if not trilinear:
-                sens = torch.empty(B, H * W, 8, dtype=torch.float32, device=dev)
-                v = vol.contiguous()
-                fn, head, name = _vol_entry(lib, "b200drr_siddon_fwd_sens_pose", v)
-                _lib.check(fn(*head, *v.shape, _ptr(src), _ptr(G), _ptr(Wd), _ptr(rows), _ptr(cols), _ptr(out), _ptr(sens), B, H,
-                              W, float(r.voxel_shift), float(r.eps), _stream()), name)
+                out, sens = _siddon_sens_pose(vol.contiguous(), src, G, Wd, rows, cols, float(r.voxel_shift), float(r.eps))
                 stop_grad = int(bool(r.stop_gradients_through_grid_sample if stop_grad is None else stop_grad))
                 _lib.check(lib.b200drr_siddon_jac_sens_pose(_ptr(sens), _ptr(dsrc), _ptr(dG), _ptr(dWd), _ptr(Wd), _ptr(rows),
                                                             _ptr(cols), _ptr(J), B, H, W, P, stop_grad, _stream()),
@@ -171,13 +166,8 @@ def drr_jacobian(drr, *args, parameterization, convention=None, degrees=False, c
                 drange = range_tangents(vol.shape, float(r.voxel_shift), float(r.eps), src, G, rows, cols, arg, tangents[0],
                                         tangents[1])
                 drange = drange.float().contiguous()
-                sens = torch.empty(B, H * W, 12, dtype=torch.float32, device=dev)
-                code = _VOL16.get(vol.dtype)
-                fn = lib.b200drr_trilinear_fwd_sens_pose if code is None else lib.b200drr_trilinear_fwd_sens_pose_v16
-                head = (_ptr(packed),) if code is None else (_ptr(packed), code)
-                _lib.check(fn(*head, *vol.shape, _ptr(src), _ptr(G), _ptr(Wd), _ptr(rows), _ptr(cols), _ptr(out), _ptr(sens), B, H,
-                              W, float(r.voxel_shift), float(r.eps), int(n_points), _ptr(arange),
-                              _PACKED_SLAB_SENS if B >= _PACKED_SLAB_MIN_BATCH else 0, _stream()), fn.__name__)
+                out, sens = _trilinear_sens_pose(vol, packed, src, G, Wd, rows, cols, float(r.voxel_shift), float(r.eps),
+                                                 int(n_points), arange)
                 _lib.check(lib.b200drr_trilinear_jac_sens_pose(_ptr(sens), _ptr(dsrc), _ptr(dG), _ptr(dWd), _ptr(Wd), _ptr(rows),
                                                                _ptr(cols), _ptr(drange), _ptr(J), B, H, W, P, _stream()),
                            "b200drr_trilinear_jac_sens_pose")

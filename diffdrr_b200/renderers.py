@@ -182,38 +182,63 @@ def _wants_sens(needs_input_grad, stop_grad) -> bool:
     return any(needs_input_grad[1:4]) and not need_vol
 
 
+def _ray_grads(ctx, B, N, dtype, device, stop_grad=False):
+    """Gradient buffers of the ray inputs that need one -- inputs 1..3 (source, target, img) of every ray-tensor autograd
+    function: g_src (B,3), g_tgt (B,N,3), g_len (B,N), or None; stop_grad drops the ray-length gradient."""
+    _, need_src, need_tgt, need_len = ctx.needs_input_grad[:4]
+    return (torch.empty(B, 3, dtype=dtype, device=device) if need_src else None,
+            torch.empty(B, N, 3, dtype=dtype, device=device) if need_tgt else None,
+            torch.empty(B, N, dtype=dtype, device=device) if (need_len and not stop_grad) else None)
+
+
+def _ray_grads_back(ctx, g_src, g_tgt, g_len):
+    """The buffers of _ray_grads viewed as the shapes forward received (ctx.ray_shapes)."""
+    src_shape, img_shape = ctx.ray_shapes
+    return None if g_src is None else g_src.view(src_shape), g_tgt, None if g_len is None else g_len.view(img_shape)
+
+
 class _SiddonFunction(torch.autograd.Function):
-    """out (B,1,N) = Siddon line integrals; backward = closed-form kernel (include/b200drr.h)."""
+    """out (B,1,N) = Siddon line integrals; backward = closed-form kernel (include/b200drr.h).  An fp64 volume takes the
+    reference-literal kernels (csrc/literal.cu: b200drr_siddon_fwd_f64 / _bwd_f64, what `drr.to(torch.float64)` reaches in
+    the reference, drr.py:75) and mode = 1 (Siddon(mode="bilinear"), reference renderers.py:18,66: trilinear sampling at the
+    segment midpoints) the general walk (b200drr_siddon_fwd_general / _bwd_general); both run one thread per ray whatever the
+    ray set, and their reducefn="max" is forward-only."""
 
     @staticmethod
-    def forward(ctx, volume, source, target, img, voxel_shift, eps, reduce, align_corners, stop_grad, grid, subset=None):
-        B, N = _check_inputs(volume, source, target, img, vol16=True)
+    def forward(ctx, volume, source, target, img, voxel_shift, eps, reduce, align_corners, stop_grad, grid, subset=None,
+                mode=0):
+        fp64 = volume.dtype == torch.float64
+        B, N = _check_inputs(volume, source, target, img, torch.float64 if fp64 else torch.float32, vol16=True)
         vol = volume.contiguous()
         src = source.reshape(B, 3).contiguous()
         tgt = target.contiguous()
         raylen = img.reshape(B, N).contiguous()
-        out = torch.empty(B, N, dtype=torch.float32, device=vol.device)
+        out = torch.empty(B, N, dtype=torch.float64 if fp64 else torch.float32, device=vol.device)
+        literal = fp64 or mode != 0
         # full detector grid + default options -> tiled, slab-major kernels (include/b200drr.h: *_grid)
-        if grid is not None and (grid[0] * grid[1] != N or reduce != 0 or align_corners or vol.numel() >= 2**31 - 1):
+        if grid is not None and (literal or grid[0] * grid[1] != N or reduce != 0 or align_corners
+                                 or vol.numel() >= 2**31 - 1):
             grid = None
         lib = _lib.load()
+        fast = not literal and reduce == 0 and not align_corners and vol.numel() < 2**31 - 1
         # Ray gradients wanted and no volume gradient: ONE walk yields the image and the 6 per-ray sensitivities, and the
         # backward is elementwise (include/b200drr.h: b200drr_siddon_fwd_sens_grid / _bwd_sens).
         sens = None
-        if (_FUSED_SENSITIVITIES and _wants_sens(ctx.needs_input_grad, stop_grad) and reduce == 0 and not align_corners
-                and vol.numel() < 2**31 - 1):
+        if fast and _FUSED_SENSITIVITIES and _wants_sens(ctx.needs_input_grad, stop_grad):
             sens = torch.empty(B, N, 8, dtype=torch.float32, device=vol.device)
         if vol.dtype in _VOL16 and sens is None and any(ctx.needs_input_grad[1:4]):
             raise NotImplementedError(f"ray gradients from a {vol.dtype} volume come from the fused sensitivities walk only")
         with torch.cuda.device(vol.device):
-            fast = reduce == 0 and not align_corners and vol.numel() < 2**31 - 1
-            if (grid is None and fast and sens is None and subset is not None and subset[0].numel() == subset[2] * subset[3]
+            if literal:   # b200drr_siddon_fwd_f64 takes the arguments of b200drr_siddon_fwd; the general walk adds the mode
+                name = "b200drr_siddon_fwd_f64" if fp64 else "b200drr_siddon_fwd_general"
+                _lib.check(getattr(lib, name)(_ptr(vol), *vol.shape, _ptr(src), _ptr(tgt), _ptr(raylen), _ptr(out), B, N,
+                                              voxel_shift, eps, reduce, int(align_corners), *(() if fp64 else (mode,)),
+                                              _stream()), name)
+            elif (grid is None and fast and sens is None and subset is not None and subset[0].numel() == subset[2] * subset[3]
                     and N == subset[4] and _brick_ok(vol, B, subset[2], subset[3], check_density=False)):
                 # inference on a sub-sampled detector: brick-major kernel with a pixel -> ray map (include/b200drr.h)
                 pix, corners, Hs, Ws, _n = subset
-                need = int(lib.b200drr_siddon_brick_workspace_bytes(B, 1, N))
                 ws = _brick_workspace(vol.device, B, 1, N)
-                assert ws.numel() >= need
                 fn, head, name = _vol_entry(lib, "b200drr_siddon_fwd_brick_subset", vol)
                 _lib.check(fn(*head, *vol.shape, _ptr(src), _ptr(tgt), _ptr(raylen), ctypes.c_void_p(pix.data_ptr()),
                               _ptr(corners.contiguous().float()), _ptr(out), ctypes.c_void_p(ws.data_ptr()), ws.numel(), B, Hs, Ws,
@@ -262,42 +287,46 @@ class _SiddonFunction(torch.autograd.Function):
         else:
             ctx.save_for_backward(vol, src, tgt, raylen)
         ctx.fused = sens is not None
-        ctx.cfg = (voxel_shift, eps, reduce, align_corners, stop_grad, tuple(source.shape), tuple(img.shape), grid)
+        ctx.cfg = (voxel_shift, eps, reduce, align_corners, stop_grad, grid, mode)
+        ctx.ray_shapes = (tuple(source.shape), tuple(img.shape))
         return out.view(B, 1, N)
 
     @staticmethod
     @once_differentiable
     def backward(ctx, gout):
-        voxel_shift, eps, reduce, align_corners, stop_grad, src_shape, img_shape, grid = ctx.cfg
+        voxel_shift, eps, reduce, align_corners, stop_grad, grid, mode = ctx.cfg
         if ctx.fused:
             (sens,) = ctx.saved_tensors
             B, N = sens.shape[0], sens.shape[1]
-            _, need_src, need_tgt, need_len = ctx.needs_input_grad[:4]
             gout = gout.reshape(B, N).contiguous().float()
-            g_src = torch.empty(B, 3, dtype=torch.float32, device=sens.device) if need_src else None
-            g_tgt = torch.empty(B, N, 3, dtype=torch.float32, device=sens.device) if need_tgt else None
-            g_len = torch.empty(B, N, dtype=torch.float32, device=sens.device) if (need_len and not stop_grad) else None
+            g_src, g_tgt, g_len = _ray_grads(ctx, B, N, torch.float32, sens.device, stop_grad)
             with torch.cuda.device(sens.device):
                 _lib.check(_lib.load().b200drr_siddon_bwd_sens(_ptr(sens), _ptr(gout), _ptr(g_src), _ptr(g_tgt), _ptr(g_len),
                                                                B, N, int(stop_grad), _stream()), "b200drr_siddon_bwd_sens")
-            return (None, None if g_src is None else g_src.view(src_shape), g_tgt,
-                    None if g_len is None else g_len.view(img_shape), None, None, None, None, None, None, None)
+            return (None, *_ray_grads_back(ctx, g_src, g_tgt, g_len), None, None, None, None, None, None, None, None)
         vol, src, tgt, raylen = ctx.saved_tensors
+        fp64 = vol.dtype == torch.float64
+        if fp64 and reduce != 0:
+            raise NotImplementedError("fp64 Siddon: backward is implemented for reducefn='sum'")
+        if mode != 0 and reduce != 0:
+            raise NotImplementedError("backward through Siddon(mode='bilinear', reducefn='max') is not implemented")
         B, N = tgt.shape[0], tgt.shape[1]
-        need_vol, need_src, need_tgt, need_len = ctx.needs_input_grad[:4]
-        gout = gout.reshape(B, N).contiguous().float()
-        g_src = torch.empty(B, 3, dtype=torch.float32, device=vol.device) if need_src else None
-        g_tgt = torch.empty(B, N, 3, dtype=torch.float32, device=vol.device) if need_tgt else None
-        g_len = torch.empty(B, N, dtype=torch.float32, device=vol.device) if (need_len and not stop_grad) else None
-        vol_by_brick = (need_vol and not stop_grad and grid is not None and reduce == 0 and not align_corners
+        gout = gout.reshape(B, N).contiguous().to(torch.float64 if fp64 else torch.float32)
+        g_src, g_tgt, g_len = _ray_grads(ctx, B, N, gout.dtype, vol.device, stop_grad)
+        need_vol = ctx.needs_input_grad[0] and not stop_grad
+        vol_by_brick = (need_vol and grid is not None and reduce == 0 and not align_corners
                         and _brick_bwd_ok(vol, B, grid[0], grid[1]))
-        g_vol = (torch.empty_like(vol) if vol_by_brick else torch.zeros_like(vol)) if (need_vol and not stop_grad) else None
+        g_vol = (torch.empty_like(vol) if vol_by_brick else torch.zeros_like(vol)) if need_vol else None
         lib = _lib.load()
         with torch.cuda.device(vol.device):
-            if reduce != 0 or align_corners:  # options outside the fast kernels: plane-by-plane general walk
+            if fp64:   # b200drr_siddon_bwd_f64 takes the arguments of b200drr_siddon_bwd
+                _lib.check(lib.b200drr_siddon_bwd_f64(_ptr(vol), *vol.shape, _ptr(src), _ptr(tgt), _ptr(raylen), _ptr(gout),
+                                                      _ptr(g_src), _ptr(g_tgt), _ptr(g_len), _ptr(g_vol), B, N, voxel_shift, eps,
+                                                      int(stop_grad), int(align_corners), _stream()), "b200drr_siddon_bwd_f64")
+            elif reduce != 0 or align_corners or mode != 0:  # options outside the fast kernels: plane-by-plane general walk
                 _lib.check(lib.b200drr_siddon_bwd_general(_ptr(vol), *vol.shape, _ptr(src), _ptr(tgt), _ptr(raylen), _ptr(gout),
                                                           _ptr(g_src), _ptr(g_tgt), _ptr(g_len), _ptr(g_vol), B, N, voxel_shift,
-                                                          eps, int(stop_grad), reduce, int(align_corners), 0, _stream()),
+                                                          eps, int(stop_grad), reduce, int(align_corners), mode, _stream()),
                            "b200drr_siddon_bwd_general")
             elif vol_by_brick:
                 # volume gradient by the brick kernel's scatter mode (no global atomics; g_vol overwritten), ray gradients --
@@ -322,50 +351,20 @@ class _SiddonFunction(torch.autograd.Function):
                                                   _ptr(g_src), _ptr(g_tgt), _ptr(g_len), _ptr(g_vol), B, N, voxel_shift, eps,
                                                   int(stop_grad), int(align_corners), _stream()),
                            "b200drr_siddon_bwd")
-        return (g_vol, None if g_src is None else g_src.view(src_shape), g_tgt,
-                None if g_len is None else g_len.view(img_shape), None, None, None, None, None, None, None)
+        return (g_vol, *_ray_grads_back(ctx, g_src, g_tgt, g_len), None, None, None, None, None, None, None, None)
 
 
-class _SiddonBilinearFunction(torch.autograd.Function):
-    """Siddon(mode="bilinear") (reference renderers.py:18,66): trilinear sampling at the segment midpoints through the general
-    walk (include/b200drr.h: b200drr_siddon_fwd_general / _bwd_general with mode = 1)."""
-
-    @staticmethod
-    def forward(ctx, volume, source, target, img, voxel_shift, eps, reduce, align_corners, stop_grad):
-        B, N = _check_inputs(volume, source, target, img)
-        vol, src, tgt = volume.contiguous(), source.reshape(B, 3).contiguous(), target.contiguous()
-        raylen = img.reshape(B, N).contiguous()
-        out = torch.empty(B, N, dtype=torch.float32, device=vol.device)
-        with torch.cuda.device(vol.device):
-            _lib.check(_lib.load().b200drr_siddon_fwd_general(_ptr(vol), *vol.shape, _ptr(src), _ptr(tgt), _ptr(raylen),
-                                                              _ptr(out), B, N, voxel_shift, eps, reduce, int(align_corners), 1,
-                                                              _stream()), "b200drr_siddon_fwd_general")
-        ctx.save_for_backward(vol, src, tgt, raylen)
-        ctx.cfg = (voxel_shift, eps, reduce, align_corners, stop_grad, tuple(source.shape), tuple(img.shape))
-        return out.view(B, 1, N)
-
-    @staticmethod
-    @once_differentiable
-    def backward(ctx, gout):
-        vol, src, tgt, raylen = ctx.saved_tensors
-        voxel_shift, eps, reduce, align_corners, stop_grad, src_shape, img_shape = ctx.cfg
-        if reduce != 0:
-            raise NotImplementedError("backward through Siddon(mode='bilinear', reducefn='max') is not implemented")
-        B, N = tgt.shape[0], tgt.shape[1]
-        need_vol, need_src, need_tgt, need_len = ctx.needs_input_grad[:4]
-        gout = gout.reshape(B, N).contiguous().float()
-        dev = vol.device
-        g_src = torch.empty(B, 3, dtype=torch.float32, device=dev) if need_src else None
-        g_tgt = torch.empty(B, N, 3, dtype=torch.float32, device=dev) if need_tgt else None
-        g_len = torch.empty(B, N, dtype=torch.float32, device=dev) if (need_len and not stop_grad) else None
-        g_vol = torch.zeros_like(vol) if (need_vol and not stop_grad) else None
-        with torch.cuda.device(dev):
-            _lib.check(_lib.load().b200drr_siddon_bwd_general(_ptr(vol), *vol.shape, _ptr(src), _ptr(tgt), _ptr(raylen),
-                                                              _ptr(gout), _ptr(g_src), _ptr(g_tgt), _ptr(g_len), _ptr(g_vol), B,
-                                                              N, voxel_shift, eps, int(stop_grad), 0, int(align_corners), 1,
-                                                              _stream()), "b200drr_siddon_bwd_general")
-        return (g_vol, None if g_src is None else g_src.view(src_shape), g_tgt,
-                None if g_len is None else g_len.view(img_shape), None, None, None, None, None)
+def _siddon_sens_pose(vol, src, G, Wd, rows, cols, voxel_shift, eps):
+    """The sensitivities walk of the in-kernel rays of a full detector grid (include/b200drr.h: b200drr_siddon_fwd_sens_pose):
+    -> (out (B, H*W), sens (B, H*W, 8)), the image and every ray's end-point sensitivities.  Inputs contiguous fp32."""
+    B, H, W = G.shape[0], rows.numel(), cols.numel()
+    out = torch.empty(B, H * W, dtype=torch.float32, device=vol.device)
+    sens = torch.empty(B, H * W, 8, dtype=torch.float32, device=vol.device)
+    fn, head, name = _vol_entry(_lib.load(), "b200drr_siddon_fwd_sens_pose", vol)
+    with torch.cuda.device(vol.device):
+        _lib.check(fn(*head, *vol.shape, _ptr(src), _ptr(G), _ptr(Wd), _ptr(rows), _ptr(cols), _ptr(out), _ptr(sens), B, H, W,
+                      voxel_shift, eps, _stream()), name)
+    return out, sens
 
 
 class _SiddonPoseFunction(torch.autograd.Function):
@@ -378,20 +377,17 @@ class _SiddonPoseFunction(torch.autograd.Function):
         B, H, W = G.shape[0], rows.numel(), cols.numel()
         src, G, Wd = src.contiguous().float(), G.contiguous().float(), Wd.contiguous().float()
         rows, cols = rows.contiguous().float(), cols.contiguous().float()
-        out = torch.empty(B, H * W, dtype=torch.float32, device=vol.device)
         ctx.fused = _FUSED_SENSITIVITIES and _wants_sens(ctx.needs_input_grad, stop_grad)
         ctx.cfg = (voxel_shift, eps, stop_grad)
         if vol.dtype in _VOL16 and not ctx.fused and any(ctx.needs_input_grad[1:4]):
             raise NotImplementedError(f"pose gradients from a {vol.dtype} volume come from the fused sensitivities walk only")
+        if ctx.fused:  # one walk: image + per-ray sensitivities; backward is elementwise
+            out, sens = _siddon_sens_pose(vol, src, G, Wd, rows, cols, voxel_shift, eps)
+            ctx.save_for_backward(sens, Wd, rows, cols)
+            return out.view(B, 1, H * W)
+        out = torch.empty(B, H * W, dtype=torch.float32, device=vol.device)
         lib = _lib.load()
         with torch.cuda.device(vol.device):
-            if ctx.fused:  # one walk: image + per-ray sensitivities; backward is elementwise
-                sens = torch.empty(B, H * W, 8, dtype=torch.float32, device=vol.device)
-                fn, head, name = _vol_entry(lib, "b200drr_siddon_fwd_sens_pose", vol)
-                _lib.check(fn(*head, *vol.shape, _ptr(src), _ptr(G), _ptr(Wd), _ptr(rows), _ptr(cols), _ptr(out), _ptr(sens), B,
-                              H, W, voxel_shift, eps, _stream()), name)
-                ctx.save_for_backward(sens, Wd, rows, cols)
-                return out.view(B, 1, H * W)
             if _brick_full_grid_ok(vol, B, H, W):
                 ws = _brick_workspace(vol.device, B, H, W)
                 fn, head, name = _vol_entry(lib, "b200drr_siddon_fwd_brick", vol)
@@ -457,13 +453,16 @@ class _SiddonPoseFunction(torch.autograd.Function):
 
 
 class _TrilinearFunction(torch.autograd.Function):
-    """out (B,1,N) = fixed-step trilinear line integrals for the range alpha_range = [alphamin, alphamax]."""
+    """out (B,1,N) = fixed-step trilinear line integrals for the range alpha_range = [alphamin, alphamax].  An fp64 volume
+    takes the reference-literal kernels (b200drr_trilinear_fwd_f64 / _bwd_f64; alpha_range fp64, reducefn="max" forward-only)
+    whatever the ray set."""
 
     @staticmethod
     def forward(ctx, volume, source, target, img, alpha_range, voxel_shift, eps, n_points, reduce, align_corners, grid,
                 packed):
-        B, N = _check_inputs(volume, source, target, img, vol16=True)
-        if grid is not None and (grid[0] * grid[1] != N or reduce != 0 or align_corners):
+        fp64 = volume.dtype == torch.float64
+        B, N = _check_inputs(volume, source, target, img, torch.float64 if fp64 else torch.float32, vol16=True)
+        if grid is not None and (fp64 or grid[0] * grid[1] != N or reduce != 0 or align_corners):
             grid = None
         if grid is None:
             packed = None
@@ -471,18 +470,24 @@ class _TrilinearFunction(torch.autograd.Function):
         src = source.reshape(B, 3).contiguous()
         tgt = target.contiguous()
         raylen = img.reshape(B, N).contiguous()
-        arange = alpha_range.detach().to(device=vol.device, dtype=torch.float32).contiguous()
-        out = torch.empty(B, N, dtype=torch.float32, device=vol.device)
+        dtype = torch.float64 if fp64 else torch.float32
+        arange = alpha_range.detach().to(device=vol.device, dtype=dtype).contiguous()
+        out = torch.empty(B, N, dtype=dtype, device=vol.device)
         lib = _lib.load()
         # training-step fast path (twin of the Siddon one): ray gradients wanted, static (packed) volume -> one march
         # yields the image and the per-ray sensitivities; backward is elementwise (b200drr_trilinear_bwd_sens)
         sens = None
-        if _FUSED_SENSITIVITIES and reduce == 0 and any(ctx.needs_input_grad[1:5]) and not ctx.needs_input_grad[0]:
+        if (not fp64 and _FUSED_SENSITIVITIES and reduce == 0 and any(ctx.needs_input_grad[1:5])
+                and not ctx.needs_input_grad[0]):
             sens = torch.empty(B, N, 12, dtype=torch.float32, device=vol.device)
         if vol.dtype in _VOL16 and sens is None and any(ctx.needs_input_grad[1:5]):
             raise NotImplementedError(f"ray gradients from a {vol.dtype} volume come from the fused sensitivities march only")
         with torch.cuda.device(vol.device):
-            if sens is not None and packed is None:   # plain volume: arbitrary ray sets, or the grid without a packed copy
+            if fp64:   # b200drr_trilinear_fwd_f64 takes the arguments of b200drr_trilinear_fwd
+                _lib.check(lib.b200drr_trilinear_fwd_f64(_ptr(vol), *vol.shape, _ptr(src), _ptr(tgt), _ptr(raylen), _ptr(out), B,
+                                                         N, voxel_shift, eps, n_points, _ptr(arange), reduce,
+                                                         int(align_corners), _stream()), "b200drr_trilinear_fwd_f64")
+            elif sens is not None and packed is None:   # plain volume: arbitrary ray sets, or the grid without a packed copy
                 h, w_ = grid if grid is not None else (0, 0)
                 fn, head, name = _vol_entry(lib, "b200drr_trilinear_fwd_sens", vol)
                 _lib.check(fn(*head, *vol.shape, _ptr(src), _ptr(tgt), _ptr(raylen), _ptr(out), _ptr(sens), B, N, h, w_,
@@ -511,41 +516,44 @@ class _TrilinearFunction(torch.autograd.Function):
         else:
             ctx.save_for_backward(vol, src, tgt, raylen, arange)
         ctx.packed = None if ctx.fused else packed
-        ctx.cfg = (voxel_shift, eps, n_points, reduce, align_corners, tuple(source.shape), tuple(img.shape), grid)
+        ctx.cfg = (voxel_shift, eps, n_points, reduce, align_corners, grid)
+        ctx.ray_shapes = (tuple(source.shape), tuple(img.shape))
         return out.view(B, 1, N)
 
     @staticmethod
     @once_differentiable
     def backward(ctx, gout):
-        voxel_shift, eps, n_points, reduce, align_corners, src_shape, img_shape, grid = ctx.cfg
+        voxel_shift, eps, n_points, reduce, align_corners, grid = ctx.cfg
+        need_ar = ctx.needs_input_grad[4]
         if ctx.fused:
             (sens,) = ctx.saved_tensors
             B, N = sens.shape[0], sens.shape[1]
-            _, need_src, need_tgt, need_len, need_ar = ctx.needs_input_grad[:5]
             dev = sens.device
             gout = gout.reshape(B, N).contiguous().float()
-            g_src = torch.empty(B, 3, dtype=torch.float32, device=dev) if need_src else None
-            g_tgt = torch.empty(B, N, 3, dtype=torch.float32, device=dev) if need_tgt else None
-            g_len = torch.empty(B, N, dtype=torch.float32, device=dev) if need_len else None
+            g_src, g_tgt, g_len = _ray_grads(ctx, B, N, torch.float32, dev)
             g_ar = torch.zeros(2, dtype=torch.float32, device=dev) if need_ar else None
             with torch.cuda.device(dev):
                 _lib.check(_lib.load().b200drr_trilinear_bwd_sens(_ptr(sens), _ptr(gout), _ptr(g_src), _ptr(g_tgt), _ptr(g_len),
                                                                   _ptr(g_ar), B, N, _stream()), "b200drr_trilinear_bwd_sens")
-            return (None, None if g_src is None else g_src.view(src_shape), g_tgt,
-                    None if g_len is None else g_len.view(img_shape), g_ar, None, None, None, None, None, None, None)
+            return (None, *_ray_grads_back(ctx, g_src, g_tgt, g_len), g_ar, None, None, None, None, None, None, None)
         vol, src, tgt, raylen, arange = ctx.saved_tensors
+        fp64 = vol.dtype == torch.float64
+        if fp64 and reduce != 0:
+            raise NotImplementedError("fp64 trilinear: backward is implemented for reducefn='sum'")
         B, N = tgt.shape[0], tgt.shape[1]
-        need_vol, need_src, need_tgt, need_len, need_ar = ctx.needs_input_grad[:5]
-        gout = gout.reshape(B, N).contiguous().float()
+        gout = gout.reshape(B, N).contiguous().to(torch.float64 if fp64 else torch.float32)
         dev = vol.device
-        g_src = torch.empty(B, 3, dtype=torch.float32, device=dev) if need_src else None
-        g_tgt = torch.empty(B, N, 3, dtype=torch.float32, device=dev) if need_tgt else None
-        g_len = torch.empty(B, N, dtype=torch.float32, device=dev) if need_len else None
-        g_vol = torch.zeros_like(vol) if need_vol else None
-        g_ar = torch.zeros(2, dtype=torch.float32, device=dev) if need_ar else None
+        g_src, g_tgt, g_len = _ray_grads(ctx, B, N, gout.dtype, dev)
+        g_vol = torch.zeros_like(vol) if ctx.needs_input_grad[0] else None
+        g_ar = torch.zeros(2, dtype=gout.dtype, device=dev) if need_ar else None
         lib = _lib.load()
         with torch.cuda.device(dev):
-            if reduce != 0:  # reducefn="max": the first maximal sample carries the gradient
+            if fp64:   # b200drr_trilinear_bwd_f64 takes the arguments of b200drr_trilinear_bwd
+                _lib.check(lib.b200drr_trilinear_bwd_f64(_ptr(vol), *vol.shape, _ptr(src), _ptr(tgt), _ptr(raylen), _ptr(gout),
+                                                         _ptr(g_src), _ptr(g_tgt), _ptr(g_len), _ptr(g_vol), _ptr(g_ar), B, N,
+                                                         voxel_shift, eps, n_points, _ptr(arange), int(align_corners),
+                                                         _stream()), "b200drr_trilinear_bwd_f64")
+            elif reduce != 0:  # reducefn="max": the first maximal sample carries the gradient
                 _lib.check(lib.b200drr_trilinear_bwd_max(_ptr(vol), *vol.shape, _ptr(src), _ptr(tgt), _ptr(raylen), _ptr(gout),
                                                          _ptr(g_src), _ptr(g_tgt), _ptr(g_len), _ptr(g_vol), _ptr(g_ar), B, N,
                                                          voxel_shift, eps, n_points, _ptr(arange), int(align_corners),
@@ -565,8 +573,22 @@ class _TrilinearFunction(torch.autograd.Function):
                                                      _ptr(g_src), _ptr(g_tgt), _ptr(g_len), _ptr(g_vol), _ptr(g_ar), B, N,
                                                      voxel_shift, eps, n_points, _ptr(arange), int(align_corners), _stream()),
                            "b200drr_trilinear_bwd")
-        return (g_vol, None if g_src is None else g_src.view(src_shape), g_tgt,
-                None if g_len is None else g_len.view(img_shape), g_ar, None, None, None, None, None, None, None)
+        return (g_vol, *_ray_grads_back(ctx, g_src, g_tgt, g_len), g_ar, None, None, None, None, None, None, None)
+
+
+def _trilinear_sens_pose(volume, packed, src, G, Wd, rows, cols, voxel_shift, eps, n_points, arange):
+    """The sensitivities march of the in-kernel rays of a full detector grid through the packed-corner copy of `volume`
+    (include/b200drr.h: b200drr_trilinear_fwd_sens_pose): -> (out (B, H*W), sens (B, H*W, 12)), the image and every ray's
+    end-point and range sensitivities.  Inputs contiguous fp32."""
+    B, H, W = G.shape[0], rows.numel(), cols.numel()
+    out = torch.empty(B, H * W, dtype=torch.float32, device=packed.device)
+    sens = torch.empty(B, H * W, 12, dtype=torch.float32, device=packed.device)
+    fn, head, name = _vol_entry(_lib.load(), "b200drr_trilinear_fwd_sens_pose", volume, packed)
+    with torch.cuda.device(packed.device):
+        _lib.check(fn(*head, *volume.shape, _ptr(src), _ptr(G), _ptr(Wd), _ptr(rows), _ptr(cols), _ptr(out), _ptr(sens), B, H,
+                      W, voxel_shift, eps, n_points, _ptr(arange), _PACKED_SLAB_SENS if B >= _PACKED_SLAB_MIN_BATCH else 0,
+                      _stream()), name)
+    return out, sens
 
 
 class _TrilinearPoseFunction(torch.autograd.Function):
@@ -575,20 +597,12 @@ class _TrilinearPoseFunction(torch.autograd.Function):
     gradients come back as matrices + the two range partials, no (B,N,3) tensors exist."""
 
     @staticmethod
-    def forward(ctx, packed, dims, src, G, Wd, rows, cols, alpha_range, voxel_shift, eps, n_points, vol_dtype=torch.float32):
+    def forward(ctx, volume, packed, src, G, Wd, rows, cols, alpha_range, voxel_shift, eps, n_points):
         B, H, W = G.shape[0], rows.numel(), cols.numel()
         src, G, Wd = src.contiguous().float(), G.contiguous().float(), Wd.contiguous().float()
         rows, cols = rows.contiguous().float(), cols.contiguous().float()
         arange = alpha_range.detach().to(device=packed.device, dtype=torch.float32).contiguous()
-        out = torch.empty(B, H * W, dtype=torch.float32, device=packed.device)
-        sens = torch.empty(B, H * W, 12, dtype=torch.float32, device=packed.device)
-        with torch.cuda.device(packed.device):
-            lib, code = _lib.load(), _VOL16.get(vol_dtype)
-            fn = lib.b200drr_trilinear_fwd_sens_pose if code is None else lib.b200drr_trilinear_fwd_sens_pose_v16
-            head = (_ptr(packed),) if code is None else (_ptr(packed), code)
-            _lib.check(fn(*head, *dims, _ptr(src), _ptr(G), _ptr(Wd), _ptr(rows), _ptr(cols), _ptr(out), _ptr(sens), B, H, W,
-                          voxel_shift, eps, n_points, _ptr(arange), _PACKED_SLAB_SENS if B >= _PACKED_SLAB_MIN_BATCH else 0,
-                          _stream()), fn.__name__)
+        out, sens = _trilinear_sens_pose(volume, packed, src, G, Wd, rows, cols, voxel_shift, eps, n_points, arange)
         ctx.save_for_backward(sens, Wd, rows, cols)
         return out.view(B, 1, H * W)
 
@@ -607,7 +621,7 @@ class _TrilinearPoseFunction(torch.autograd.Function):
             _lib.check(_lib.load().b200drr_trilinear_bwd_sens_pose(_ptr(sens), _ptr(gout), _ptr(Wd), _ptr(rows), _ptr(cols),
                                                                    _ptr(g_src), _ptr(g_G), _ptr(g_Wd), _ptr(g_ar), B, H, W,
                                                                    _stream()), "b200drr_trilinear_bwd_sens_pose")
-        return None, None, g_src, g_G, g_Wd, None, None, g_ar, None, None, None, None
+        return None, None, g_src, g_G, g_Wd, None, None, g_ar, None, None, None
 
 
 def trilinear_pose_render(renderer, volume, packed, src, G, Wd, rows, cols, n_points):
@@ -617,8 +631,8 @@ def trilinear_pose_render(renderer, volume, packed, src, G, Wd, rows, cols, n_po
     if volume.dtype in _VOL16:
         _check_vol16(volume, src, G)
     alpha_range, _ = pose_alpha_range(renderer, volume, src, G, Wd, rows, cols)
-    return _TrilinearPoseFunction.apply(packed, tuple(volume.shape), src, G, Wd, rows, cols, alpha_range,
-                                        float(renderer.voxel_shift), float(renderer.eps), int(n_points), volume.dtype)
+    return _TrilinearPoseFunction.apply(volume, packed, src, G, Wd, rows, cols, alpha_range, float(renderer.voxel_shift),
+                                        float(renderer.eps), int(n_points))
 
 
 def pose_alpha_range(renderer, volume, src, G, Wd, rows, cols):
@@ -647,90 +661,6 @@ def pose_alpha_range(renderer, volume, src, G, Wd, rows, cols):
     return torch.stack([amin[0, 0, 0], amax[1, 0, 0]]), arg
 
 
-class _SiddonFunction64(torch.autograd.Function):
-    """fp64 Siddon (csrc/literal.cu; include/b200drr.h: b200drr_siddon_fwd_f64 / _bwd_f64): what `drr.to(torch.float64)` reaches in the
-    reference (drr.py:75).  mode="nearest"; reduce "max" is forward-only."""
-
-    @staticmethod
-    def forward(ctx, volume, source, target, img, voxel_shift, eps, reduce, align_corners, stop_grad):
-        B, N = _check_inputs(volume, source, target, img, torch.float64)
-        vol, src = volume.contiguous(), source.reshape(B, 3).contiguous()
-        tgt, raylen = target.contiguous(), img.reshape(B, N).contiguous()
-        out = torch.empty(B, N, dtype=torch.float64, device=vol.device)
-        with torch.cuda.device(vol.device):
-            _lib.check(_lib.load().b200drr_siddon_fwd_f64(_ptr(vol), *vol.shape, _ptr(src), _ptr(tgt), _ptr(raylen), _ptr(out), B, N,
-                                                          voxel_shift, eps, reduce, int(align_corners), _stream()),
-                       "b200drr_siddon_fwd_f64")
-        ctx.save_for_backward(vol, src, tgt, raylen)
-        ctx.cfg = (voxel_shift, eps, reduce, align_corners, stop_grad, tuple(source.shape), tuple(img.shape))
-        return out.view(B, 1, N)
-
-    @staticmethod
-    @once_differentiable
-    def backward(ctx, gout):
-        voxel_shift, eps, reduce, align_corners, stop_grad, src_shape, img_shape = ctx.cfg
-        if reduce != 0:
-            raise NotImplementedError("fp64 Siddon: backward is implemented for reducefn='sum'")
-        vol, src, tgt, raylen = ctx.saved_tensors
-        B, N = tgt.shape[0], tgt.shape[1]
-        need_vol, need_src, need_tgt, need_len = ctx.needs_input_grad[:4]
-        gout = gout.reshape(B, N).contiguous().double()
-        dev = vol.device
-        g_src = torch.empty(B, 3, dtype=torch.float64, device=dev) if need_src else None
-        g_tgt = torch.empty(B, N, 3, dtype=torch.float64, device=dev) if need_tgt else None
-        g_len = torch.empty(B, N, dtype=torch.float64, device=dev) if (need_len and not stop_grad) else None
-        g_vol = torch.zeros_like(vol) if (need_vol and not stop_grad) else None
-        with torch.cuda.device(dev):
-            _lib.check(_lib.load().b200drr_siddon_bwd_f64(_ptr(vol), *vol.shape, _ptr(src), _ptr(tgt), _ptr(raylen), _ptr(gout),
-                                                          _ptr(g_src), _ptr(g_tgt), _ptr(g_len), _ptr(g_vol), B, N, voxel_shift, eps,
-                                                          int(stop_grad), int(align_corners), _stream()), "b200drr_siddon_bwd_f64")
-        return (g_vol, None if g_src is None else g_src.view(src_shape), g_tgt,
-                None if g_len is None else g_len.view(img_shape), None, None, None, None, None)
-
-
-class _TrilinearFunction64(torch.autograd.Function):
-    """fp64 trilinear (b200drr_trilinear_fwd_f64 / _bwd_f64); alpha_range (2,) fp64 carries the batch-global range."""
-
-    @staticmethod
-    def forward(ctx, volume, source, target, img, alpha_range, voxel_shift, eps, n_points, reduce, align_corners):
-        B, N = _check_inputs(volume, source, target, img, torch.float64)
-        vol, src = volume.contiguous(), source.reshape(B, 3).contiguous()
-        tgt, raylen = target.contiguous(), img.reshape(B, N).contiguous()
-        arange = alpha_range.detach().to(device=vol.device, dtype=torch.float64).contiguous()
-        out = torch.empty(B, N, dtype=torch.float64, device=vol.device)
-        with torch.cuda.device(vol.device):
-            _lib.check(_lib.load().b200drr_trilinear_fwd_f64(_ptr(vol), *vol.shape, _ptr(src), _ptr(tgt), _ptr(raylen), _ptr(out), B,
-                                                             N, voxel_shift, eps, n_points, _ptr(arange), reduce,
-                                                             int(align_corners), _stream()), "b200drr_trilinear_fwd_f64")
-        ctx.save_for_backward(vol, src, tgt, raylen, arange)
-        ctx.cfg = (voxel_shift, eps, n_points, reduce, align_corners, tuple(source.shape), tuple(img.shape))
-        return out.view(B, 1, N)
-
-    @staticmethod
-    @once_differentiable
-    def backward(ctx, gout):
-        voxel_shift, eps, n_points, reduce, align_corners, src_shape, img_shape = ctx.cfg
-        if reduce != 0:
-            raise NotImplementedError("fp64 trilinear: backward is implemented for reducefn='sum'")
-        vol, src, tgt, raylen, arange = ctx.saved_tensors
-        B, N = tgt.shape[0], tgt.shape[1]
-        need_vol, need_src, need_tgt, need_len, need_ar = ctx.needs_input_grad[:5]
-        gout = gout.reshape(B, N).contiguous().double()
-        dev = vol.device
-        g_src = torch.empty(B, 3, dtype=torch.float64, device=dev) if need_src else None
-        g_tgt = torch.empty(B, N, 3, dtype=torch.float64, device=dev) if need_tgt else None
-        g_len = torch.empty(B, N, dtype=torch.float64, device=dev) if need_len else None
-        g_vol = torch.zeros_like(vol) if need_vol else None
-        g_ar = torch.zeros(2, dtype=torch.float64, device=dev) if need_ar else None
-        with torch.cuda.device(dev):
-            _lib.check(_lib.load().b200drr_trilinear_bwd_f64(_ptr(vol), *vol.shape, _ptr(src), _ptr(tgt), _ptr(raylen), _ptr(gout),
-                                                             _ptr(g_src), _ptr(g_tgt), _ptr(g_len), _ptr(g_vol), _ptr(g_ar), B, N,
-                                                             voxel_shift, eps, n_points, _ptr(arange), int(align_corners),
-                                                             _stream()), "b200drr_trilinear_bwd_f64")
-        return (g_vol, None if g_src is None else g_src.view(src_shape), g_tgt,
-                None if g_len is None else g_len.view(img_shape), g_ar, None, None, None, None, None)
-
-
 class _SegmentsFunction(torch.autograd.Function):
     """Un-reduced render for a CALLABLE `reducefn` (reference renderers.py:175-183 hands it the per-segment tensor):
     kind 0 = Siddon -> (B, N, D0+D1+D2+2) segments in the reference's sorted order, kind 1 = trilinear -> (B, N, n_points).
@@ -750,30 +680,27 @@ class _SegmentsFunction(torch.autograd.Function):
                                                         _ptr(raylen), _ptr(out), B, N, voxel_shift, eps, int(n_points),
                                                         _ptr(arange), int(align_corners), _stream()), "b200drr_segments_fwd")
         ctx.save_for_backward(vol, src, tgt, raylen, arange)
-        ctx.cfg = (kind, voxel_shift, eps, int(n_points), align_corners, stop_grad, tuple(source.shape), tuple(img.shape))
+        ctx.cfg = (kind, voxel_shift, eps, int(n_points), align_corners, stop_grad)
+        ctx.ray_shapes = (tuple(source.shape), tuple(img.shape))
         return out
 
     @staticmethod
     @once_differentiable
     def backward(ctx, gseg):
-        kind, voxel_shift, eps, n_points, align_corners, stop_grad, src_shape, img_shape = ctx.cfg
+        kind, voxel_shift, eps, n_points, align_corners, stop_grad = ctx.cfg
         vol, src, tgt, raylen, arange = ctx.saved_tensors
         B, N = tgt.shape[0], tgt.shape[1]
-        need_vol, need_src, need_tgt, need_len, need_ar = ctx.needs_input_grad[:5]
         dev, dtype = vol.device, vol.dtype
         gseg = gseg.to(dtype).contiguous()
-        g_src = torch.empty(B, 3, dtype=dtype, device=dev) if need_src else None
-        g_tgt = torch.empty(B, N, 3, dtype=dtype, device=dev) if need_tgt else None
-        g_len = torch.empty(B, N, dtype=dtype, device=dev) if (need_len and not stop_grad) else None
-        g_vol = torch.zeros_like(vol) if (need_vol and not stop_grad) else None
-        g_ar = torch.zeros(2, dtype=dtype, device=dev) if (need_ar and kind == 1) else None
+        g_src, g_tgt, g_len = _ray_grads(ctx, B, N, dtype, dev, stop_grad)
+        g_vol = torch.zeros_like(vol) if (ctx.needs_input_grad[0] and not stop_grad) else None
+        g_ar = torch.zeros(2, dtype=dtype, device=dev) if (ctx.needs_input_grad[4] and kind == 1) else None
         with torch.cuda.device(dev):
             _lib.check(_lib.load().b200drr_segments_bwd(kind, int(dtype == torch.float64), _ptr(vol), *vol.shape, _ptr(src), _ptr(tgt),
                                                         _ptr(raylen), _ptr(gseg), _ptr(g_src), _ptr(g_tgt), _ptr(g_len), _ptr(g_vol),
                                                         _ptr(g_ar), B, N, voxel_shift, eps, n_points, _ptr(arange), int(stop_grad),
                                                         int(align_corners), _stream()), "b200drr_segments_bwd")
-        return (g_vol, None if g_src is None else g_src.view(src_shape), g_tgt,
-                None if g_len is None else g_len.view(img_shape), g_ar, None, None, None, None, None, None)
+        return (g_vol, *_ray_grads_back(ctx, g_src, g_tgt, g_len), g_ar, None, None, None, None, None, None)
 
 
 def _mask_channels(mask: torch.Tensor) -> int:
@@ -818,22 +745,21 @@ class _MaskFunction(torch.autograd.Function):
                                                           _ptr(ar), int(align_corners), _stream()),
                            "b200drr_trilinear_fwd_mask")
         ctx.save_for_backward(vol, msk, src, tgt, raylen, ar)
-        ctx.cfg = (kind, voxel_shift, eps, n_points, align_corners, stop_grad, C, tuple(source.shape), tuple(img.shape), grid)
+        ctx.cfg = (kind, voxel_shift, eps, n_points, align_corners, stop_grad, C, grid)
+        ctx.ray_shapes = (tuple(source.shape), tuple(img.shape))
         return out
 
     @staticmethod
     @once_differentiable
     def backward(ctx, gout):
         vol, msk, src, tgt, raylen, ar = ctx.saved_tensors
-        kind, voxel_shift, eps, n_points, align_corners, stop_grad, C, src_shape, img_shape, grid = ctx.cfg
+        kind, voxel_shift, eps, n_points, align_corners, stop_grad, C, grid = ctx.cfg
         B, N = tgt.shape[0], tgt.shape[1]
-        need_vol, need_src, need_tgt, need_len, need_ar = ctx.needs_input_grad[:5]
+        need_ar = ctx.needs_input_grad[4]
         dev = vol.device
         gout = gout.reshape(B, C, N).contiguous().float()
-        g_src = torch.empty(B, 3, dtype=torch.float32, device=dev) if need_src else None
-        g_tgt = torch.empty(B, N, 3, dtype=torch.float32, device=dev) if need_tgt else None
-        g_len = torch.empty(B, N, dtype=torch.float32, device=dev) if (need_len and not stop_grad) else None
-        g_vol = torch.zeros_like(vol) if (need_vol and not stop_grad) else None
+        g_src, g_tgt, g_len = _ray_grads(ctx, B, N, torch.float32, dev, stop_grad)
+        g_vol = torch.zeros_like(vol) if (ctx.needs_input_grad[0] and not stop_grad) else None
         g_ar = None
         lib = _lib.load()
         with torch.cuda.device(dev):
@@ -860,8 +786,7 @@ class _MaskFunction(torch.autograd.Function):
                                                           _ptr(g_vol), _ptr(g_ar), B, N, C, voxel_shift, eps, int(n_points),
                                                           _ptr(ar), int(align_corners), _stream()),
                            "b200drr_trilinear_bwd_mask")
-        return (g_vol, None if g_src is None else g_src.view(src_shape), g_tgt,
-                None if g_len is None else g_len.view(img_shape), g_ar, None, None, None, None, None, None, None, None, None)
+        return (g_vol, *_ray_grads_back(ctx, g_src, g_tgt, g_len), g_ar, None, None, None, None, None, None, None, None, None)
 
 
 def _render_mask(kind, volume, mask, source, target, img, voxel_shift, eps, n_points=None, alpha_range=None,
@@ -944,23 +869,18 @@ class Siddon(torch.nn.Module):
         if volume.dtype == torch.float64:  # `drr.to(torch.float64)` (reference drr.py:75): the reference-literal fp64 kernels
             if mask is not None or self.mode != "nearest":
                 raise NotImplementedError("fp64 Siddon is implemented for mode='nearest' without mask_to_channels")
-            return _SiddonFunction64.apply(volume, source, target, img, float(self.voxel_shift), float(self.eps),
-                                           _reduce_code(self.reducefn), bool(align_corners),
-                                           bool(self.stop_gradients_through_grid_sample))
-        if mask is not None:
+        elif mask is not None:
             if align_corners or _reduce_code(self.reducefn) != 0:
                 raise NotImplementedError("mask_to_channels is implemented for reducefn='sum', align_corners=False")
             if self.mode != "nearest":
                 raise NotImplementedError("mask_to_channels is implemented for mode='nearest'")
             return _render_mask("siddon", volume, mask, source, target, img, float(self.voxel_shift), float(self.eps),
                                 stop_grad=self.stop_gradients_through_grid_sample, grid=self.detector_shape)
-        if self.mode == "bilinear":  # trilinear sampling at the segment midpoints: general walk (slow path)
-            return _SiddonBilinearFunction.apply(volume, source, target, img, float(self.voxel_shift), float(self.eps),
-                                                 _reduce_code(self.reducefn), bool(align_corners),
-                                                 bool(self.stop_gradients_through_grid_sample))
+        # mode="bilinear" (trilinear sampling at the segment midpoints) is the general walk's mode 1
         return _SiddonFunction.apply(volume, source, target, img, float(self.voxel_shift), float(self.eps),
                                      _reduce_code(self.reducefn), bool(align_corners),
-                                     bool(self.stop_gradients_through_grid_sample), self.detector_shape, self.ray_subset)
+                                     bool(self.stop_gradients_through_grid_sample), self.detector_shape, self.ray_subset,
+                                     int(self.mode == "bilinear"))
 
 
 def siddon_pose_render(renderer, volume, src, G, Wd, rows, cols):
@@ -1061,15 +981,12 @@ class Trilinear(torch.nn.Module):
             smp = _SegmentsFunction.apply(volume, source, target, img, alpha_range, 1, float(self.voxel_shift), float(self.eps),
                                           int(n_points), bool(align_corners), False)
             return self.reducefn(smp).unsqueeze(1)
-        if volume.dtype == torch.float64:  # `drr.to(torch.float64)`: reference-literal fp64 kernels
-            if mask is not None:
-                raise NotImplementedError("fp64 trilinear is implemented without mask_to_channels")
-            alpha_range = torch.stack([torch.as_tensor(alphamin, dtype=torch.float64, device=volume.device),
-                                       torch.as_tensor(alphamax, dtype=torch.float64, device=volume.device)])
-            return _TrilinearFunction64.apply(volume, source, target, img, alpha_range, float(self.voxel_shift), float(self.eps),
-                                              int(n_points), _reduce_code(self.reducefn), bool(align_corners))
-        alpha_range = torch.stack([torch.as_tensor(alphamin, dtype=torch.float32, device=volume.device),
-                                   torch.as_tensor(alphamax, dtype=torch.float32, device=volume.device)])
+        fp64 = volume.dtype == torch.float64  # `drr.to(torch.float64)`: reference-literal fp64 kernels
+        if fp64 and mask is not None:
+            raise NotImplementedError("fp64 trilinear is implemented without mask_to_channels")
+        dtype = torch.float64 if fp64 else torch.float32
+        alpha_range = torch.stack([torch.as_tensor(alphamin, dtype=dtype, device=volume.device),
+                                   torch.as_tensor(alphamax, dtype=dtype, device=volume.device)])
         if mask is not None:
             return _render_mask("trilinear", volume, mask, source, target, img, float(self.voxel_shift), float(self.eps),
                                 n_points=n_points, alpha_range=alpha_range, align_corners=align_corners,

@@ -95,6 +95,12 @@ _SIGNATURES = {
     "b200drr_trilinear_jac_sens_pose": (ctypes.c_int, [
         _c_float_p, _c_float_p, _c_float_p, _c_float_p, _c_float_p, _c_float_p, _c_float_p, _c_float_p, _c_float_p,
         ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_void_p]),
+    "b200drr_label_boxes": (ctypes.c_int, [
+        ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p]),
+    "b200drr_siddon_fwd_sens_structures": (ctypes.c_int, [
+        _c_float_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, _c_float_p, _c_float_p, _c_float_p, _c_float_p,
+        _c_float_p, ctypes.c_void_p, ctypes.c_void_p, _c_float_p, _c_float_p, ctypes.c_int, ctypes.c_int, ctypes.c_int,
+        ctypes.c_int, ctypes.c_float, ctypes.c_float, ctypes.c_void_p]),
     "b200drr_euler_pose_fwd": (ctypes.c_int, [
         _c_float_p, _c_float_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_float, _c_float_p, ctypes.c_int,
         ctypes.c_void_p]),
@@ -268,6 +274,10 @@ _SIGNATURES = {
         ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, _c_float_p, _c_float_p, _c_float_p, _c_float_p,
         _c_float_p, _c_float_p, _c_float_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_float, ctypes.c_float,
         ctypes.c_void_p]),
+    "b200drr_siddon_fwd_sens_structures_v16": (ctypes.c_int, [
+        ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, _c_float_p, _c_float_p,
+        _c_float_p, _c_float_p, _c_float_p, ctypes.c_void_p, ctypes.c_void_p, _c_float_p, _c_float_p, ctypes.c_int, ctypes.c_int,
+        ctypes.c_int, ctypes.c_int, ctypes.c_float, ctypes.c_float, ctypes.c_void_p]),
     "b200drr_pack_corners_v16": (ctypes.c_int, [
         ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p]),
     "b200drr_trilinear_fwd_v16": (ctypes.c_int, [

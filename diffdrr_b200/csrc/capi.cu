@@ -1,6 +1,8 @@
 // capi.cu -- the C ABI of libb200drr.so (see include/b200drr.h for the contract of every entry point).
 #include <cuda_runtime.h>
 
+#include <algorithm>
+
 #include "../../include/b200drr.h"
 #ifdef B200DRR_EXPERIMENTS
 #include "../../include/b200drr_experimental.h"
@@ -376,6 +378,27 @@ int b200drr_siddon_fwd_sens_pose(const float* vol, int D0, int D1, int D2, const
     if ((int64_t)D0 * D1 * D2 >= (int64_t)INT32_MAX) return B200DRR_EUNSUPPORTED;
     return ret(launch_siddon_fwd_sens_pose(vol, mk(D0, D1, D2), src, G, Wd, rows, cols, out, sens, B, H, W, voxel_shift, eps,
                                            (cudaStream_t)stream));
+}
+
+int b200drr_label_boxes(const uint8_t* labels, int D0, int D1, int D2, int32_t* boxes, void* stream)
+{
+    if (!labels || !boxes || bad_dims(D0, D1, D2)) return B200DRR_EINVAL;
+    if (too_big(D0, D1, D2)) return B200DRR_EUNSUPPORTED;
+    return ret(launch_label_boxes(labels, mk(D0, D1, D2), boxes, (cudaStream_t)stream));
+}
+
+int b200drr_siddon_fwd_sens_structures(const float* vol, const uint8_t* labels, int D0, int D1, int D2, const float* src,
+                                       const float* G, const float* Wd, const float* rows, const float* cols,
+                                       const int32_t* slot_of_label, const int32_t* box, float* out, float* sens, int B, int S,
+                                       int H, int W, float voxel_shift, float eps, void* stream)
+{
+    if (!vol || !labels || !src || !G || !Wd || !rows || !cols || !slot_of_label || !box || !out || bad_dims(D0, D1, D2) ||
+        S <= 0 || S > 256 || B <= 0 || bad_rays((int)std::min<int64_t>((int64_t)B * S, INT32_MAX), (int64_t)H * W) || H <= 0 ||
+        W <= 0)
+        return B200DRR_EINVAL;
+    if (too_big(D0, D1, D2)) return B200DRR_EUNSUPPORTED;
+    return ret(launch_siddon_fwd_sens_structures(vol, labels, mk(D0, D1, D2), src, G, Wd, rows, cols, slot_of_label, box, out, sens,
+                                                 B, S, H, W, voxel_shift, eps, (cudaStream_t)stream));
 }
 
 int b200drr_siddon_bwd_sens(const float* sens, const float* gout, float* g_src, float* g_tgt, float* g_raylen, int B,
@@ -789,6 +812,23 @@ int b200drr_siddon_fwd_sens_pose_v16(const void* vol, int vol_type, int D0, int 
         if (too_big(D0, D1, D2)) return (int)B200DRR_EUNSUPPORTED;
         return ret(launch_siddon_fwd_sens_pose((const V*)vol, mk(D0, D1, D2), src, G, Wd, rows, cols, out, sens, B, H, W,
                                                voxel_shift, eps, (cudaStream_t)stream));
+    });
+}
+
+int b200drr_siddon_fwd_sens_structures_v16(const void* vol, int vol_type, const uint8_t* labels, int D0, int D1, int D2,
+                                           const float* src, const float* G, const float* Wd, const float* rows, const float* cols,
+                                           const int32_t* slot_of_label, const int32_t* box, float* out, float* sens, int B,
+                                           int S, int H, int W, float voxel_shift, float eps, void* stream)
+{
+    if (!vol || !labels || !src || !G || !Wd || !rows || !cols || !slot_of_label || !box || !out || bad_dims(D0, D1, D2) ||
+        S <= 0 || S > 256 || B <= 0 || bad_rays((int)std::min<int64_t>((int64_t)B * S, INT32_MAX), (int64_t)H * W) || H <= 0 ||
+        W <= 0)
+        return B200DRR_EINVAL;
+    return with_vox16(vol_type, [&](auto v) {
+        using V = decltype(v);
+        if (too_big(D0, D1, D2)) return (int)B200DRR_EUNSUPPORTED;
+        return ret(launch_siddon_fwd_sens_structures((const V*)vol, labels, mk(D0, D1, D2), src, G, Wd, rows, cols, slot_of_label,
+                                                     box, out, sens, B, S, H, W, voxel_shift, eps, (cudaStream_t)stream));
     });
 }
 

@@ -188,6 +188,40 @@ B200_HD Ray load_ray(const float* src, const float* tgt, int b, int64_t r, float
 // alpha of plane i on axis a with the reference's own rounding sequence ((i - shift) - s) / d
 B200_HD float plane_alpha(const Ray& ray, int a, float i, float shift) { return ((i - shift) - ray.s[a]) / ray.d[a]; }
 
+// Optional in-kernel ray generation ("pose-in" entry points): when G != nullptr the rays of pose b are made from
+//   target_voxel(h, w) = G[b] . (cols[w], rows[h], 1, 1),   raylen(h, w) = | Wd[b] . (cols[w], rows[h], 1, 1) |
+// (G = affine_inverse . extrinsic . reorient . calibration, Wd = the same without affine_inverse and with the source
+// subtracted; reference detector.py:144-154 + drr.py:201-205 collapsed into two 3x4 matrices per pose), so the
+// (B, N, 3) target tensor and the ray-length image never exist in HBM.
+struct PoseRays {
+    const float* G;     // [B][3][4]
+    const float* Wd;    // [B][3][4]
+    const float* rows;  // [H]  canonical detector y of image row h   (detector.py:114-126)
+    const float* cols;  // [W]  canonical detector x of image column w
+};
+
+// The pose-in ray of pixel (px, py) of pose b and its length L (host+device: tests/hostemu builds this same source).
+B200_HD Ray pose_ray(const float* G, const float* Wd, const float* rows, const float* cols, const float* src, int b, int px, int py,
+                     float eps, float& L)
+{
+    const float c = ldg(cols + px), rr = ldg(rows + py);
+    const float* g = G + b * 12;
+    const float* wd = Wd + b * 12;
+    Ray ray;
+    float l2 = 0.0f;
+#pragma unroll
+    for (int a = 0; a < 3; ++a) {
+        const float t = fmaf(ldg(g + a * 4), c, fmaf(ldg(g + a * 4 + 1), rr, ldg(g + a * 4 + 2) + ldg(g + a * 4 + 3)));
+        const float dw = fmaf(ldg(wd + a * 4), c, fmaf(ldg(wd + a * 4 + 1), rr, ldg(wd + a * 4 + 2) + ldg(wd + a * 4 + 3)));
+        l2 = fmaf(dw, dw, l2);
+        ray.s[a] = ldg(src + b * 3 + a);
+        ray.d[a] = (t - ray.s[a]) + eps;
+        ray.inv[a] = 1.0f / ray.d[a];
+    }
+    L = sqrtf(l2);
+    return ray;
+}
+
 #if defined(__CUDACC__)
 __device__ __forceinline__ float warp_sum(float v)
 {
@@ -231,18 +265,6 @@ inline dim3 tiled_ray_grid(int B, int64_t N, int W)
     return dim3((unsigned)(((W + 15) / 16) * ((H + 7) / 8)), (unsigned)B, 1);
 }
 
-// Optional in-kernel ray generation ("pose-in" entry points): when G != nullptr the rays of pose b are made from
-//   target_voxel(h, w) = G[b] . (cols[w], rows[h], 1, 1),   raylen(h, w) = | Wd[b] . (cols[w], rows[h], 1, 1) |
-// (G = affine_inverse . extrinsic . reorient . calibration, Wd = the same without affine_inverse and with the source
-// subtracted; reference detector.py:144-154 + drr.py:201-205 collapsed into two 3x4 matrices per pose), so the
-// (B, N, 3) target tensor and the ray-length image never exist in HBM.
-struct PoseRays {
-    const float* G;     // [B][3][4]
-    const float* Wd;    // [B][3][4]
-    const float* rows;  // [H]  canonical detector y of image row h   (detector.py:114-126)
-    const float* cols;  // [W]  canonical detector x of image column w
-};
-
 __device__ __forceinline__ Ray make_ray(const PoseRays& pr, const float* __restrict__ src, const float* __restrict__ tgt,
                                         const float* __restrict__ raylen, int b, int64_t r, int px, int py, float eps,
                                         float& L)
@@ -251,22 +273,7 @@ __device__ __forceinline__ Ray make_ray(const PoseRays& pr, const float* __restr
         L = __ldg(raylen + r);
         return load_ray(src, tgt, b, r, eps);
     }
-    const float c = __ldg(pr.cols + px), rr = __ldg(pr.rows + py);
-    const float* g = pr.G + b * 12;
-    const float* wd = pr.Wd + b * 12;
-    Ray ray;
-    float l2 = 0.0f;
-#pragma unroll
-    for (int a = 0; a < 3; ++a) {
-        const float t = fmaf(__ldg(g + a * 4), c, fmaf(__ldg(g + a * 4 + 1), rr, __ldg(g + a * 4 + 2) + __ldg(g + a * 4 + 3)));
-        const float dw = fmaf(__ldg(wd + a * 4), c, fmaf(__ldg(wd + a * 4 + 1), rr, __ldg(wd + a * 4 + 2) + __ldg(wd + a * 4 + 3)));
-        l2 = fmaf(dw, dw, l2);
-        ray.s[a] = __ldg(src + b * 3 + a);
-        ray.d[a] = (t - ray.s[a]) + eps;
-        ray.inv[a] = 1.0f / ray.d[a];
-    }
-    L = sqrtf(l2);
-    return ray;
+    return pose_ray(pr.G, pr.Wd, pr.rows, pr.cols, src, b, px, py, eps, L);
 }
 #endif
 

@@ -66,6 +66,13 @@ cudaError_t launch_siddon_fwd_sens_pose(const V* vol, VolDims dims, const float*
                                         float shift, float eps, cudaStream_t stream);
 cudaError_t launch_siddon_bwd_sens(const float* sens, const float* gout, float* g_src, float* g_tgt, float* g_raylen,
                                    int B, int64_t N, int stop_grad, cudaStream_t stream);
+// piecewise-rigid renders (structures.cu): label boxes, and one gated pose-in walk per (pixel, pose, slot); sens may be NULL
+cudaError_t launch_label_boxes(const uint8_t* labels, VolDims dims, int32_t* boxes, cudaStream_t stream);
+template <class V>
+cudaError_t launch_siddon_fwd_sens_structures(const V* vol, const uint8_t* labels, VolDims dims, const float* src, const float* G,
+                                              const float* Wd, const float* rows, const float* cols, const int32_t* slot_of_label,
+                                              const int32_t* box, float* out, float* sens, int B, int S, int H, int W, float shift,
+                                              float eps, cudaStream_t stream);
 cudaError_t launch_siddon_bwd_sens_pose(const float* sens, const float* gout, const float* Wd, const float* rows,
                                         const float* cols, float* g_src, float* g_G, float* g_Wd, int B, int H, int W,
                                         int stop_grad, cudaStream_t stream);

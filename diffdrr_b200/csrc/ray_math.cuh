@@ -654,10 +654,24 @@ B200_HD void lean_init(const Walk& w, int st0, int st1, int st2, LeanState& s, L
     s.off = w.idx[0] * st0 + w.idx[1] * st1 + w.idx[2] * st2;
 }
 
+// How the walks fetch their voxels: one scalar load per visit from the volume as stored (production), or -- EXPERIMENT, see
+// siddon_ray_lean_box_chunk -- W-voxel chunks from a major-axis-fastest copy, re-used across visits (LoadChunk below), or only
+// the voxels of one labelled structure (LoadGated, structures_math.cuh).
+struct LoadPlain {
+    template <int U, class V>
+    B200_HD void batch(const V* vol, const int (&offs)[U], float (&v)[U])
+    {
+#pragma unroll
+        for (int j = 0; j < U; ++j) v[j] = ldg(vol + offs[j]);
+    }
+    template <class V>
+    B200_HD float at(const V* vol, int off) const { return ldg(vol + off); }
+};
+
 // Lean walk over the sub-box [lo, hi) of a volume whose element strides are (st0, st1, st2).
-template <int U, class V = float>
+template <int U, class V = float, class Load = LoadPlain>
 B200_HD float siddon_ray_lean_box(const V* vol, const int lo_v[3], const int hi_v[3], int st0, int st1, int st2,
-                                  const Ray& ray, float shift)
+                                  const Ray& ray, float shift, Load loader = Load())
 {
     const Walk w = start_walk_box(ray, lo_v, hi_v, shift);
     if (!w.hit) return 0.0f;
@@ -673,8 +687,7 @@ B200_HD float siddon_ray_lean_box(const V* vol, const int lo_v[3], const int hi_
             offs[j] = s.off;
             len[j] = lean_step(s, k);
         }
-#pragma unroll
-        for (int j = 0; j < U; ++j) v[j] = ldg(vol + offs[j]);
+        loader.template batch<U>(vol, offs, v);
 #pragma unroll
         for (int j = 0; j < U; ++j) acc = fmaf(len[j], v[j], acc);
     }
@@ -999,19 +1012,6 @@ B200_HD void minor_accumulate(int ax, float coef, float alpha, float& Au, float&
     if (ax == 1) { Av = fmaf(coef, alpha, Av); Cv += coef; }
 #endif
 }
-
-// How the sensitivities walk fetches its voxels: one scalar load per visit from the volume as stored (production), or --
-// EXPERIMENT, see siddon_ray_lean_box_chunk -- W-voxel chunks from a major-axis-fastest copy, re-used across visits.
-struct LoadPlain {
-    template <int U, class V>
-    B200_HD void batch(const V* vol, const int (&offs)[U], float (&v)[U])
-    {
-#pragma unroll
-        for (int j = 0; j < U; ++j) v[j] = ldg(vol + offs[j]);
-    }
-    template <class V>
-    B200_HD float at(const V* vol, int off) const { return ldg(vol + off); }
-};
 
 template <int W>
 struct LoadChunk {

@@ -170,6 +170,23 @@ class DRR(nn.Module):
         return drr_jacobian(self, *args, parameterization=parameterization, convention=convention, degrees=degrees,
                             calibration=calibration, n_points=n_points, return_range_terms=return_range_terms)
 
+    def render_structures(self, *args, motions, labels, parameterization: str = None, convention: str = None,
+                          degrees: bool = False, calibration: RigidTransform = None, background: bool = True, **kwargs):
+        """Piecewise-rigid DRR (DESIGN.md 6f) -> (B, K + 1, H, W), or (B, K, H, W) with background=False.
+
+        Channel k renders the voxels of `self.mask` labelled labels[k], moved by the rigid world motion motions[..., k, :, :]
+        (x -> X x), with the camera pose `*args` (meaning as in forward); the last channel renders every other voxel, label 0
+        included, with the camera pose alone.  motions: (K, 4, 4) shared by every pose, or (B, K, 4, 4), fp32 on the density's
+        device (a tensor or a RigidTransform; it may require grad).  labels: K distinct integers 0..255 present in the mask.
+        With identity motions the channels sum to forward(*args).  Gradients reach the camera pose, the calibration and the
+        motions; the density must not require grad.  Supported: Siddon with default options (stop_gradients_through_grid_sample
+        honoured), fp32 / fp16 / bf16 densities, the full detector; anything else raises before any launch."""
+        from .structures import render_structures
+
+        return render_structures(self, *args, motions=motions, labels=labels, parameterization=parameterization,
+                                 convention=convention, degrees=degrees, calibration=calibration, background=background,
+                                 **kwargs)
+
     # ---- fused pose-in path (SURVEY.md 8f-2) ------------------------------------------------------------------
     def _pose_in_ok(self, mask_to_channels, kwargs) -> bool:
         """True when the whole pose -> rays -> Siddon chain can run as ONE kernel with in-kernel ray generation."""
@@ -307,6 +324,7 @@ class DRR(nn.Module):
         out = super()._apply(fn, *args, **kwargs)  # .to(device) / .float() / ... replace the buffers
         object.__setattr__(self, "_pose_consts", None)
         object.__setattr__(self, "_grid_axes_cache", None)
+        object.__setattr__(self, "_structures_cache", None)  # the label copy and label boxes of render_structures
         return out
 
     def rescale_detector_(self, scale: float):

@@ -293,6 +293,25 @@ int b200drr_trilinear_jac_sens_pose(const float *sens, const float *dsrc, const 
                                     int P, void *stream);
 
 /*
+ * Piecewise-rigid renders (DESIGN.md 6f): every labelled structure of the CT under its own pose, in one launch.
+ *   b200drr_label_boxes: one pass over the label volume labels [D0][D1][D2] (uint8) -> boxes [256][6] int32 (overwritten), the
+ *     voxel-index box {lo0, lo1, lo2, hi0, hi1, hi2} = [lo, hi) of every label 0..255; an absent label gets lo > hi.
+ *   b200drr_siddon_fwd_sens_structures: S slots per pose.  Slot s of pose b renders the voxels whose label l has
+ *     slot_of_label[l] == s (slot_of_label [256] int32, -1 = no slot) with the pose-in rays of src [B*S][3], G, Wd [B*S][3][4]
+ *     (index b*S + s; rows [H], cols [W] as in b200drr_siddon_fwd_pose), walking only the box box[s] ([S][6] as above; it must
+ *     contain every voxel of the slot's labels).  out [B][S][H*W] and sens [B][S][H*W][8] (layout of b200drr_siddon_fwd_sens_pose,
+ *     so b200drr_siddon_bwd_sens_pose with batch B*S is the backward) are overwritten; sens = NULL renders the image only.
+ *     Equal, to fp32 round-off, to b200drr_siddon_fwd_sens_pose of the density times (label in slot s).  Pixels outside the
+ *     detector rectangle that covers the projection of box[s] (one-pixel margin; the whole detector when the box reaches the
+ *     source plane) are written as zeros without a walk.  No atomics on the outputs.  1 <= S <= 256, B*S <= 65535.
+ */
+int b200drr_label_boxes(const uint8_t *labels, int D0, int D1, int D2, int32_t *boxes, void *stream);
+int b200drr_siddon_fwd_sens_structures(const float *vol, const uint8_t *labels, int D0, int D1, int D2, const float *src,
+                                       const float *G, const float *Wd, const float *rows, const float *cols,
+                                       const int32_t *slot_of_label, const int32_t *box, float *out, float *sens, int B, int S,
+                                       int H, int W, float voxel_shift, float eps, void *stream);
+
+/*
  * mask_to_channels forward (reference renderers.py:77-89 and 242-252): `mask` is the label volume [D0][D1][D2] stored
  * as fp32 (as DRR registers it, drr.py:86-91); every segment / sample contributes to channel label(voxel), sampled
  * nearest with zero padding.  out [B][C][N] is overwritten.  Siddon: reduce="sum", align_corners=0.
@@ -606,6 +625,10 @@ int b200drr_siddon_fwd_pose_v16(const void *vol, int vol_type, int D0, int D1, i
 int b200drr_siddon_fwd_sens_pose_v16(const void *vol, int vol_type, int D0, int D1, int D2, const float *src, const float *G,
                                      const float *Wd, const float *rows, const float *cols, float *out, float *sens, int B, int H,
                                      int W, float voxel_shift, float eps, void *stream);
+int b200drr_siddon_fwd_sens_structures_v16(const void *vol, int vol_type, const uint8_t *labels, int D0, int D1, int D2,
+                                           const float *src, const float *G, const float *Wd, const float *rows, const float *cols,
+                                           const int32_t *slot_of_label, const int32_t *box, float *out, float *sens, int B,
+                                           int S, int H, int W, float voxel_shift, float eps, void *stream);
 
 /*
  * 16-bit volumes, Trilinear (DESIGN.md 4.5): twins of the trilinear entry points with the same fp32 arguments after vol_type.

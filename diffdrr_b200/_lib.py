@@ -227,6 +227,14 @@ _SIGNATURES = {
         _c_float_p, _c_float_p, _c_float_p, ctypes.c_int64, ctypes.c_int64, ctypes.c_int64, ctypes.c_int64, ctypes.c_int,
         ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_double, ctypes.c_double, ctypes.c_void_p,
         ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p]),
+    "b200drr_structure_footprints": (ctypes.c_int, [
+        _c_float_p, _c_float_p, _c_float_p, _c_float_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int,
+        ctypes.c_int, ctypes.c_float, ctypes.c_void_p]),
+    "b200drr_ncc_normal_structures_workspace_bytes": (ctypes.c_int64, [ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int]),
+    "b200drr_ncc_normal_structures": (ctypes.c_int, [
+        _c_float_p, _c_float_p, ctypes.c_int, _c_float_p, ctypes.c_int64, ctypes.c_int64, ctypes.c_int64, ctypes.c_int64,
+        ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_double, ctypes.c_double,
+        ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p]),
     "b200drr_sobel_workspace_bytes": (ctypes.c_int64, [ctypes.c_int, ctypes.c_int, ctypes.c_int]),
     "b200drr_sobel_fwd": (ctypes.c_int, [
         _c_float_p, _c_float_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, _c_float_p, ctypes.c_int, ctypes.c_void_p]),

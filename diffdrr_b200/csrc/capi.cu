@@ -1073,6 +1073,37 @@ int b200drr_ncc_normal(const float* x, const float* t, const float* J, int64_t s
     return ret(launch_ncc_normal(x, t, J, sJb, sJc, sJk, sJn, B, C, H, W, p, P, eps, weight, workspace, A, g, (cudaStream_t)stream));
 }
 
+int b200drr_structure_footprints(const float* src, const float* G, const float* rows, const float* cols, const int32_t* box,
+                                 int32_t* rects, int B, int S, int H, int W, float voxel_shift, void* stream)
+{
+    if (!src || !G || !rows || !cols || !box || !rects || B <= 0 || S <= 0 || S > 256 || (int64_t)B * S > INT32_MAX || H <= 0 ||
+        W <= 0)
+        return B200DRR_EINVAL;
+    return ret(launch_structure_footprints(src, G, rows, cols, box, rects, B, S, H, W, voxel_shift, (cudaStream_t)stream));
+}
+
+static bool bad_ncc_normal_structures(int B, int K, int H, int W)
+{
+    return B <= 0 || B > 65535 || K < 1 || K > 255 || H <= 0 || W <= 0;
+}
+
+int64_t b200drr_ncc_normal_structures_workspace_bytes(int B, int K, int H, int W)
+{
+    if (bad_ncc_normal_structures(B, K, H, W)) return 0;
+    return ncc_normal_structures_workspace_bytes(B, K, H);
+}
+
+int b200drr_ncc_normal_structures(const float* x, const float* t, int t_batch, const float* J, int64_t sJb, int64_t sJs, int64_t sJn,
+                                  int64_t sJk, const int32_t* rects, int B, int K, int S, int H, int W, double eps, double weight,
+                                  void* workspace, double* A, double* g, void* stream)
+{
+    if (!x || !t || !J || !rects || !workspace || !A || !g || sJb < 0 || sJs < 0 || sJn < 0 || sJk < 0 || !(eps >= 0.0) ||
+        bad_ncc_normal_structures(B, K, H, W) || S < K || S > 256 || (t_batch != 1 && t_batch != B))
+        return B200DRR_EINVAL;
+    return ret(launch_ncc_normal_structures(x, t, t_batch, J, sJb, sJs, sJn, sJk, rects, B, K, S, H, W, eps, weight, workspace, A, g,
+                                            (cudaStream_t)stream));
+}
+
 // odd kernel size, blur radius below both image sides (reflect padding), shared-memory tiles that fit
 static bool bad_sobel(int B, int H, int W, int ksize)
 {

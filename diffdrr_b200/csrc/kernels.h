@@ -256,6 +256,15 @@ cudaError_t launch_ncc_normal(const float* x, const float* t, const float* J, in
                               int C, int H, int W, int p, int P, double eps, double weight, void* workspace, double* A, double* g,
                               cudaStream_t stream);
 
+// global-NCC normal equations of a piecewise-rigid composite, block-sparse over the structures' footprints, and the footprints
+// themselves (ncc_normal_structures.cu)
+cudaError_t launch_structure_footprints(const float* src, const float* G, const float* rows, const float* cols, const int32_t* box,
+                                        int32_t* rects, int B, int S, int H, int W, float shift, cudaStream_t stream);
+int64_t ncc_normal_structures_workspace_bytes(int B, int K, int H);
+cudaError_t launch_ncc_normal_structures(const float* x, const float* t, int t_batch, const float* J, int64_t sb, int64_t ss,
+                                         int64_t sn, int64_t sk, const int32_t* rects, int B, int K, int S, int H, int W, double eps,
+                                         double weight, void* workspace, double* A, double* g, cudaStream_t stream);
+
 // blur + Sobel front end of the gradient NCC (sobel.cu)
 int64_t sobel_workspace_bytes(int B, int H, int W);
 bool sobel_kernel_fits(int k);

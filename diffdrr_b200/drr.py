@@ -187,6 +187,23 @@ class DRR(nn.Module):
                                  convention=convention, degrees=degrees, calibration=calibration, background=background,
                                  **kwargs)
 
+    def structures_jacobian(self, *args, motions, labels, parameterization: str = None, convention: str = None,
+                            degrees: bool = False, calibration: RigidTransform = None, background: bool = True, stop_grad=None,
+                            **kwargs):
+        """(img, J): the render_structures image (B, S, H, W) and the per-pixel Jacobian J (B, K, H, W, 6) of channel k with
+        respect to the increment xi_k = (omega, v) of structure k's motion (DESIGN.md 6g).  Only channel k depends on motion k,
+        so J[:, k] is also the derivative of the composite img.sum(1).  xi_k is a left increment about the structure's pivot c_k,
+        in world coordinates: X_k(xi) = T(c_k) exp(xi^) T(-c_k) X_k; c_k is the world position of the centre of label k's box
+        (structures.structure_pivots).  Columns: the rotation's three, then the translation's three.  Arguments as in
+        render_structures; stop_grad drops Siddon's ray-length term (None = the renderer's
+        stop_gradients_through_grid_sample).  The same set as render_structures is supported, anything else raises before any
+        launch.  Detached results; no host sync once the label tables are cached."""
+        from .structures import structures_jacobian
+
+        return structures_jacobian(self, *args, motions=motions, labels=labels, parameterization=parameterization,
+                                   convention=convention, degrees=degrees, calibration=calibration, background=background,
+                                   stop_grad=stop_grad, **kwargs)
+
     # ---- fused pose-in path (SURVEY.md 8f-2) ------------------------------------------------------------------
     def _pose_in_ok(self, mask_to_channels, kwargs) -> bool:
         """True when the whole pose -> rays -> Siddon chain can run as ONE kernel with in-kernel ray generation."""

@@ -163,3 +163,122 @@ class LevenbergMarquardt:
             xyz.copy_(torch.where(accept[:, None], xyz_t, xyz))
             self.damping = torch.where(accept, self.damping / 10.0, self.damping * 10.0).clamp(1e-12, 1e12)
             return torch.where(accept, trial, loss)
+
+
+def ncc_normal_structures_equations(x, t, J, rects, eps, weight, A, g):
+    """A += weight * sum_q Jz_q Jz_q^T, g += weight * sum_q Jz_q r_q of the global NCC between the composite x (B, H, W) and the
+    target t (1 or B, H, W) (fp32 CUDA, contiguous), for the motions of K structures, through b200drr_ncc_normal_structures
+    (csrc/ncc_normal_structures.cu).  J: DRR.structures_jacobian's (B, K, H, W, 6) (or (B, K, H*W, 6)) view; rects (B, S, 4)
+    int32 its footprints; A (B, 6K, 6K) and g (B, 6K) float64 (DESIGN.md 6g)."""
+    from . import _lib
+    B, H, W = x.shape
+    K, S = J.shape[1], rects.shape[1]
+    sn = J.stride(-2)
+    if (J.shape[0] != B or J.shape[-1] != 6 or J[0, 0, ..., 0].numel() != H * W or (J.dim() == 5 and J.stride(2) != W * sn)
+            or tuple(rects.shape) != (B, S, 4) or S < K or tuple(A.shape) != (B, 6 * K, 6 * K) or tuple(g.shape) != (B, 6 * K)):
+        raise ValueError(f"ncc_normal_structures_equations: J {tuple(J.shape)} must be (B, K, H, W, 6) or (B, K, H*W, 6) with "
+                         f"evenly strided pixels, rects (B, S >= K, 4), A (B, 6K, 6K) and g (B, 6K) for x {tuple(x.shape)}; got "
+                         f"rects {tuple(rects.shape)}, A {tuple(A.shape)}, g {tuple(g.shape)}")
+    lib = _lib.load()
+    ws = torch.empty(max(int(lib.b200drr_ncc_normal_structures_workspace_bytes(B, K, H, W)) // 8, 1), dtype=torch.float64,
+                     device=x.device)
+    _lib.check(lib.b200drr_ncc_normal_structures(x.data_ptr(), t.data_ptr(), t.shape[0], J.data_ptr(), J.stride(0), J.stride(1), sn,
+                                                 J.stride(-1), rects.data_ptr(), B, K, S, H, W, float(eps), float(weight),
+                                                 ws.data_ptr(), A.data_ptr(), g.data_ptr(),
+                                                 torch.cuda.current_stream(x.device).cuda_stream), "b200drr_ncc_normal_structures")
+
+
+class StructuresLevenbergMarquardt:
+    """Levenberg-Marquardt registration of the K structures of a piecewise-rigid DRR (DRR.render_structures) towards `target`
+    on the global NCC of the composite image (the sum of the channels), with the camera pose fixed (DESIGN.md 6g).
+
+    The unknowns are the motions: `motions` (K, 4, 4), shared by the B views, or (B, K, 4, 4), one set per pose; a tensor or a
+    Parameter, fp32 on the density's device, updated in place by step().  Each step takes one DRR.structures_jacobian (the full
+    derivative of the image, whatever the renderer's stop_gradients_through_grid_sample), forms the Gauss-Newton system of the
+    z-normalised residual block by block over the structures' footprints (b200drr_ncc_normal_structures), solves
+    (A + lambda diag A) delta = -g in float64, and renders one trial image.  delta_k = (omega, v) moves structure k as
+        X_k <- T(c_k) exp(delta_k^) T(-c_k) X_k
+    (a left increment about the pivot c_k, the world centre of label k's box, structures.structure_pivots; exp is the matrix
+    exponential of the twist, not pose.se3_exp_map's transposed convention).  The trial is kept if its true loss is lower
+    (lambda / 10 on accept, x 10 on reject).  Shared motions: one system, the mean over the views of the per-view systems,
+    modelling the mean of 1 - NCC, and one decision per step on that mean.  Per-pose motions: B independent systems and
+    decisions.  No host sync.
+
+    Only the global NCC is modelled: `loss` None (NormalizedCrossCorrelation2d(eps=eps)) or a NormalizedCrossCorrelation2d
+    without patch_size; anything else raises TypeError here."""
+
+    def __init__(self, drr, rot: torch.Tensor, xyz: torch.Tensor, motions: torch.Tensor, labels, target: torch.Tensor,
+                 parameterization: str = "euler_angles", convention: str | None = None, degrees: bool = False, calibration=None,
+                 background: bool = True, loss=None, damping: float = 1e-3, eps: float = 1e-5):
+        from .metrics import NormalizedCrossCorrelation2d
+        from .structures import _batch_size, _label_tuple, check_supported, structure_pivots
+
+        if loss is None:
+            loss = NormalizedCrossCorrelation2d(eps=eps)
+        elif type(loss) is not NormalizedCrossCorrelation2d or loss.patch_size is not None:
+            raise TypeError(f"StructuresLevenbergMarquardt models the global NCC only: NormalizedCrossCorrelation2d without "
+                            f"patch_size (or loss=None), not {type(loss).__name__}"
+                            f"{'' if getattr(loss, 'patch_size', None) is None else f'(patch_size={loss.patch_size})'}; patch-wise, "
+                            f"multiscale and gradient NCC have no block-sparse system here (use a first-order optimizer)")
+        if not torch.is_tensor(motions) or motions.dim() not in (3, 4):
+            raise ValueError(f"motions must be a (K, 4, 4) or (B, K, 4, 4) tensor updated in place, got "
+                             f"{tuple(motions.shape) if torch.is_tensor(motions) else type(motions).__name__}")
+        if not torch.is_tensor(target) or target.dim() != 4 or target.shape[1] != 1:
+            raise ValueError(f"StructuresLevenbergMarquardt takes a one-channel target image (B, 1, H, W) of the composite, got "
+                             f"{tuple(target.shape) if torch.is_tensor(target) else type(target).__name__}")
+        det = drr.detector
+        if tuple(target.shape[-2:]) != (det.height, det.width):
+            raise ValueError(f"the target {tuple(target.shape)} does not match the {det.height} x {det.width} detector")
+        B = _batch_size((rot, xyz), parameterization)
+        if target.shape[0] not in (1, B):
+            raise ValueError(f"the target's batch ({target.shape[0]}) must be 1 or the number of poses ({B})")
+        labels, _, B = check_supported(drr, (rot, xyz), parameterization, motions, _label_tuple(labels), {})
+        if not (target.is_cuda and target.dtype == torch.float32):
+            raise ValueError("StructuresLevenbergMarquardt's normal equations run on the GPU: the target must be a CUDA fp32 tensor")
+        self.drr, self.rot, self.xyz, self.motions, self.labels = drr, rot.detach(), xyz.detach(), motions, labels
+        self.kw = dict(parameterization=parameterization, convention=convention, degrees=degrees, calibration=calibration,
+                       background=background)
+        self.loss, self.eps = loss, float(loss.eps)
+        self.shared = motions.dim() == 3
+        self.target = target.detach().expand(B, 1, det.height, det.width).contiguous()
+        self._t = self.target[:, 0]
+        self.pivots = structure_pivots(drr, labels)
+        self.damping = torch.full((1 if self.shared else B,), float(damping), dtype=torch.float64, device=motions.device)
+
+    def _loss(self, img):
+        """(B,) 1 - NCC of the composite of each view."""
+        return 1.0 - self.loss(self.target, img.sum(1, keepdim=True))
+
+    def normal_equations(self, img, J, rects):
+        """(A (B, 6K, 6K), g (B, 6K)) float64 of each view's Gauss-Newton model of 1 - NCC (weight 1 / (H W)) at the image `img`
+        (B, S, H, W) with Jacobian J (B, K, H, W, 6) and footprints rects (B, S, 4)."""
+        B, K, H, W = img.shape[0], J.shape[1], self._t.shape[-2], self._t.shape[-1]
+        x = img.sum(1).reshape(B, H, W).contiguous()
+        A = torch.zeros(B, 6 * K, 6 * K, dtype=torch.float64, device=img.device)
+        g = torch.zeros(B, 6 * K, dtype=torch.float64, device=img.device)
+        ncc_normal_structures_equations(x, self._t, J, rects, self.eps, 1.0 / (H * W), A, g)
+        return A, g
+
+    def step(self) -> torch.Tensor:
+        """One damped Gauss-Newton step; -> the loss after it: the mean over the views of 1 - NCC (a 0-d tensor) for shared
+        motions, the per-pose (B,) losses otherwise."""
+        from .structures import apply_increments, render_structures, structures_jacobian
+
+        X, drr = self.motions, self.drr
+        with torch.no_grad():
+            img, J, rects = structures_jacobian(drr, self.rot, self.xyz, motions=X, labels=self.labels, stop_grad=False,
+                                                return_footprints=True, **self.kw)
+            A, g = self.normal_equations(img, J, rects)
+            if self.shared:
+                A, g = A.mean(0, keepdim=True), g.mean(0, keepdim=True)
+            D = torch.diag_embed(torch.diagonal(A, dim1=-2, dim2=-1).clamp_min(1e-12))
+            delta = torch.linalg.solve_ex(A + self.damping[:, None, None] * D, -g.unsqueeze(-1))[0].squeeze(-1)
+            X_t = apply_increments(X.detach(), delta.reshape(*X.shape[:-2], 6), self.pivots)   # (..., K, 6): (omega, v) per k
+            loss = self._loss(img)
+            trial = self._loss(render_structures(drr, self.rot, self.xyz, motions=X_t, labels=self.labels, **self.kw))
+            if self.shared:
+                loss, trial = loss.mean(), trial.mean()
+            accept = trial < loss  # a NaN trial is rejected
+            X.copy_(torch.where(accept.reshape(-1, *[1] * (X.dim() - 1)), X_t, X))
+            self.damping = torch.where(accept, self.damping / 10.0, self.damping * 10.0).clamp(1e-12, 1e12)
+            return torch.where(accept, trial, loss)

@@ -153,23 +153,30 @@ def check_supported(drr, args, parameterization, motions, labels, kwargs):
     return labels, X, B
 
 
+def _structures_walk(vol, labels, src, G, Wd, rows, cols, slot_of_label, box, S, voxel_shift, eps, want_sens):
+    """The one launch site of b200drr_siddon_fwd_sens_structures: -> (out (B, S, H*W), sens (B, S, H*W, 8) or None for the
+    image-only walk).  vol contiguous; src, G, Wd, rows, cols contiguous fp32."""
+    BS, H, W = G.shape[0], rows.numel(), cols.numel()
+    B = BS // S
+    out = torch.empty(B, S, H * W, dtype=torch.float32, device=vol.device)
+    sens = torch.empty(B, S, H * W, 8, dtype=torch.float32, device=vol.device) if want_sens else None
+    fn, head, name = _vol_entry(_lib.load(), "b200drr_siddon_fwd_sens_structures", vol)
+    with torch.cuda.device(vol.device):
+        _lib.check(fn(*head, _ptr(labels), *vol.shape, _ptr(src), _ptr(G), _ptr(Wd), _ptr(rows), _ptr(cols), _ptr(slot_of_label),
+                      _ptr(box), _ptr(out), _ptr(sens), B, S, H, W, voxel_shift, eps, _stream()), name)
+    return out, sens
+
+
 class _StructuresFunction(torch.autograd.Function):
     """(src, G, Wd) of the B * S (pose, slot) pairs -> out (B, S, H*W); gradients come back as the pose-in matrices'."""
 
     @staticmethod
     def forward(ctx, volume, labels, src, G, Wd, rows, cols, slot_of_label, box, S, voxel_shift, eps, stop_grad):
         vol = volume.contiguous()
-        BS, H, W = G.shape[0], rows.numel(), cols.numel()
-        B = BS // S
         src, G, Wd = src.contiguous().float(), G.contiguous().float(), Wd.contiguous().float()
         rows, cols = rows.contiguous().float(), cols.contiguous().float()
         ctx.want = any(ctx.needs_input_grad[2:5])
-        out = torch.empty(B, S, H * W, dtype=torch.float32, device=vol.device)
-        sens = torch.empty(B, S, H * W, 8, dtype=torch.float32, device=vol.device) if ctx.want else None
-        fn, head, name = _vol_entry(_lib.load(), "b200drr_siddon_fwd_sens_structures", vol)
-        with torch.cuda.device(vol.device):
-            _lib.check(fn(*head, _ptr(labels), *vol.shape, _ptr(src), _ptr(G), _ptr(Wd), _ptr(rows), _ptr(cols), _ptr(slot_of_label),
-                          _ptr(box), _ptr(out), _ptr(sens), B, S, H, W, voxel_shift, eps, _stream()), name)
+        out, sens = _structures_walk(vol, labels, src, G, Wd, rows, cols, slot_of_label, box, S, voxel_shift, eps, ctx.want)
         if ctx.want:
             ctx.save_for_backward(sens, Wd, rows, cols)
         ctx.stop_grad = stop_grad
@@ -201,11 +208,8 @@ def _rigid_inverse(X):
     return torch.cat([torch.cat([Rt, t], dim=-1), bottom], dim=-2)
 
 
-def render_structures(drr, *args, motions, labels, parameterization=None, convention=None, degrees=False, calibration=None,
-                      background=True, **kwargs):
-    """See DRR.render_structures."""
-    labels, X, B = check_supported(drr, args, parameterization, motions, labels, kwargs)
-    vol = drr.density
+def _camera_pose(args, B, parameterization, convention, degrees):
+    """The camera pose matrices (B, 4, 4), built as DRR.forward builds them."""
     if (parameterization == "euler_angles" and len(args) == 2 and geometry.euler_convention_ok(convention)
             and all(a.is_cuda and a.dtype == torch.float32 and a.dim() == 2 and a.shape[-1] == 3 for a in args)
             and args[0].shape == args[1].shape):
@@ -216,7 +220,13 @@ def render_structures(drr, *args, motions, labels, parameterization=None, conven
         P = convert(*args, parameterization=parameterization, convention=convention, degrees=degrees).matrix
     if P.shape[0] != B:
         raise ValueError(f"the camera pose arguments describe {P.shape[0]} poses where their leading dimension says {B}")
-    K = len(labels)
+    return P
+
+
+def _slot_inputs(drr, P, X, K, background, calibration):
+    """The pose-in inputs (src, G, Wd, rows, cols) of the B * S (pose, slot) pairs: slot k < K sees its structure through
+    X_k^-1 P, the background slot through P."""
+    B = P.shape[0]
     S = K + int(background)
     Ps = _rigid_inverse(X) @ P[:, None]                       # (B, K, 4, 4): structure k seen through X_k^-1 P
     if background:
@@ -224,7 +234,18 @@ def render_structures(drr, *args, motions, labels, parameterization=None, conven
     Ps = Ps.reshape(B * S, 4, 4)
     if calibration is not None and len(calibration) == B and B > 1:
         calibration = RigidTransform(calibration.matrix.repeat_interleave(S, dim=0))
-    src, G, Wd, rows, cols = drr._pose_in_inputs(RigidTransform(Ps), calibration)
+    return drr._pose_in_inputs(RigidTransform(Ps), calibration)
+
+
+def render_structures(drr, *args, motions, labels, parameterization=None, convention=None, degrees=False, calibration=None,
+                      background=True, **kwargs):
+    """See DRR.render_structures."""
+    labels, X, B = check_supported(drr, args, parameterization, motions, labels, kwargs)
+    vol = drr.density
+    P = _camera_pose(args, B, parameterization, convention, degrees)
+    K = len(labels)
+    S = K + int(background)
+    src, G, Wd, rows, cols = _slot_inputs(drr, P, X, K, background, calibration)
     if vol.dtype in _VOL16:
         _check_vol16(vol, src, G)
     state = _mask_state(drr)
@@ -233,3 +254,138 @@ def render_structures(drr, *args, motions, labels, parameterization=None, conven
     out = _StructuresFunction.apply(vol, state["labels"], src, G, Wd, rows, cols, slot_of_label, box, S, float(r.voxel_shift),
                                     float(r.eps), bool(r.stop_gradients_through_grid_sample))
     return drr.reshape_transform(out, batch_size=B)
+
+
+def structure_pivots(drr, labels):
+    """(K, 3) world positions of the centres of the labels' boxes, float64, from the cached label boxes (no host sync).  Voxel i
+    spans index coordinates [i - 1/2, i + 1/2], so a box [lo, hi) is centred at (lo + hi - 1) / 2; the affine maps it to world."""
+    state = _mask_state(drr)
+    slot_of_label, box = _slots(state, _label_tuple(labels), False, tuple(drr.density.shape))
+    centre = (box[:, :3] + box[:, 3:]).double() * 0.5 - 0.5
+    A = drr._affine.reshape(4, 4).double()
+    return centre @ A[:3, :3].mT + A[:3, 3]
+
+
+def _translation(c):
+    """(..., 3) -> (..., 4, 4) translations by c."""
+    T = torch.eye(4, dtype=c.dtype, device=c.device).expand(*c.shape[:-1], 4, 4).clone()
+    T[..., :3, 3] = c
+    return T
+
+
+def twist_matrix(xi):
+    """(..., 6) twists (omega, v) -> (..., 4, 4) matrices [[omega^, v], [0, 0]] (se(3)); their matrix exponential is the rigid
+    motion exp(xi^)."""
+    w, v = xi[..., :3], xi[..., 3:]
+    z = torch.zeros_like(w[..., 0])
+    rows = [torch.stack([z, -w[..., 2], w[..., 1], v[..., 0]], -1), torch.stack([w[..., 2], z, -w[..., 0], v[..., 1]], -1),
+            torch.stack([-w[..., 1], w[..., 0], z, v[..., 2]], -1), torch.stack([z, z, z, z], -1)]
+    return torch.stack(rows, dim=-2)
+
+
+def se3_exp(xi):
+    """(..., 6) twists (omega, v) -> exp(xi^) (..., 4, 4), the matrix exponential of twist_matrix(xi) in closed form:
+    [[R, V v], [0, 1]] with R = I + a W + b W^2, V = I + b W + c W^2, W = omega^, theta = |omega|, a = sin(theta) / theta,
+    b = (1 - cos(theta)) / theta^2, c = (theta - sin(theta)) / theta^3 (their Taylor series near 0).  No host sync, unlike
+    torch.linalg.matrix_exp on CUDA, which reads the norm on the host to choose its degree."""
+    W = twist_matrix(torch.cat([xi[..., :3], torch.zeros_like(xi[..., 3:])], dim=-1))[..., :3, :3]
+    th2 = (xi[..., :3] ** 2).sum(-1)
+    th = th2.sqrt()
+    small = th < 1e-4
+    ths = torch.where(small, torch.ones_like(th), th)
+    a = torch.where(small, 1 - th2 / 6, ths.sin() / ths)
+    b = torch.where(small, 0.5 - th2 / 24, (1 - ths.cos()) / ths**2)
+    c = torch.where(small, 1.0 / 6 - th2 / 120, (ths - ths.sin()) / ths**3)
+    eye = torch.eye(3, dtype=xi.dtype, device=xi.device)
+    W2 = W @ W
+    R = eye + a[..., None, None] * W + b[..., None, None] * W2
+    V = eye + b[..., None, None] * W + c[..., None, None] * W2
+    top = torch.cat([R, V @ xi[..., 3:, None]], dim=-1)
+    bottom = torch.zeros_like(top[..., :1, :])
+    bottom[..., 0, 3] = 1.0
+    return torch.cat([top, bottom], dim=-2)
+
+
+def apply_increments(X, xi, pivots):
+    """X_k <- T(c_k) exp(xi_k^) T(-c_k) X_k: the left increment of every motion about its structure's pivot, in world coordinates.
+    X (..., K, 4, 4) fp32; xi (..., K, 6) float64 (omega, v); pivots (K, 3) float64.  exp is the rigid motion se3_exp (the
+    exponential of the 4 x 4 twist matrix; pose.se3_exp_map uses the transposed, right-multiplying convention)."""
+    return (_translation(pivots) @ se3_exp(xi) @ _translation(-pivots) @ X.double()).to(X.dtype)
+
+
+def motion_tangents(drr, P, X, pivots, K, background, calibration):
+    """d(src, G, Wd)/d xi of every (pose, slot) in float64, xi_k = (omega, v) the left increment of motion k about pivot c_k:
+    -> dsrc (B*S, 6, 3), dG, dWd (B*S, 6, 3, 4); the background slot's are zero.
+
+    Slot k sees X_k(xi)^-1 P with X_k(xi) = T(c) exp(xi^) T(-c) X_k, so X_k(xi)^-1 P = X_k^-1 T(c) exp(-xi^) T(-c) P.  Only the
+    derivative at xi = 0 is wanted, and exp(-xi^) = I - xi^ to first order, so the map below is that first-order form; one
+    forward-mode pass over 6 stacked copies (copy i carries the unit tangent of parameter i) gives all six columns."""
+    from .drr import pose_in_matrices
+
+    B = P.shape[0]
+    dev = P.device
+    det = drr.detector
+    Xi = _rigid_inverse(X.detach().double()).expand(B, K, 4, 4)
+    left = Xi @ _translation(pivots)                                    # (B, K, 4, 4)
+    right = _translation(-pivots) @ P.detach().double()[:, None]        # (B, K, 4, 4)
+    calib = (det._calibration if calibration is None else calibration.matrix).detach().double().reshape(-1, 4, 4)
+    calib = calib.reshape(1, -1, 1, 4, 4).expand(6, B, K, 4, 4).reshape(6 * B * K, 4, 4)
+    consts = (det._reorient.detach().double(), drr._affine_inverse.detach().double())
+    eye = torch.eye(6, dtype=torch.float64, device=dev)
+
+    def f(xi):
+        Ps = left @ (torch.eye(4, dtype=torch.float64, device=dev) - twist_matrix(xi)) @ right     # (6, B, K, 4, 4)
+        return pose_in_matrices(Ps.reshape(6 * B * K, 4, 4), consts[0], calib, consts[1])
+
+    zero = torch.zeros(6, B, K, 6, dtype=torch.float64, device=dev)
+    _, (dsrc, dG, dWd) = torch.func.jvp(f, (zero,), (eye[:, None, None, :].expand(6, B, K, 6).clone(),))
+    S = K + int(background)
+
+    def slots(d):   # (6, B, K, ...) -> (B*S, 6, ...), zeros for the background slot
+        d = d.reshape(6, B, K, *d.shape[1:]).movedim(0, 2)
+        if background:
+            d = torch.cat([d, torch.zeros_like(d[:, :1])], dim=1)
+        return d.reshape(B * S, 6, *d.shape[3:])
+
+    return slots(dsrc), slots(dG), slots(dWd)
+
+
+def structures_jacobian(drr, *args, motions, labels, parameterization=None, convention=None, degrees=False, calibration=None,
+                        background=True, stop_grad=None, return_footprints=False, **kwargs):
+    """See DRR.structures_jacobian.  stop_grad: drop Siddon's ray-length term (None = the renderer's
+    stop_gradients_through_grid_sample).  return_footprints adds the (B, S, 4) int32 pixel rectangles {w0, w1, h0, h1} the render
+    culls each (pose, slot) to (b200drr_structure_footprints): J[:, k] is zero outside rectangle k."""
+    labels, X, B = check_supported(drr, args, parameterization, motions, labels, kwargs)
+    vol = drr.density
+    r = drr.renderer
+    K = len(labels)
+    S = K + int(background)
+    with torch.no_grad():
+        P = _camera_pose(args, B, parameterization, convention, degrees)
+        src, G, Wd, rows, cols = _slot_inputs(drr, P, X, K, background, calibration)
+        if vol.dtype in _VOL16:
+            _check_vol16(vol, src, G)
+        state = _mask_state(drr)
+        slot_of_label, box = _slots(state, labels, bool(background), tuple(vol.shape))
+        src, G, Wd = src.contiguous().float(), G.contiguous().float(), Wd.contiguous().float()
+        rows, cols = rows.contiguous().float(), cols.contiguous().float()
+        shift = float(r.voxel_shift)
+        out, sens = _structures_walk(vol.contiguous(), state["labels"], src, G, Wd, rows, cols, slot_of_label, box, S, shift,
+                                     float(r.eps), True)
+        dsrc, dG, dWd = (t.float().contiguous() for t in
+                         motion_tangents(drr, P, X, structure_pivots(drr, labels), K, background, calibration))
+        H, W = rows.numel(), cols.numel()
+        J = torch.empty(B * S, H * W, 6, dtype=torch.float32, device=vol.device)
+        stop_grad = int(bool(r.stop_gradients_through_grid_sample if stop_grad is None else stop_grad))
+        lib = _lib.load()
+        with torch.cuda.device(vol.device):
+            _lib.check(lib.b200drr_siddon_jac_sens_pose(_ptr(sens), _ptr(dsrc), _ptr(dG), _ptr(dWd), _ptr(Wd), _ptr(rows), _ptr(cols),
+                                                        _ptr(J), B * S, H, W, 6, stop_grad, _stream()),
+                       "b200drr_siddon_jac_sens_pose")
+            if return_footprints:
+                rects = torch.empty(B, S, 4, dtype=torch.int32, device=vol.device)
+                _lib.check(lib.b200drr_structure_footprints(_ptr(src), _ptr(G), _ptr(rows), _ptr(cols), _ptr(box), _ptr(rects), B,
+                                                            S, H, W, shift, _stream()), "b200drr_structure_footprints")
+    img = drr.reshape_transform(out, batch_size=B)
+    J = J.view(B, S, *img.shape[2:], 6)[:, :K]
+    return (img, J, rects) if return_footprints else (img, J)

@@ -544,6 +544,29 @@ int b200drr_ncc_normal(const float *x, const float *t, const float *J, int64_t s
                        void *stream);
 
 /*
+ * Global-NCC normal equations of a piecewise-rigid composite image, block by block (DESIGN.md 6g).
+ *   b200drr_structure_footprints: per (pose b, slot s) of src [B*S][3], G [B*S][3][4] (index b*S + s), rows [H], cols [W] and the
+ *     slot boxes box [S][6] (as b200drr_siddon_fwd_sens_structures takes them) -> rects [B*S][4] int32 = {w0, w1, h0, h1}
+ *     (inclusive; empty when w0 > w1 or h0 > h1), the pixel rectangle that kernel culls the slot to, or the whole detector when
+ *     it walks every pixel.  1 <= S <= 256.
+ *   b200drr_ncc_normal_structures: the composite x [B][H][W] (device, contiguous), the target t [t_batch][H][W] (t_batch 1 or B),
+ *     and per structure k < K the Jacobian of x with respect to its 6 motion parameters: fp32, pixel n, parameter i of (pose b,
+ *     structure k) at J[b*sJb + k*sJs + n*sJn + i*sJk] (element strides >= 0; DRR.structures_jacobian's (B, S, H*W, 6) is
+ *     {S*H*W*6, H*W*6, 6, 1}), zero outside rects[b*S + k].  With P = 6K, the global NCC's system of b200drr_ncc_normal (p = 0,
+ *     C = 1) is accumulated: A [B][P][P] += weight * sum_q Jz_q Jz_q^T, g [B][P] += weight * sum_q Jz_q r_q (float64).  The image
+ *     moments run over the whole image, those of structure k over rects k, and block (j, k) of sum J J^T over the intersection of
+ *     rects j and k only.  Fixed-order double sums, no atomics: repeated calls give identical bits.  1 <= K <= 255, K <= S <= 256,
+ *     B <= 65535, eps >= 0.  workspace: b200drr_ncc_normal_structures_workspace_bytes(B, K, H, W) bytes, 8-byte aligned (0 for
+ *     bad arguments); it holds no pixels x P^2 or pairs x pixels array.
+ */
+int b200drr_structure_footprints(const float *src, const float *G, const float *rows, const float *cols, const int32_t *box,
+                                 int32_t *rects, int B, int S, int H, int W, float voxel_shift, void *stream);
+int64_t b200drr_ncc_normal_structures_workspace_bytes(int B, int K, int H, int W);
+int b200drr_ncc_normal_structures(const float *x, const float *t, int t_batch, const float *J, int64_t sJb, int64_t sJs, int64_t sJn,
+                                  int64_t sJk, const int32_t *rects, int B, int K, int S, int H, int W, double eps, double weight,
+                                  void *workspace, double *A, double *g, void *stream);
+
+/*
  * Gaussian blur + Sobel gradients of one-channel images (reference diffdrr/metrics.py:69-93, the Sobel front end of
  * GradientNormalizedCrossCorrelation2d).  x [B][H][W] (device) -> out [B][2][H][W]:
  *   blur   separable, 1-D weights [ksize] (device; torchvision's normalised Gaussian, ksize odd; ksize = 1 with weight 1 is no

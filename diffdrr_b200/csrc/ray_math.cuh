@@ -657,6 +657,13 @@ B200_HD void lean_init(const Walk& w, int st0, int st1, int st2, LeanState& s, L
 // How the walks fetch their voxels: one scalar load per visit from the volume as stored (production), or -- EXPERIMENT, see
 // siddon_ray_lean_box_chunk -- W-voxel chunks from a major-axis-fastest copy, re-used across visits (LoadChunk below), or only
 // the voxels of one labelled structure (LoadGated, structures_math.cuh).
+// load_cut<Load>::value is the default CUT rule of the sensitivities walks with that load (start_walk_in_frame): false for the
+// whole-volume and slab loads; a load whose boxes have interior faces on every axis specialises it to true (LoadGated).
+template <class Load>
+struct load_cut {
+    static constexpr bool value = false;
+};
+
 struct LoadPlain {
     template <int U, class V>
     B200_HD void batch(const V* vol, const int (&offs)[U], float (&v)[U])
@@ -1115,7 +1122,7 @@ B200_HD float siddon_ray_sens_walk_m(const V* vol, const Walk& w, int st0, int s
     return acc;
 }
 
-template <int U, int M, class Load = LoadPlain, bool CUT = false, class V = float>
+template <int U, int M, class Load = LoadPlain, bool CUT = load_cut<Load>::value, class V = float>
 B200_HD float siddon_ray_sens_box_m(const V* vol, const VolDims& dims, const int lo_v[3], const int hi_v[3], int st0,
                                     int st1, int st2, const Ray& ray, float shift, float A[3], float C[3], Load loader = Load())
 {
@@ -1123,7 +1130,7 @@ B200_HD float siddon_ray_sens_box_m(const V* vol, const VolDims& dims, const int
 }
 
 // Dispatch on the ray's major axis (uniform per warp except for rays near a 45-degree direction).
-template <int U, class Load = LoadPlain, bool CUT = false, class V = float>
+template <int U, class Load = LoadPlain, bool CUT = load_cut<Load>::value, class V = float>
 B200_HD float siddon_ray_sens_box(const V* vol, const VolDims& dims, const int lo_v[3], const int hi_v[3], int st0,
                                   int st1, int st2, const Ray& ray, float shift, float A[3], float C[3], Load loader = Load())
 {

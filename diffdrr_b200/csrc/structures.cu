@@ -119,6 +119,8 @@ __global__ void __launch_bounds__(TW* TH, 8) siddon_structures_kernel(const V* _
         if (!box_surely_missed(ray, lo_v, hi_v, shift)) {
             const LoadGated ld{labels, mine};
             if constexpr (SENS) {
+                // the CUT entry rule of gated walks (load_cut<LoadGated>, structures_math.cuh): ties at the label box's faces are
+                // booked as the un-cut walk of density * (label in slot) books them
                 float A[3] = {0.0f, 0.0f, 0.0f}, C[3] = {0.0f, 0.0f, 0.0f};
                 S_ = siddon_ray_sens_box<U, LoadGated>(vol, dims, lo_v, hi_v, dims.d[1] * dims.d[2], dims.d[2], 1, ray, shift, A, C, ld);
 #pragma unroll

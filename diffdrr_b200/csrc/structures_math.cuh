@@ -38,6 +38,14 @@ struct LoadGated {
     B200_HD float at(const V* vol, int off) const { return mine[ldg_u8(label + off)] ? ldg(vol + off) : 0.0f; }
 };
 
+// A gated walk runs over a label box, whose faces are interior planes on every axis: its sensitivities walk takes the CUT entry
+// rule, so a crossing that ties with the box's entry face, and a ray that only touches the box along an edge or at a corner, are
+// booked as the un-cut walk of density * (label in slot) books them (DESIGN.md 6f).
+template <>
+struct load_cut<LoadGated> {
+    static constexpr bool value = true;
+};
+
 // Detector footprint of a box.  The pose-in ray of detector point (u, v) is x = src + t (G0 u + G1 v + c), c = G2 + G3 - src (G
 // row-major [3][4], columns G0..G3).  Corner x of the box then projects to (u, v) = (y0, y1) / y2 with y = M^-1 (x - src), M = [G0 |
 // G1 | c], and t = y2.  t is affine in x, so when every corner has t > 0 the whole box lies in front of the source and every line

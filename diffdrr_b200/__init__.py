@@ -14,3 +14,4 @@ from .metrics import (  # noqa: F401,E402
     MutualInformation, NormalizedCrossCorrelation2d, Sobel)
 from .registration import LevenbergMarquardt, Registration, StructuresLevenbergMarquardt  # noqa: F401,E402
 from .structures import structures_jacobian  # noqa: F401,E402
+from .polyrigid import polyrigid_weights  # noqa: F401,E402

@@ -312,6 +312,29 @@ _SIGNATURES = {
         ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, _c_float_p, _c_float_p, _c_float_p, _c_float_p,
         _c_float_p, _c_float_p, _c_float_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_float, ctypes.c_float,
         ctypes.c_int, _c_float_p, ctypes.c_int, ctypes.c_void_p]),
+    # blended-rigid (skinned) trilinear render
+    "b200drr_polyrigid_weight_floats": (ctypes.c_int64, [ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int]),
+    "b200drr_polyrigid_pack_weights": (ctypes.c_int, [
+        _c_float_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, _c_float_p, ctypes.c_void_p]),
+    "b200drr_polyrigid_scratch_floats": (ctypes.c_int64, [ctypes.c_int, ctypes.c_int64, ctypes.c_int, ctypes.c_int, ctypes.c_int]),
+    "b200drr_polyrigid_fwd": (ctypes.c_int, [
+        _c_float_p, _c_float_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, _c_float_p, _c_float_p, _c_float_p, _c_float_p,
+        ctypes.c_int, ctypes.c_int, _c_float_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, _c_float_p, ctypes.c_int, ctypes.c_int64,
+        ctypes.c_int, ctypes.c_int, ctypes.c_float, ctypes.c_float, ctypes.c_int, _c_float_p, ctypes.c_void_p]),
+    "b200drr_polyrigid_bwd": (ctypes.c_int, [
+        _c_float_p, _c_float_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, _c_float_p, _c_float_p, _c_float_p, _c_float_p,
+        ctypes.c_int, ctypes.c_int, _c_float_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, _c_float_p, _c_float_p, _c_float_p,
+        _c_float_p, _c_float_p, _c_float_p, _c_float_p, ctypes.c_int, ctypes.c_int64, ctypes.c_int, ctypes.c_int, ctypes.c_float,
+        ctypes.c_float, ctypes.c_int, _c_float_p, ctypes.c_void_p]),
+    "b200drr_polyrigid_fwd_v16": (ctypes.c_int, [
+        ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, _c_float_p, _c_float_p, _c_float_p,
+        _c_float_p, ctypes.c_int, ctypes.c_int, _c_float_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, _c_float_p, ctypes.c_int,
+        ctypes.c_int64, ctypes.c_int, ctypes.c_int, ctypes.c_float, ctypes.c_float, ctypes.c_int, _c_float_p, ctypes.c_void_p]),
+    "b200drr_polyrigid_bwd_v16": (ctypes.c_int, [
+        ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, _c_float_p, _c_float_p, _c_float_p,
+        _c_float_p, ctypes.c_int, ctypes.c_int, _c_float_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, _c_float_p, _c_float_p,
+        _c_float_p, _c_float_p, _c_float_p, _c_float_p, _c_float_p, ctypes.c_int, ctypes.c_int64, ctypes.c_int, ctypes.c_int,
+        ctypes.c_float, ctypes.c_float, ctypes.c_int, _c_float_p, ctypes.c_void_p]),
 }
 
 # entry points of rejected experiments (include/b200drr_experimental.h): bound only when the experimental build is loaded

@@ -279,4 +279,19 @@ cudaError_t launch_mi_fwd(const float* x1, const float* x2, int B, int64_t N, co
 cudaError_t launch_mi_bwd(const float* x1, const float* x2, const float* bins, const float* sigma, const float* stats,
                           const float* gscore, float* g_x1, float* g_x2, int B, int64_t N, int nb, cudaStream_t stream);
 
+// blended-rigid (skinned) trilinear render (polyrigid.cu).  Exactly one of vol / packed is given; vol_type 0 = fp32, else
+// B200DRR_VOL_F16 / B200DRR_VOL_BF16.  W > 0: the N rays of a pose are a full row-major grid of width W.
+int polyrigid_channels(int K);  // K padded to the 4 or 8 channels the packed weight lattice stores
+int64_t polyrigid_scratch_floats(int B, int64_t N, int W, int K);
+cudaError_t launch_polyrigid_pack_weights(const float* weights, int K, int g0, int g1, int g2, float* packed, cudaStream_t stream);
+cudaError_t launch_polyrigid_fwd(const void* vol, const void* packed, int vol_type, VolDims dims, const float* src, const float* tgt,
+                                 const float* raylen, const float* M, int Bm, int K, const float* weights, int g0, int g1, int g2,
+                                 float* out, int B, int64_t N, int W, float shift, float eps, int n_points, const float* alpha_range,
+                                 cudaStream_t stream);
+cudaError_t launch_polyrigid_bwd(const void* vol, const void* packed, int vol_type, VolDims dims, const float* src, const float* tgt,
+                                 const float* raylen, const float* M, int Bm, int K, const float* weights, int g0, int g1, int g2,
+                                 const float* gout, float* g_src, float* g_tgt, float* g_raylen, float* g_M, float* g_alpha_range,
+                                 float* scratch, int B, int64_t N, int W, float shift, float eps, int n_points,
+                                 const float* alpha_range, cudaStream_t stream);
+
 }  // namespace b200drr

@@ -204,6 +204,26 @@ class DRR(nn.Module):
                                    convention=convention, degrees=degrees, calibration=calibration, background=background,
                                    stop_grad=stop_grad, **kwargs)
 
+    def render_polyrigid(self, *args, motions, weights, parameterization: str = None, convention: str = None,
+                         degrees: bool = False, calibration: RigidTransform = None, n_points: int = 500, alphamin=None,
+                         alphamax=None, **kwargs):
+        """Blended-rigid (skinned) DRR (DESIGN.md 6h) -> (B, 1, H, W): the volume deformed by K rigid motions that smooth weights
+        blend into one continuous map, marched with the Trilinear renderer's rays and samples.
+
+        Every sample x reads the density at x + sum_k w_k(x) (M_k x - x), M_k the voxel-space form of X_k^-1: linear blend skinning
+        of the pull-back, rigid wherever one weight is 1 and the identity where all are 0.  motions: (K, 4, 4) shared by the poses
+        or (B, K, 4, 4) world motions x -> X x as in render_structures (a tensor or a RigidTransform; it may require grad).
+        weights: (K, g0, g1, g2) fp32 lattice over the volume with values in [0, 1] and sum_k <= 1, e.g. from
+        polyrigid.polyrigid_weights; K <= 8.  The camera pose `*args`, calibration, n_points and alphamin / alphamax mean what they
+        do in forward.  Gradients reach the camera pose, the calibration and the motions; the density and the weights get none.
+        Supported: Trilinear with default options, fp32 / fp16 / bf16 densities, the full detector, p_subsample and patch_size;
+        anything else raises before any launch.  No host synchronisation once the lattice has been seen."""
+        from .polyrigid import render_polyrigid
+
+        return render_polyrigid(self, *args, motions=motions, weights=weights, parameterization=parameterization,
+                                convention=convention, degrees=degrees, calibration=calibration, n_points=n_points,
+                                alphamin=alphamin, alphamax=alphamax, **kwargs)
+
     # ---- fused pose-in path (SURVEY.md 8f-2) ------------------------------------------------------------------
     def _pose_in_ok(self, mask_to_channels, kwargs) -> bool:
         """True when the whole pose -> rays -> Siddon chain can run as ONE kernel with in-kernel ray generation."""
@@ -342,6 +362,7 @@ class DRR(nn.Module):
         object.__setattr__(self, "_pose_consts", None)
         object.__setattr__(self, "_grid_axes_cache", None)
         object.__setattr__(self, "_structures_cache", None)  # the label copy and label boxes of render_structures
+        object.__setattr__(self, "_polyrigid_cache", None)   # the packed weight lattice of render_polyrigid
         return out
 
     def rescale_detector_(self, scale: float):

@@ -1,0 +1,218 @@
+"""Blended-rigid (skinned) DRRs (`DRR.render_polyrigid`; DESIGN.md 6h): the volume under K rigid motions blended by smooth weights.
+
+The rays and samples are the Trilinear renderer's.  Every sample x (voxel-index coordinates) reads the density at
+    y = x + sum_k w_k(x) (M_k [x; 1] - x),        M_k = A^-1 X_k^-1 A,
+X_k the world motion of structure k (meaning as in render_structures), A = drr.affine, w_k a coarse weight lattice over the volume
+with sum_k w_k <= 1 (the rest of the weight stays on the identity).  M is formed here with torch ops, so autograd carries the
+kernel's g_M (include/b200drr.h: b200drr_polyrigid_bwd) on to whatever parameterises the motions.
+"""
+from __future__ import annotations
+
+import weakref
+
+import torch
+from torch.autograd.function import once_differentiable
+
+from . import _lib
+from .pose import RigidTransform
+from .renderers import _VOL16, Trilinear, _check_vol16, _dims_tensor, _get_alpha_minmax, _ptr, _stream, _vol_entry
+from .structures import _batch_size, _camera_pose, _label_tuple, _motion_matrices, _rigid_inverse
+
+MAX_STRUCTURES = 8
+_weights_cache = None   # (key, weak reference to the mask, lattice) of the last polyrigid_weights call
+
+
+def _gaussian_1d(sigma, device):
+    radius = max(1, int(3.0 * sigma + 0.5))
+    x = torch.arange(-radius, radius + 1, dtype=torch.float32, device=device)
+    k = torch.exp(-0.5 * (x / sigma) ** 2)
+    return k / k.sum()
+
+
+def polyrigid_weights(mask, labels, grid=(64, 64, 64), sigma=6.0, spacing=(1.0, 1.0, 1.0)):
+    """Blend weights for render_polyrigid from a label volume: -> (K, g0, g1, g2) fp32 on the mask's device, in [0, 1], sum_k <= 1.
+
+    Channel k is the occupancy of labels[k] in `mask` (D0, D1, D2) averaged onto the lattice, smoothed by a Gaussian of `sigma`
+    mm (`spacing` = voxel size in mm per axis; zero beyond the volume), and the channels are scaled down together wherever they
+    sum above 1.  Set-up code in plain torch; the result of the last call is kept and returned again while the mask tensor is
+    unchanged.  Any lattice of the same form may be passed to render_polyrigid instead."""
+    global _weights_cache
+    labels = _label_tuple(labels)
+    grid = tuple(int(g) for g in grid)
+    spacing = tuple(float(s) for s in spacing)
+    if mask.dim() != 3 or len(grid) != 3 or min(grid) < 1 or len(spacing) != 3 or not sigma > 0:
+        raise ValueError(f"polyrigid_weights needs a 3-D label volume, a 3-D lattice and sigma > 0, got mask {tuple(mask.shape)}, "
+                         f"grid {grid}, sigma {sigma}")
+    key = (mask.data_ptr(), mask._version, mask.device, tuple(mask.shape), labels, grid, float(sigma), spacing)
+    if _weights_cache is not None and _weights_cache[0] == key and _weights_cache[1]() is mask:
+        return _weights_cache[2]
+    with torch.no_grad():
+        occ = torch.stack([(mask == lab).float() for lab in labels])[None]                  # (1, K, D0, D1, D2)
+        w = torch.nn.functional.adaptive_avg_pool3d(occ, grid)[0]                           # (K, g0, g1, g2)
+        for a in range(3):
+            cell_mm = spacing[a] * mask.shape[a] / grid[a]
+            k = _gaussian_1d(max(float(sigma) / cell_mm, 1e-3), mask.device)
+            w = w.movedim(1 + a, -1)
+            shape = w.shape
+            w = torch.nn.functional.conv1d(w.reshape(-1, 1, shape[-1]), k[None, None], padding=k.numel() // 2).reshape(shape)
+            w = w.movedim(-1, 1 + a)
+        w = (w / w.sum(0, keepdim=True).clamp_min(1.0)).clamp_(0.0, 1.0).contiguous()
+    _weights_cache = (key, weakref.ref(mask), w)
+    return w
+
+
+def _packed_weights(drr, weights):
+    """The kernels' copy of the lattice (channel-last, K padded to 4 or 8), cached per lattice tensor on `drr`.  Building it is the
+    one place the lattice's values are read on the host: weights outside [0, 1] or summing above 1 are refused here."""
+    key = (weights.data_ptr(), weights._version, weights.device, tuple(weights.shape))
+    cached = getattr(drr, "_polyrigid_cache", None)
+    if cached is not None and cached[0] == key and cached[1]() is weights:
+        return cached[2]
+    K, g0, g1, g2 = weights.shape
+    with torch.no_grad():
+        w = weights.detach().contiguous()
+        lo, hi, total = torch.stack([w.min(), w.max(), w.sum(0).max()]).tolist()   # one device-to-host copy per lattice
+        if not (lo >= 0.0 and hi <= 1.0 and total <= 1.0 + 1e-5):
+            raise ValueError(f"render_polyrigid needs blend weights in [0, 1] that sum to at most 1 over the structures; got values "
+                             f"in [{lo:g}, {hi:g}] and a largest sum of {total:g}")
+        lib = _lib.load()
+        packed = torch.empty(int(lib.b200drr_polyrigid_weight_floats(K, g0, g1, g2)), dtype=torch.float32, device=w.device)
+        with torch.cuda.device(w.device):
+            _lib.check(lib.b200drr_polyrigid_pack_weights(_ptr(w), K, g0, g1, g2, _ptr(packed), _stream()),
+                       "b200drr_polyrigid_pack_weights")
+    object.__setattr__(drr, "_polyrigid_cache", (key, weakref.ref(weights), packed))
+    return packed
+
+
+def check_supported(drr, args, parameterization, motions, weights, kwargs):
+    """Refuse, before any launch, what the blended-rigid render does not cover: -> (motion matrices, B, K)."""
+    r = drr.renderer
+    if not isinstance(r, Trilinear):
+        raise NotImplementedError(f"render_polyrigid supports the Trilinear renderer, not {type(r).__name__}: the blended motion bends "
+                                  "the rays inside the volume, and Siddon's voxel walk follows straight lines")
+    if r.mode != "bilinear" or not isinstance(r.reducefn, str) or r.reducefn != "sum":
+        raise NotImplementedError("render_polyrigid supports Trilinear with its default options (mode='bilinear', reducefn='sum')")
+    if kwargs.get("align_corners", False) or kwargs.get("mask") is not None or kwargs.get("mask_to_channels", False) or \
+            set(kwargs) - {"align_corners", "mask", "mask_to_channels"}:
+        raise NotImplementedError(f"render_polyrigid takes no renderer options besides n_points, alphamin and alphamax, got "
+                                  f"{sorted(kwargs)}")
+    if not torch.is_tensor(weights) or weights.dim() != 4 or weights.dtype != torch.float32:
+        got = f"{weights.dtype} {tuple(weights.shape)}" if torch.is_tensor(weights) else type(weights).__name__
+        raise ValueError(f"weights must be an fp32 lattice (K, g0, g1, g2), got {got}")
+    K = weights.shape[0]
+    if K > MAX_STRUCTURES:
+        raise NotImplementedError(f"render_polyrigid blends at most {MAX_STRUCTURES} structures, got {K}")
+    if weights.requires_grad:
+        raise NotImplementedError("render_polyrigid produces no gradient for the blend weights: they must not require grad")
+    B = _batch_size(args, parameterization)
+    X = _motion_matrices(motions, K, B)
+    vol = drr.density
+    if vol.dtype not in (torch.float32, *_VOL16) or vol.dim() != 3 or vol.numel() >= 2**31 - 1:
+        raise NotImplementedError(f"render_polyrigid needs a 3-D fp32 / fp16 / bf16 density below 2^31 voxels, got {vol.dtype} "
+                                  f"{tuple(vol.shape)}")
+    if vol.requires_grad:
+        raise NotImplementedError("render_polyrigid produces no volume gradient: the density must not require grad")
+    if not vol.is_cuda:
+        raise _lib.B200DRRError(f"diffdrr_b200 renderers run on CUDA devices only (density is on {vol.device}); there is no CPU "
+                                "fallback")
+    if X.device != vol.device or weights.device != vol.device:
+        raise ValueError(f"motions and weights must be on the density's device {vol.device}, not {X.device} and {weights.device}")
+    return X, B, K
+
+
+class _PolyrigidFunction(torch.autograd.Function):
+    """out (B, 1, N) for rays in voxel-index space, the maps M (Bm, K, 3, 4) and the range alpha_range = [alphamin, alphamax]; the
+    density comes from its packed-corner copy when there is one, fp32 or 16-bit, through the entry point that takes it."""
+
+    @staticmethod
+    def forward(ctx, volume, packed, source, target, img, M, alpha_range, wpacked, lattice, voxel_shift, eps, n_points, grid):
+        B, N = target.shape[0], target.shape[1]
+        vol = volume.contiguous()
+        src = source.reshape(B, 3).contiguous().float()
+        tgt = target.contiguous().float()
+        raylen = img.reshape(B, N).contiguous().float()
+        M = M.contiguous().float()
+        arange = alpha_range.detach().to(device=vol.device, dtype=torch.float32).contiguous()
+        H, W = grid if grid is not None and grid[0] * grid[1] == N else (0, 0)
+        out = torch.empty(B, N, dtype=torch.float32, device=vol.device)
+        lib = _lib.load()
+        # (vol, packed[, vol_type]): exactly one of the two arrays is passed
+        fn, head, name = _vol_entry(lib, "b200drr_polyrigid_fwd", vol)
+        head = (_ptr(vol) if packed is None else None, _ptr(packed), *head[1:])
+        tail = (B, N, H, W, voxel_shift, eps, n_points, _ptr(arange), _stream())
+        geom = (*vol.shape, _ptr(src), _ptr(tgt), _ptr(raylen), _ptr(M), M.shape[0], M.shape[1], _ptr(wpacked), *lattice)
+        with torch.cuda.device(vol.device):
+            _lib.check(fn(*head, *geom, _ptr(out), *tail), name)
+        ctx.save_for_backward(vol, packed, src, tgt, raylen, M, arange, wpacked)
+        ctx.consts = (lattice, voxel_shift, eps, n_points, H, W, source.shape, img.shape)
+        return out.view(B, 1, N)
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, gout):
+        vol, packed, src, tgt, raylen, M, arange, wpacked = ctx.saved_tensors
+        lattice, voxel_shift, eps, n_points, H, W, source_shape, img_shape = ctx.consts
+        B, N = tgt.shape[0], tgt.shape[1]
+        dev = vol.device
+        gout = gout.reshape(B, N).contiguous().float()
+        g_src = torch.empty(B, 3, dtype=torch.float32, device=dev)
+        g_tgt = torch.empty(B, N, 3, dtype=torch.float32, device=dev)
+        g_raylen = torch.empty(B, N, dtype=torch.float32, device=dev)
+        g_M = torch.empty_like(M)
+        g_range = torch.empty(2, dtype=torch.float32, device=dev)
+        lib = _lib.load()
+        scratch = torch.empty(int(lib.b200drr_polyrigid_scratch_floats(B, N, H, W, M.shape[1])), dtype=torch.float32, device=dev)
+        fn, head, name = _vol_entry(lib, "b200drr_polyrigid_bwd", vol)
+        head = (_ptr(vol) if packed is None else None, _ptr(packed), *head[1:])
+        with torch.cuda.device(dev):
+            _lib.check(fn(*head, *vol.shape, _ptr(src), _ptr(tgt), _ptr(raylen), _ptr(M), M.shape[0], M.shape[1], _ptr(wpacked),
+                          *lattice, _ptr(gout), _ptr(g_src), _ptr(g_tgt), _ptr(g_raylen), _ptr(g_M), _ptr(g_range), _ptr(scratch),
+                          B, N, H, W, voxel_shift, eps, n_points, _ptr(arange), _stream()), name)
+        return (None, None, g_src.view(source_shape), g_tgt, g_raylen.view(img_shape), g_M, g_range, None, None, None, None, None,
+                None)
+
+
+def voxel_maps(drr, X):
+    """World motions X (..., K, 4, 4) -> the kernels' maps M = A^-1 X^-1 A (..., K, 3, 4), fp32; the product is taken in float64
+    so that identity motions give an exact identity rotation block (and a translation of float64 round-off)."""
+    A = drr._affine.reshape(4, 4).double()
+    Ainv = torch.linalg.inv_ex(A).inverse   # not the module's fp32 inverse: A^-1 A must be the identity to float64 round-off
+    return (Ainv @ _rigid_inverse(X.double()) @ A)[..., :3, :].float()
+
+
+def render_polyrigid(drr, *args, motions, weights, parameterization=None, convention=None, degrees=False, calibration=None,
+                     n_points=500, alphamin=None, alphamax=None, **kwargs):
+    """See DRR.render_polyrigid."""
+    X, B, K = check_supported(drr, args, parameterization, motions, weights, kwargs)
+    vol, r = drr.density, drr.renderer
+    wpacked = _packed_weights(drr, weights)
+    P = _camera_pose(args, B, parameterization, convention, degrees)
+    source, target = drr.detector(RigidTransform(P), calibration)
+    img = (target - source).norm(dim=-1).unsqueeze(1)
+    source, target = drr.affine_inverse(source), drr.affine_inverse(target)
+    if vol.dtype in _VOL16:
+        _check_vol16(vol, source, target)
+    M = voxel_maps(drr, X)
+    M = M if M.dim() == 4 else M[None]
+    det = drr.detector
+    full_grid = det.n_subsample is None and drr.patch_size is None
+    packed = r._packed_volume(vol)
+    dims = _dims_tensor(vol.shape, source.device, source.dtype)
+
+    def march(tgt, lens, grid):
+        if alphamin is None or alphamax is None:   # the batch-global range of the rays in this call, as Trilinear.forward
+            amin, amax = _get_alpha_minmax(source, tgt, dims, r.voxel_shift, r.eps)
+            lo, hi = amin.min(), amax.max()
+        else:
+            lo, hi = alphamin, alphamax
+        alpha_range = torch.stack([torch.as_tensor(lo, dtype=torch.float32, device=vol.device),
+                                   torch.as_tensor(hi, dtype=torch.float32, device=vol.device)])
+        return _PolyrigidFunction.apply(vol, packed, source, tgt, lens, M, alpha_range, wpacked, tuple(weights.shape[1:]),
+                                        float(r.voxel_shift), float(r.eps), int(n_points), grid)
+
+    if drr.patch_size is None:
+        out = march(target, img, (det.height, det.width) if full_grid else None)
+    else:   # serial patches with a range each, as DRR.render
+        out = torch.cat([march(t, i, None) for t, i in zip(target.chunk(drr.n_patches, dim=1), img.chunk(drr.n_patches, dim=-1))],
+                        dim=-1)
+    return drr.reshape_transform(out, batch_size=B)

@@ -682,6 +682,49 @@ int b200drr_trilinear_fwd_sens_pose_v16(const void *packed, int vol_type, int D0
                                         int W, float voxel_shift, float eps, int n_points, const float *alpha_range, int slab,
                                         void *stream);
 
+/*
+ * Blended-rigid (skinned) trilinear render (DESIGN.md 6h).  The rays and samples are b200drr_trilinear_fwd's (x_m = s + alpha_m d,
+ * alpha_range as there, align_corners = 0, reduce = sum); every sample is pulled back through a linear blend of K affine maps,
+ * the rest of the weight on the identity:
+ *     y_m = x_m + sum_k w_k(x_m) (M_k [x_m; 1] - x_m),      out = raylen * step * sum_m tri(V, y_m).
+ * M [Bm][K][12]: row-major 3 x 4 maps in voxel-index coordinates, Bm = 1 (shared by the poses) or B.  K <= 8
+ * (B200DRR_EUNSUPPORTED above).  weights: the PACKED lattice b200drr_polyrigid_pack_weights writes from a (K, g0, g1, g2) fp32
+ * lattice: channel-last, K padded with zeros to 4 or 8, b200drr_polyrigid_weight_floats(K, g0, g1, g2) floats, 16-byte aligned.
+ * The lattice is sampled trilinearly with the align_corners = False convention over the volume (node i of axis a at voxel
+ * coordinate (i + 1/2) D_a / g_a - 1/2) and is zero outside itself.
+ * The density is read from `vol` (D0 x D1 x D2) or from its packed-corner copy `packed` (b200drr_pack_corners): exactly one of
+ * the two is non-NULL; both give the same bits.  The rays of a pose are N arbitrary rays (H = W = 0) or a full row-major
+ * H x W grid (N = H * W), marched in 16 x 8 pixel tiles.  out [B][N] is overwritten.
+ *
+ * b200drr_polyrigid_bwd: gradients of sum(gout * out), every output OVERWRITTEN and NULL where not wanted: g_src [B][3],
+ * g_tgt [B][N][3], g_raylen [B][N], g_M [Bm][K][12], g_alpha_range [2] (the partials w.r.t. alpha_range, as
+ * b200drr_trilinear_bwd's).  No volume and no weight gradient.  scratch: b200drr_polyrigid_scratch_floats(B, N, H, W, K) floats;
+ * the sums over rays are taken from it in a fixed order, so repeated calls return identical bits.  The library allocates
+ * nothing.  The _v16 twins read a 16-bit volume (vol_type as above; `packed` from b200drr_pack_corners_v16) and equal the fp32
+ * call on the up-cast volume.
+ */
+int64_t b200drr_polyrigid_weight_floats(int K, int g0, int g1, int g2);
+int b200drr_polyrigid_pack_weights(const float *weights, int K, int g0, int g1, int g2, float *packed, void *stream);
+int64_t b200drr_polyrigid_scratch_floats(int B, int64_t N, int H, int W, int K);
+int b200drr_polyrigid_fwd(const float *vol, const float *packed, int D0, int D1, int D2, const float *src, const float *tgt,
+                          const float *raylen, const float *M, int Bm, int K, const float *weights, int g0, int g1, int g2, float *out,
+                          int B, int64_t N, int H, int W, float voxel_shift, float eps, int n_points, const float *alpha_range,
+                          void *stream);
+int b200drr_polyrigid_bwd(const float *vol, const float *packed, int D0, int D1, int D2, const float *src, const float *tgt,
+                          const float *raylen, const float *M, int Bm, int K, const float *weights, int g0, int g1, int g2,
+                          const float *gout, float *g_src, float *g_tgt, float *g_raylen, float *g_M, float *g_alpha_range,
+                          float *scratch, int B, int64_t N, int H, int W, float voxel_shift, float eps, int n_points,
+                          const float *alpha_range, void *stream);
+int b200drr_polyrigid_fwd_v16(const void *vol, const void *packed, int vol_type, int D0, int D1, int D2, const float *src,
+                              const float *tgt, const float *raylen, const float *M, int Bm, int K, const float *weights, int g0,
+                              int g1, int g2, float *out, int B, int64_t N, int H, int W, float voxel_shift, float eps, int n_points,
+                              const float *alpha_range, void *stream);
+int b200drr_polyrigid_bwd_v16(const void *vol, const void *packed, int vol_type, int D0, int D1, int D2, const float *src,
+                              const float *tgt, const float *raylen, const float *M, int Bm, int K, const float *weights, int g0,
+                              int g1, int g2, const float *gout, float *g_src, float *g_tgt, float *g_raylen, float *g_M,
+                              float *g_alpha_range, float *scratch, int B, int64_t N, int H, int W, float voxel_shift, float eps,
+                              int n_points, const float *alpha_range, void *stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -114,4 +114,17 @@ for (B, C, H, W), P, ps in (((2, 2, 37, 45), 1, (None, 1, 5, 37)), ((1, 1, 9, 70
         ncc_normal_equations(x, t, J, (P * C * H * W, H * W, C * H * W, 1), p, 1e-5, 1.0, A, g)
         torch.cuda.synchronize()
         print((B, C, H, W), P, p, "ncc_normal ok", float(A.abs().max()), float(g.abs().max()))
+# blended-rigid render (polyrigid.cu): a detector that is not a multiple of the 16 x 8 tiles, K = 3 (one padded channel), a lattice
+# that does not divide the volume, per-pose motions, plain and sub-sampled (ragged) ray sets, fp32 and bf16 densities
+from diffdrr_b200.structures import se3_exp  # noqa: E402
+for kw, dtype in ((dict(), torch.float32), (dict(p_subsample=0.37), torch.float32), (dict(), torch.bfloat16)):
+    drr = DRR(synthetic.make_subject(vol), **synthetic.detector_kwargs(23), renderer="trilinear", **kw).to(dev)
+    drr.density = drr.density.to(dtype)
+    W = torch.rand(3, 7, 5, 9, device=dev) / 3
+    xi = ((torch.rand(3, 3, 6, device=dev) - 0.5) * torch.tensor([0.1, 0.1, 0.1, 8.0, 8.0, 8.0], device=dev)).requires_grad_(True)
+    r, x = rot.detach().clone().requires_grad_(True), xyz.detach().clone().requires_grad_(True)
+    img = drr.render_polyrigid(r, x, motions=se3_exp(xi), weights=W, n_points=64, parameterization="euler_angles", convention="ZXY")
+    img.sum().backward()
+    torch.cuda.synchronize()
+    print("polyrigid", kw, dtype, "ok", float(img.sum()), float(r.grad.abs().max()), float(xi.grad.abs().max()))
 print("done")

@@ -1023,6 +1023,75 @@ int b200drr_polyrigid_bwd_v16(const void* vol, const void* packed, int vol_type,
                                     (cudaStream_t)stream));
 }
 
+// ---- deformable (dense displacement field) trilinear render (deform.cu) ------------------------------------------------------------
+namespace {
+// the checks every deform entry point shares; 0 = go on
+int deform_bad(const void* vol, const void* packed, int D0, int D1, int D2, const float* src, const float* tgt, const float* raylen,
+               const float* field, int Bf, int g0, int g1, int g2, int B, int64_t N, int H, int W, int n_points, const float* alpha_range)
+{
+    if ((vol == nullptr) == (packed == nullptr) || !src || !tgt || !raylen || !field || !alpha_range || bad_dims(D0, D1, D2) ||
+        bad_dims(g0, g1, g2) || bad_rays(B, N) || (Bf != 1 && Bf != B) || n_points < 2 || H < 0 || W < 0 ||
+        ((H > 0 || W > 0) && (int64_t)H * W != N) || (((uintptr_t)field | (uintptr_t)packed) & 15u) != 0)
+        return B200DRR_EINVAL;
+    if (too_big(D0, D1, D2) || (int64_t)g0 * g1 * g2 * 4 >= (int64_t)INT32_MAX) return B200DRR_EUNSUPPORTED;
+    return 0;
+}
+}  // namespace
+
+int64_t b200drr_deform_scratch_floats(int B, int64_t N, int H, int W)
+{
+    if (bad_rays(B, N) || H < 0 || W < 0 || ((H > 0 || W > 0) && (int64_t)H * W != N)) return 0;
+    return deform_scratch_floats(B, N, W);
+}
+
+int b200drr_deform_fwd(const float* vol, const float* packed, int D0, int D1, int D2, const float* src, const float* tgt,
+                       const float* raylen, const float* field, int Bf, int g0, int g1, int g2, float* out, int B, int64_t N, int H,
+                       int W, float voxel_shift, float eps, int n_points, const float* alpha_range, void* stream)
+{
+    if (!out) return B200DRR_EINVAL;
+    if (const int bad = deform_bad(vol, packed, D0, D1, D2, src, tgt, raylen, field, Bf, g0, g1, g2, B, N, H, W, n_points, alpha_range))
+        return bad;
+    return ret(launch_deform_fwd(vol, packed, 0, mk(D0, D1, D2), src, tgt, raylen, field, Bf, g0, g1, g2, out, B, N, W, voxel_shift, eps,
+                                 n_points, alpha_range, (cudaStream_t)stream));
+}
+
+int b200drr_deform_bwd(const float* vol, const float* packed, int D0, int D1, int D2, const float* src, const float* tgt,
+                       const float* raylen, const float* field, int Bf, int g0, int g1, int g2, const float* gout, float* g_src,
+                       float* g_tgt, float* g_raylen, float* g_field, float* g_alpha_range, float* scratch, int B, int64_t N, int H,
+                       int W, float voxel_shift, float eps, int n_points, const float* alpha_range, void* stream)
+{
+    if (!gout || !scratch || ((uintptr_t)g_field & 15u) != 0) return B200DRR_EINVAL;
+    if (const int bad = deform_bad(vol, packed, D0, D1, D2, src, tgt, raylen, field, Bf, g0, g1, g2, B, N, H, W, n_points, alpha_range))
+        return bad;
+    return ret(launch_deform_bwd(vol, packed, 0, mk(D0, D1, D2), src, tgt, raylen, field, Bf, g0, g1, g2, gout, g_src, g_tgt, g_raylen,
+                                 g_field, g_alpha_range, scratch, B, N, W, voxel_shift, eps, n_points, alpha_range, (cudaStream_t)stream));
+}
+
+int b200drr_deform_fwd_v16(const void* vol, const void* packed, int vol_type, int D0, int D1, int D2, const float* src, const float* tgt,
+                           const float* raylen, const float* field, int Bf, int g0, int g1, int g2, float* out, int B, int64_t N, int H,
+                           int W, float voxel_shift, float eps, int n_points, const float* alpha_range, void* stream)
+{
+    if (!out || (vol_type != B200DRR_VOL_F16 && vol_type != B200DRR_VOL_BF16)) return B200DRR_EINVAL;
+    if (const int bad = deform_bad(vol, packed, D0, D1, D2, src, tgt, raylen, field, Bf, g0, g1, g2, B, N, H, W, n_points, alpha_range))
+        return bad;
+    return ret(launch_deform_fwd(vol, packed, vol_type, mk(D0, D1, D2), src, tgt, raylen, field, Bf, g0, g1, g2, out, B, N, W, voxel_shift,
+                                 eps, n_points, alpha_range, (cudaStream_t)stream));
+}
+
+int b200drr_deform_bwd_v16(const void* vol, const void* packed, int vol_type, int D0, int D1, int D2, const float* src, const float* tgt,
+                           const float* raylen, const float* field, int Bf, int g0, int g1, int g2, const float* gout, float* g_src,
+                           float* g_tgt, float* g_raylen, float* g_field, float* g_alpha_range, float* scratch, int B, int64_t N, int H,
+                           int W, float voxel_shift, float eps, int n_points, const float* alpha_range, void* stream)
+{
+    if (!gout || !scratch || ((uintptr_t)g_field & 15u) != 0 || (vol_type != B200DRR_VOL_F16 && vol_type != B200DRR_VOL_BF16))
+        return B200DRR_EINVAL;
+    if (const int bad = deform_bad(vol, packed, D0, D1, D2, src, tgt, raylen, field, Bf, g0, g1, g2, B, N, H, W, n_points, alpha_range))
+        return bad;
+    return ret(launch_deform_bwd(vol, packed, vol_type, mk(D0, D1, D2), src, tgt, raylen, field, Bf, g0, g1, g2, gout, g_src, g_tgt,
+                                 g_raylen, g_field, g_alpha_range, scratch, B, N, W, voxel_shift, eps, n_points, alpha_range,
+                                 (cudaStream_t)stream));
+}
+
 #ifdef B200DRR_EXPERIMENTS
 int b200drr_x_transpose_volume(const float* vol, int D0, int D1, int D2, int axis, float* out, void* stream)
 {

@@ -1,0 +1,171 @@
+// deform.cu -- deformable (dense displacement field) trilinear DRR kernels for sm_90a (forward + backward; math in deform_math.cuh).
+// One thread marches one ray; blockIdx.y is the pose, blockIdx.x a 16 x 8 pixel tile of a full detector grid (W > 0) or 128
+// consecutive rays of any ray set (W == 0), as tiled_ray_index lays them out.
+// g_src and the range partials go through one row of partial sums per backward CTA, added in a fixed order by
+// polyrigid_finish_kernel (polyrigid.cu), and g_tgt / g_raylen are per ray, so all of them repeat bit for bit.  The field gradient
+// is the one output accumulated with atomics (vector reductions, one per lattice node and flush): it repeats to fp32 reordering.
+#include "deform_math.cuh"
+#include "kernels.h"
+
+namespace b200drr {
+
+constexpr int kDeformThreads = 128;
+constexpr int kDeformWarps = kDeformThreads / 32;
+constexpr int kDeformRow = 5;  // partial sums one backward CTA writes: g_src [3], g_alpha_range [2]
+
+template <class Gather>
+__global__ void __launch_bounds__(kDeformThreads, 6) deform_fwd_kernel(Gather gather, VolDims dims, PolyLattice lat, int Bf,
+                                                                     const float* __restrict__ src, const float* __restrict__ tgt,
+                                                                     const float* __restrict__ raylen, float* __restrict__ out,
+                                                                     int64_t N, int W, float shift, float eps, int P,
+                                                                     const float* __restrict__ alpha_range)
+{
+    const int b = blockIdx.y;
+    const int64_t n = tiled_ray_index(N, W);
+    if (n < 0) return;
+    if (Bf != 1) lat.w += (int64_t)b * lat.g[0] * lat.g[1] * lat.g[2];
+    const int64_t r = (int64_t)b * N + n;
+    const Ray ray = load_ray(src, tgt, b, r, eps);
+    const float amin = __ldg(alpha_range), amax = __ldg(alpha_range + 1);
+    const float step = (amax - amin) / (float)(P - 1);
+    out[r] = deform_ray_fwd(gather, dims, lat, ray, shift, P, amin, amax) * (__ldg(raylen + r) * step);
+}
+
+template <class Gather>
+__global__ void __launch_bounds__(kDeformThreads) deform_bwd_kernel(Gather gather, VolDims dims, PolyLattice lat, int Bf,
+                                                                    const float* __restrict__ src, const float* __restrict__ tgt,
+                                                                    const float* __restrict__ raylen, const float* __restrict__ gout,
+                                                                    float* __restrict__ g_tgt, float* __restrict__ g_raylen,
+                                                                    float* g_field, float* __restrict__ partial, int64_t N, int W,
+                                                                    float shift, float eps, int P, const float* __restrict__ alpha_range)
+{
+    __shared__ float red[kDeformWarps][kDeformRow];
+    const int b = blockIdx.y;
+    const int64_t n = tiled_ray_index(N, W);
+    float tail[kDeformRow] = {0.0f, 0.0f, 0.0f, 0.0f, 0.0f};
+    if (n >= 0) {
+        const int64_t nodes = (int64_t)lat.g[0] * lat.g[1] * lat.g[2];
+        if (Bf != 1) {
+            lat.w += b * nodes;
+            if (g_field) g_field += b * nodes * 4;
+        }
+        const int64_t r = (int64_t)b * N + n;
+        const Ray ray = load_ray(src, tgt, b, r, eps);
+        const float amin = __ldg(alpha_range), amax = __ldg(alpha_range + 1);
+        const float step = (amax - amin) / (float)(P - 1);
+        const float L = __ldg(raylen + r), g = __ldg(gout + r);
+        int flushes;
+        const TriGrad tg = deform_ray_bwd(gather, dims, lat, ray, shift, P, amin, amax, g, L, g_field, flushes);
+#pragma unroll
+        for (int a = 0; a < 3; ++a) {
+            tail[a] = tg.gs[a];
+            if (g_tgt) g_tgt[r * 3 + a] = tg.gt[a];
+        }
+        if (g_raylen) g_raylen[r] = g * step * tg.sumV;
+        tail[3] = tg.ga0;
+        tail[4] = tg.ga1;
+    }
+    // CTA sums in a fixed order: xor-shuffle tree within a warp, then the warps in index order
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+#pragma unroll
+    for (int i = 0; i < kDeformRow; ++i) {
+        const float v = warp_sum(tail[i]);
+        if (lane == 0) red[warp][i] = v;
+    }
+    __syncthreads();
+    if (threadIdx.x < kDeformRow) {
+        float v = red[0][threadIdx.x];
+#pragma unroll
+        for (int w = 1; w < kDeformWarps; ++w) v += red[w][threadIdx.x];
+        partial[((int64_t)b * gridDim.x + blockIdx.x) * kDeformRow + threadIdx.x] = v;
+    }
+}
+
+int64_t deform_scratch_floats(int B, int64_t N, int W)
+{
+    const dim3 grid = tiled_ray_grid(B, N, W);
+    return (int64_t)grid.x * grid.y * kDeformRow;
+}
+
+namespace {
+
+struct DeformCall {
+    VolDims dims;
+    const float *src, *tgt, *raylen, *field;
+    int Bf, g0, g1, g2, B;
+    int64_t N;
+    int W;
+    float shift, eps;
+    int P;
+    const float* alpha_range;
+    cudaStream_t stream;
+};
+
+template <class Gather>
+cudaError_t run_fwd(const Gather& gather, const DeformCall& c, float* out)
+{
+    const PolyLattice lat = make_lattice(c.field, c.g0, c.g1, c.g2, c.dims);
+    deform_fwd_kernel<Gather><<<tiled_ray_grid(c.B, c.N, c.W), kDeformThreads, 0, c.stream>>>(
+        gather, c.dims, lat, c.Bf, c.src, c.tgt, c.raylen, out, c.N, c.W, c.shift, c.eps, c.P, c.alpha_range);
+    return cudaGetLastError();
+}
+
+template <class Gather>
+cudaError_t run_bwd(const Gather& gather, const DeformCall& c, const float* gout, float* g_src, float* g_tgt, float* g_raylen,
+                    float* g_field, float* g_alpha_range, float* scratch)
+{
+    const PolyLattice lat = make_lattice(c.field, c.g0, c.g1, c.g2, c.dims);
+    const dim3 grid = tiled_ray_grid(c.B, c.N, c.W);
+    if (g_field) {
+        const size_t bytes = sizeof(float) * 4 * (size_t)c.Bf * c.g0 * c.g1 * c.g2;
+        const cudaError_t e = cudaMemsetAsync(g_field, 0, bytes, c.stream);
+        if (e != cudaSuccess) return e;
+    }
+    deform_bwd_kernel<Gather><<<grid, kDeformThreads, 0, c.stream>>>(gather, c.dims, lat, c.Bf, c.src, c.tgt, c.raylen, gout, g_tgt,
+                                                                     g_raylen, g_field, scratch, c.N, c.W, c.shift, c.eps, c.P,
+                                                                     c.alpha_range);
+    cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return e;
+    // the finish of the blended-rigid backward with no maps: its columns are then g_src [3] and g_alpha_range [2]
+    polyrigid_finish_kernel<<<(unsigned)(3 * c.B + 2), 256, 0, c.stream>>>(scratch, kDeformRow, 0, c.B, (int)grid.x, 1, 0, nullptr,
+                                                                         g_src, g_alpha_range);
+    return cudaGetLastError();
+}
+
+// f(gather) with the gather policy of the volume the caller gave: the packed-corner copy when there is one, the plain volume
+// otherwise; vol_type 0 = fp32, B200DRR_VOL_F16, B200DRR_VOL_BF16
+template <class F>
+cudaError_t with_gather(const void* vol, const void* packed, int vol_type, F&& f)
+{
+    switch (vol_type) {
+    case 0: return packed ? f(GatherPacked{(const float4*)packed}) : f(GatherPlainT<float>{(const float*)vol});
+    case 1:
+        return packed ? f(GatherPacked16<VoxF16>{(const Cell16<VoxF16>*)packed}) : f(GatherPlainT<VoxF16>{(const VoxF16*)vol});
+    case 2:
+        return packed ? f(GatherPacked16<VoxBF16>{(const Cell16<VoxBF16>*)packed}) : f(GatherPlainT<VoxBF16>{(const VoxBF16*)vol});
+    }
+    return cudaErrorInvalidValue;
+}
+
+}  // namespace
+
+cudaError_t launch_deform_fwd(const void* vol, const void* packed, int vol_type, VolDims dims, const float* src, const float* tgt,
+                              const float* raylen, const float* field, int Bf, int g0, int g1, int g2, float* out, int B, int64_t N,
+                              int W, float shift, float eps, int n_points, const float* alpha_range, cudaStream_t stream)
+{
+    const DeformCall c{dims, src, tgt, raylen, field, Bf, g0, g1, g2, B, N, W, shift, eps, n_points, alpha_range, stream};
+    return with_gather(vol, packed, vol_type, [&](auto gather) { return run_fwd(gather, c, out); });
+}
+
+cudaError_t launch_deform_bwd(const void* vol, const void* packed, int vol_type, VolDims dims, const float* src, const float* tgt,
+                              const float* raylen, const float* field, int Bf, int g0, int g1, int g2, const float* gout, float* g_src,
+                              float* g_tgt, float* g_raylen, float* g_field, float* g_alpha_range, float* scratch, int B, int64_t N,
+                              int W, float shift, float eps, int n_points, const float* alpha_range, cudaStream_t stream)
+{
+    const DeformCall c{dims, src, tgt, raylen, field, Bf, g0, g1, g2, B, N, W, shift, eps, n_points, alpha_range, stream};
+    return with_gather(vol, packed, vol_type, [&](auto gather) {
+        return run_bwd(gather, c, gout, g_src, g_tgt, g_raylen, g_field, g_alpha_range, scratch);
+    });
+}
+
+}  // namespace b200drr

@@ -293,5 +293,20 @@ cudaError_t launch_polyrigid_bwd(const void* vol, const void* packed, int vol_ty
                                  const float* gout, float* g_src, float* g_tgt, float* g_raylen, float* g_M, float* g_alpha_range,
                                  float* scratch, int B, int64_t N, int W, float shift, float eps, int n_points,
                                  const float* alpha_range, cudaStream_t stream);
+// the fixed-order finish of the blended-rigid backward's per-CTA partial rows; deform.cu launches it too
+__global__ void __launch_bounds__(256) polyrigid_finish_kernel(const float* __restrict__ partial, int row, int KP, int B, int T, int Bm,
+                                                               int K, float* __restrict__ g_M, float* __restrict__ g_src,
+                                                               float* __restrict__ g_alpha_range);
+
+// deformable (dense displacement field) trilinear render (deform.cu).  Arguments as the polyrigid ones; field: [Bf][g0][g1][g2][4]
+// voxel-index displacements, lane 3 zero; g_field: the same layout, zeroed here before the scatter.
+int64_t deform_scratch_floats(int B, int64_t N, int W);
+cudaError_t launch_deform_fwd(const void* vol, const void* packed, int vol_type, VolDims dims, const float* src, const float* tgt,
+                              const float* raylen, const float* field, int Bf, int g0, int g1, int g2, float* out, int B, int64_t N,
+                              int W, float shift, float eps, int n_points, const float* alpha_range, cudaStream_t stream);
+cudaError_t launch_deform_bwd(const void* vol, const void* packed, int vol_type, VolDims dims, const float* src, const float* tgt,
+                              const float* raylen, const float* field, int Bf, int g0, int g1, int g2, const float* gout, float* g_src,
+                              float* g_tgt, float* g_raylen, float* g_field, float* g_alpha_range, float* scratch, int B, int64_t N,
+                              int W, float shift, float eps, int n_points, const float* alpha_range, cudaStream_t stream);
 
 }  // namespace b200drr

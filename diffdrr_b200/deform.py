@@ -1,0 +1,148 @@
+"""Deformable DRRs (`DRR.render_deformed`; DESIGN.md 6i): the volume under a dense displacement field, marched with the Trilinear
+renderer's rays and samples.
+
+Every sample at world point p reads the CT density at p + u(p): u is a pull-back displacement in world millimetres given on a
+lattice over the volume (polyrigid.py's convention: node i of axis a at voxel coordinate (i + 1/2) D_a / g_a - 1/2, trilinear,
+zero outside the lattice).  The kernels take u in voxel-index units, channel-last and padded to 4 channels; that conversion is
+torch ops here, so autograd carries the kernel's field gradient (include/b200drr.h: b200drr_deform_bwd) back to the world-mm field
+and on to whatever produced it.  Nothing is cached and nothing is read on the host: the field changes every optimiser step.
+"""
+from __future__ import annotations
+
+import torch
+from torch.autograd.function import once_differentiable
+
+from . import _lib
+from .pose import RigidTransform
+from .renderers import _VOL16, Trilinear, _check_vol16, _dims_tensor, _get_alpha_minmax, _ptr, _stream, _vol_entry
+from .structures import _batch_size, _camera_pose
+
+
+def check_supported(drr, args, parameterization, field, kwargs):
+    """Refuse, before any launch, what the deformable render does not cover: -> B."""
+    r = drr.renderer
+    if not isinstance(r, Trilinear):
+        raise NotImplementedError(f"render_deformed supports the Trilinear renderer, not {type(r).__name__}: the displacement field "
+                                  "bends the rays inside the volume, and Siddon's voxel walk follows straight lines")
+    if r.mode != "bilinear" or not isinstance(r.reducefn, str) or r.reducefn != "sum":
+        raise NotImplementedError("render_deformed supports Trilinear with its default options (mode='bilinear', reducefn='sum')")
+    if kwargs.get("align_corners", False) or kwargs.get("mask") is not None or kwargs.get("mask_to_channels", False) or \
+            set(kwargs) - {"align_corners", "mask", "mask_to_channels"}:
+        raise NotImplementedError(f"render_deformed takes no renderer options besides n_points, alphamin and alphamax, got "
+                                  f"{sorted(kwargs)}")
+    B = _batch_size(args, parameterization)
+    if not torch.is_tensor(field) or field.dtype != torch.float32 or field.dim() not in (4, 5) or field.shape[-4] != 3 or \
+            (field.dim() == 5 and field.shape[0] != B) or min(field.shape[-3:]) < 1:
+        got = f"{field.dtype} {tuple(field.shape)}" if torch.is_tensor(field) else type(field).__name__
+        raise ValueError(f"field must be an fp32 displacement lattice (3, g0, g1, g2) or (B={B}, 3, g0, g1, g2), got {got}")
+    g0, g1, g2 = field.shape[-3:]
+    if 4 * g0 * g1 * g2 >= 2**31 - 1:
+        raise NotImplementedError(f"render_deformed takes a lattice below 2^31 floats per pose (4 channels), got {(g0, g1, g2)}")
+    vol = drr.density
+    if vol.dtype not in (torch.float32, *_VOL16) or vol.dim() != 3 or vol.numel() >= 2**31 - 1:
+        raise NotImplementedError(f"render_deformed needs a 3-D fp32 / fp16 / bf16 density below 2^31 voxels, got {vol.dtype} "
+                                  f"{tuple(vol.shape)}")
+    if vol.requires_grad:
+        raise NotImplementedError("render_deformed produces no volume gradient: the density must not require grad")
+    if not vol.is_cuda:
+        raise _lib.B200DRRError(f"diffdrr_b200 renderers run on CUDA devices only (density is on {vol.device}); there is no CPU "
+                                "fallback")
+    if field.device != vol.device:
+        raise ValueError(f"field must be on the density's device {vol.device}, not {field.device}")
+    return B
+
+
+class _DeformFunction(torch.autograd.Function):
+    """out (B, 1, N) for rays in voxel-index space, the kernels' field (Bf, g0, g1, g2, 4) in voxel units and the range
+    alpha_range = [alphamin, alphamax]; the density comes from its packed-corner copy when there is one, fp32 or 16-bit, through
+    the entry point that takes it."""
+
+    @staticmethod
+    def forward(ctx, volume, packed, source, target, img, field, alpha_range, voxel_shift, eps, n_points, grid):
+        B, N = target.shape[0], target.shape[1]
+        vol = volume.contiguous()
+        src = source.reshape(B, 3).contiguous().float()
+        tgt = target.contiguous().float()
+        raylen = img.reshape(B, N).contiguous().float()
+        field = field.contiguous()
+        arange = alpha_range.detach().to(device=vol.device, dtype=torch.float32).contiguous()
+        H, W = grid if grid is not None and grid[0] * grid[1] == N else (0, 0)
+        out = torch.empty(B, N, dtype=torch.float32, device=vol.device)
+        lib = _lib.load()
+        # (vol, packed[, vol_type]): exactly one of the two arrays is passed
+        fn, head, name = _vol_entry(lib, "b200drr_deform_fwd", vol)
+        head = (_ptr(vol) if packed is None else None, _ptr(packed), *head[1:])
+        geom = (*vol.shape, _ptr(src), _ptr(tgt), _ptr(raylen), _ptr(field), field.shape[0], *field.shape[1:4])
+        with torch.cuda.device(vol.device):
+            _lib.check(fn(*head, *geom, _ptr(out), B, N, H, W, voxel_shift, eps, n_points, _ptr(arange), _stream()), name)
+        ctx.save_for_backward(vol, packed, src, tgt, raylen, field, arange)
+        ctx.consts = (voxel_shift, eps, n_points, H, W, source.shape, img.shape)
+        return out.view(B, 1, N)
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, gout):
+        vol, packed, src, tgt, raylen, field, arange = ctx.saved_tensors
+        voxel_shift, eps, n_points, H, W, source_shape, img_shape = ctx.consts
+        B, N = tgt.shape[0], tgt.shape[1]
+        dev = vol.device
+        gout = gout.reshape(B, N).contiguous().float()
+        g_src = torch.empty(B, 3, dtype=torch.float32, device=dev)
+        g_tgt = torch.empty(B, N, 3, dtype=torch.float32, device=dev)
+        g_raylen = torch.empty(B, N, dtype=torch.float32, device=dev)
+        g_field = torch.empty_like(field) if ctx.needs_input_grad[5] else None   # NULL: the kernel skips the scatter
+        g_range = torch.empty(2, dtype=torch.float32, device=dev)
+        lib = _lib.load()
+        scratch = torch.empty(int(lib.b200drr_deform_scratch_floats(B, N, H, W)), dtype=torch.float32, device=dev)
+        fn, head, name = _vol_entry(lib, "b200drr_deform_bwd", vol)
+        head = (_ptr(vol) if packed is None else None, _ptr(packed), *head[1:])
+        with torch.cuda.device(dev):
+            _lib.check(fn(*head, *vol.shape, _ptr(src), _ptr(tgt), _ptr(raylen), _ptr(field), field.shape[0], *field.shape[1:4],
+                          _ptr(gout), _ptr(g_src), _ptr(g_tgt), _ptr(g_raylen), _ptr(g_field), _ptr(g_range), _ptr(scratch),
+                          B, N, H, W, voxel_shift, eps, n_points, _ptr(arange), _stream()), name)
+        return None, None, g_src.view(source_shape), g_tgt, g_raylen.view(img_shape), g_field, g_range, None, None, None, None
+
+
+def voxel_field(drr, field):
+    """World-mm pull-back displacements (3, g0, g1, g2) or (B, 3, g0, g1, g2) -> the kernels' field (Bf, g0, g1, g2, 4): voxel-index
+    vectors (the 3 x 3 linear part of drr.affine_inverse), channel last, a zero fourth channel.  Torch ops, differentiable."""
+    lin = drr._affine_inverse.reshape(4, 4)[:3, :3].to(field.dtype)
+    f = field if field.dim() == 5 else field[None]
+    u = torch.einsum("ij,bjxyz->bxyzi", lin, f)
+    return torch.nn.functional.pad(u, (0, 1)).contiguous()
+
+
+def render_deformed(drr, *args, field, parameterization=None, convention=None, degrees=False, calibration=None, n_points=500,
+                    alphamin=None, alphamax=None, **kwargs):
+    """See DRR.render_deformed."""
+    B = check_supported(drr, args, parameterization, field, kwargs)
+    vol, r = drr.density, drr.renderer
+    P = _camera_pose(args, B, parameterization, convention, degrees)
+    source, target = drr.detector(RigidTransform(P), calibration)
+    img = (target - source).norm(dim=-1).unsqueeze(1)
+    source, target = drr.affine_inverse(source), drr.affine_inverse(target)
+    if vol.dtype in _VOL16:
+        _check_vol16(vol, source, target)
+    U = voxel_field(drr, field)
+    det = drr.detector
+    full_grid = det.n_subsample is None and drr.patch_size is None
+    packed = r._packed_volume(vol)
+    dims = _dims_tensor(vol.shape, source.device, source.dtype)
+
+    def march(tgt, lens, grid):
+        if alphamin is None or alphamax is None:   # the batch-global range of the rays in this call, as Trilinear.forward
+            amin, amax = _get_alpha_minmax(source, tgt, dims, r.voxel_shift, r.eps)
+            lo, hi = amin.min(), amax.max()
+        else:
+            lo, hi = alphamin, alphamax
+        alpha_range = torch.stack([torch.as_tensor(lo, dtype=torch.float32, device=vol.device),
+                                   torch.as_tensor(hi, dtype=torch.float32, device=vol.device)])
+        return _DeformFunction.apply(vol, packed, source, tgt, lens, U, alpha_range, float(r.voxel_shift), float(r.eps),
+                                     int(n_points), grid)
+
+    if drr.patch_size is None:
+        out = march(target, img, (det.height, det.width) if full_grid else None)
+    else:   # serial patches with a range each, as DRR.render
+        out = torch.cat([march(t, i, None) for t, i in zip(target.chunk(drr.n_patches, dim=1), img.chunk(drr.n_patches, dim=-1))],
+                        dim=-1)
+    return drr.reshape_transform(out, batch_size=B)

@@ -224,6 +224,24 @@ class DRR(nn.Module):
                                 convention=convention, degrees=degrees, calibration=calibration, n_points=n_points,
                                 alphamin=alphamin, alphamax=alphamax, **kwargs)
 
+    def render_deformed(self, *args, field, parameterization: str = None, convention: str = None, degrees: bool = False,
+                        calibration: RigidTransform = None, n_points: int = 500, alphamin=None, alphamax=None, **kwargs):
+        """Deformable DRR (DESIGN.md 6i) -> (B, 1, H, W): the volume under a dense displacement field, marched with the Trilinear
+        renderer's rays and samples.
+
+        field: fp32 (3, g0, g1, g2) shared by the poses, or (B, 3, g0, g1, g2) one per pose; pull-back displacements in world mm
+        (the rendered density at world point p is the CT density at p + u(p)) on a lattice over the volume whose node i of axis a
+        sits at voxel coordinate (i + 1/2) D_a / g_a - 1/2, interpolated trilinearly and zero outside the lattice.  It may
+        require grad.  The camera pose `*args`, calibration, n_points and alphamin / alphamax mean what they do in forward.
+        Gradients reach the field, the camera pose and the calibration; the density gets none.  Supported: Trilinear with default
+        options, fp32 / fp16 / bf16 densities, the full detector, p_subsample and patch_size; anything else raises before any
+        launch.  No host synchronisation."""
+        from .deform import render_deformed
+
+        return render_deformed(self, *args, field=field, parameterization=parameterization, convention=convention,
+                               degrees=degrees, calibration=calibration, n_points=n_points, alphamin=alphamin,
+                               alphamax=alphamax, **kwargs)
+
     # ---- fused pose-in path (SURVEY.md 8f-2) ------------------------------------------------------------------
     def _pose_in_ok(self, mask_to_channels, kwargs) -> bool:
         """True when the whole pose -> rays -> Siddon chain can run as ONE kernel with in-kernel ray generation."""

@@ -725,6 +725,37 @@ int b200drr_polyrigid_bwd_v16(const void *vol, const void *packed, int vol_type,
                               float *g_alpha_range, float *scratch, int B, int64_t N, int H, int W, float voxel_shift, float eps,
                               int n_points, const float *alpha_range, void *stream);
 
+/*
+ * Deformable trilinear render (DESIGN.md 6i).  The rays and samples are b200drr_trilinear_fwd's; every sample is pulled back
+ * through a dense displacement field u given in voxel-index units on a lattice over the volume:
+ *     y_m = x_m + u(x_m),      out = raylen * step * sum_m tri(V, y_m).
+ * field [Bf][g0][g1][g2][4]: channel-last (u_0, u_1, u_2, 0), Bf = 1 (shared by the poses) or B, 16-byte aligned, fewer than 2^31
+ * floats per pose (B200DRR_EUNSUPPORTED otherwise).  The lattice convention is b200drr_polyrigid_fwd's (node i of axis a at voxel
+ * coordinate (i + 1/2) D_a / g_a - 1/2, trilinear, zero outside the lattice).  vol / packed, the ray sets and out as there.
+ *
+ * b200drr_deform_bwd: gradients of sum(gout * out), every output OVERWRITTEN and NULL where not wanted: g_src [B][3],
+ * g_tgt [B][N][3], g_raylen [B][N], g_alpha_range [2] (as b200drr_polyrigid_bwd's) and g_field, the field's layout, 16-byte
+ * aligned; lane 3 is written 0.  The entry zeroes g_field on the stream and then adds every ray's contribution with vector atomics,
+ * so g_field repeats only to fp32 reordering; every other output repeats bit for bit (sums over rays taken from scratch,
+ * b200drr_deform_scratch_floats(B, N, H, W) floats, in a fixed order).  g_field == NULL skips the scatter.  No volume gradient.
+ * The library allocates nothing.  The _v16 twins read a 16-bit volume and equal the fp32 call on the up-cast volume.
+ */
+int64_t b200drr_deform_scratch_floats(int B, int64_t N, int H, int W);
+int b200drr_deform_fwd(const float *vol, const float *packed, int D0, int D1, int D2, const float *src, const float *tgt,
+                       const float *raylen, const float *field, int Bf, int g0, int g1, int g2, float *out, int B, int64_t N, int H,
+                       int W, float voxel_shift, float eps, int n_points, const float *alpha_range, void *stream);
+int b200drr_deform_bwd(const float *vol, const float *packed, int D0, int D1, int D2, const float *src, const float *tgt,
+                       const float *raylen, const float *field, int Bf, int g0, int g1, int g2, const float *gout, float *g_src,
+                       float *g_tgt, float *g_raylen, float *g_field, float *g_alpha_range, float *scratch, int B, int64_t N, int H,
+                       int W, float voxel_shift, float eps, int n_points, const float *alpha_range, void *stream);
+int b200drr_deform_fwd_v16(const void *vol, const void *packed, int vol_type, int D0, int D1, int D2, const float *src, const float *tgt,
+                           const float *raylen, const float *field, int Bf, int g0, int g1, int g2, float *out, int B, int64_t N, int H,
+                           int W, float voxel_shift, float eps, int n_points, const float *alpha_range, void *stream);
+int b200drr_deform_bwd_v16(const void *vol, const void *packed, int vol_type, int D0, int D1, int D2, const float *src, const float *tgt,
+                           const float *raylen, const float *field, int Bf, int g0, int g1, int g2, const float *gout, float *g_src,
+                           float *g_tgt, float *g_raylen, float *g_field, float *g_alpha_range, float *scratch, int B, int64_t N, int H,
+                           int W, float voxel_shift, float eps, int n_points, const float *alpha_range, void *stream);
+
 #ifdef __cplusplus
 }
 #endif

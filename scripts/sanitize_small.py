@@ -127,4 +127,16 @@ for kw, dtype in ((dict(), torch.float32), (dict(p_subsample=0.37), torch.float3
     img.sum().backward()
     torch.cuda.synchronize()
     print("polyrigid", kw, dtype, "ok", float(img.sum()), float(r.grad.abs().max()), float(xi.grad.abs().max()))
+# deformable render (deform.cu): the same detectors and densities, a 7 x 5 x 9 field per pose that pulls samples out of the volume
+# and back, and a shared one, with the field scatter
+for kw, dtype in ((dict(), torch.float32), (dict(p_subsample=0.37), torch.float32), (dict(), torch.bfloat16)):
+    drr = DRR(synthetic.make_subject(vol), **synthetic.detector_kwargs(23), renderer="trilinear", **kw).to(dev)
+    drr.density = drr.density.to(dtype)
+    for shape in ((rot.shape[0], 3, 7, 5, 9), (3, 7, 5, 9)):
+        u = ((torch.rand(*shape, device=dev) - 0.5) * 80.0).requires_grad_(True)
+        r, x = rot.detach().clone().requires_grad_(True), xyz.detach().clone().requires_grad_(True)
+        img = drr.render_deformed(r, x, field=u, n_points=64, parameterization="euler_angles", convention="ZXY")
+        img.sum().backward()
+        torch.cuda.synchronize()
+        print("deform", kw, dtype, shape, "ok", float(img.sum()), float(r.grad.abs().max()), float(u.grad.abs().max()))
 print("done")

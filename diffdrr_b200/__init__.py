@@ -12,6 +12,7 @@ from .renderers import Siddon, Trilinear  # noqa: F401
 from .metrics import (  # noqa: F401,E402
     DoubleGeodesicSE3, GradientNormalizedCrossCorrelation2d, LogGeodesicSE3, MultiscaleNormalizedCrossCorrelation2d,
     MutualInformation, NormalizedCrossCorrelation2d, Sobel)
-from .registration import LevenbergMarquardt, Registration, StructuresLevenbergMarquardt  # noqa: F401,E402
+from .registration import (  # noqa: F401,E402
+    LevenbergMarquardt, PolyrigidLevenbergMarquardt, Registration, StructuresLevenbergMarquardt)
 from .structures import structures_jacobian  # noqa: F401,E402
-from .polyrigid import polyrigid_weights  # noqa: F401,E402
+from .polyrigid import polyrigid_jacobian, polyrigid_weights  # noqa: F401,E402

@@ -335,6 +335,16 @@ _SIGNATURES = {
         _c_float_p, ctypes.c_int, ctypes.c_int, _c_float_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, _c_float_p, _c_float_p,
         _c_float_p, _c_float_p, _c_float_p, _c_float_p, _c_float_p, ctypes.c_int, ctypes.c_int64, ctypes.c_int, ctypes.c_int,
         ctypes.c_float, ctypes.c_float, ctypes.c_int, _c_float_p, ctypes.c_void_p]),
+    "b200drr_polyrigid_jac": (ctypes.c_int, [
+        _c_float_p, _c_float_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, _c_float_p, _c_float_p, _c_float_p, _c_float_p,
+        ctypes.c_int, ctypes.c_int, _c_float_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, _c_float_p, _c_float_p, _c_float_p,
+        ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_float, ctypes.c_float, ctypes.c_int, _c_float_p,
+        ctypes.c_void_p]),
+    "b200drr_polyrigid_jac_v16": (ctypes.c_int, [
+        ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, _c_float_p, _c_float_p, _c_float_p,
+        _c_float_p, ctypes.c_int, ctypes.c_int, _c_float_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, _c_float_p, _c_float_p,
+        _c_float_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_float, ctypes.c_float, ctypes.c_int,
+        _c_float_p, ctypes.c_void_p]),
     # deformable (dense displacement field) trilinear render
     "b200drr_deform_scratch_floats": (ctypes.c_int64, [ctypes.c_int, ctypes.c_int64, ctypes.c_int, ctypes.c_int]),
     "b200drr_deform_fwd": (ctypes.c_int, [

@@ -1023,6 +1023,33 @@ int b200drr_polyrigid_bwd_v16(const void* vol, const void* packed, int vol_type,
                                     (cudaStream_t)stream));
 }
 
+int b200drr_polyrigid_jac(const float* vol, const float* packed, int D0, int D1, int D2, const float* src, const float* tgt,
+                          const float* raylen, const float* M, int Bm, int K, const float* weights, int g0, int g1, int g2,
+                          const float* T, float* img, float* J, int32_t* rects, int B, int H, int W, float voxel_shift, float eps,
+                          int n_points, const float* alpha_range, void* stream)
+{
+    if (!T || !img || !J || !rects || H <= 0 || W <= 0) return B200DRR_EINVAL;
+    if (const int bad = polyrigid_bad(vol, packed, D0, D1, D2, src, tgt, raylen, M, Bm, K, weights, g0, g1, g2, B, (int64_t)H * W, H,
+                                      W, n_points, alpha_range))
+        return bad;
+    return ret(launch_polyrigid_jac(vol, packed, 0, mk(D0, D1, D2), src, tgt, raylen, M, Bm, K, weights, g0, g1, g2, T, img, J, rects, B,
+                                    H, W, voxel_shift, eps, n_points, alpha_range, (cudaStream_t)stream));
+}
+
+int b200drr_polyrigid_jac_v16(const void* vol, const void* packed, int vol_type, int D0, int D1, int D2, const float* src,
+                              const float* tgt, const float* raylen, const float* M, int Bm, int K, const float* weights, int g0,
+                              int g1, int g2, const float* T, float* img, float* J, int32_t* rects, int B, int H, int W,
+                              float voxel_shift, float eps, int n_points, const float* alpha_range, void* stream)
+{
+    if (!T || !img || !J || !rects || H <= 0 || W <= 0 || (vol_type != B200DRR_VOL_F16 && vol_type != B200DRR_VOL_BF16))
+        return B200DRR_EINVAL;
+    if (const int bad = polyrigid_bad(vol, packed, D0, D1, D2, src, tgt, raylen, M, Bm, K, weights, g0, g1, g2, B, (int64_t)H * W, H,
+                                      W, n_points, alpha_range))
+        return bad;
+    return ret(launch_polyrigid_jac(vol, packed, vol_type, mk(D0, D1, D2), src, tgt, raylen, M, Bm, K, weights, g0, g1, g2, T, img, J,
+                                    rects, B, H, W, voxel_shift, eps, n_points, alpha_range, (cudaStream_t)stream));
+}
+
 // ---- deformable (dense displacement field) trilinear render (deform.cu) ------------------------------------------------------------
 namespace {
 // the checks every deform entry point shares; 0 = go on

@@ -1,8 +1,11 @@
-// polyrigid.cu -- blended-rigid (skinned) trilinear DRR kernels for sm_90a (forward + backward; math in polyrigid_math.cuh).
-// One thread marches one ray; blockIdx.y is the pose, blockIdx.x a 16 x 8 pixel tile of a full detector grid (W > 0) or 128
-// consecutive rays of any ray set (W == 0), as tiled_ray_index lays them out.  The pose's K affine maps sit in shared memory.
-// Every output is written by exactly one thread and no atomics are used: the backward kernel writes one row of partial sums per
-// CTA and polyrigid_finish_kernel adds the rows in a fixed order, so repeated calls give identical bits.
+// polyrigid.cu -- blended-rigid (skinned) trilinear DRR kernels for sm_90a (forward, backward and per-pixel motion Jacobian; math
+// in polyrigid_math.cuh).  One thread marches one ray; blockIdx.y is the pose, blockIdx.x a 16 x 8 pixel tile of a full detector
+// grid (W > 0) or 128 consecutive rays of any ray set (W == 0), as tiled_ray_index lays them out.  The pose's K affine maps sit in
+// shared memory.  The forward and backward write every output from exactly one thread and use no atomics: the backward kernel
+// writes one row of partial sums per CTA and polyrigid_finish_kernel adds the rows in a fixed order, so repeated calls give
+// identical bits.  The Jacobian's footprints use integer min / max atomics, which do not depend on order.
+#include <climits>
+
 #include "kernels.h"
 #include "polyrigid_math.cuh"
 
@@ -104,6 +107,110 @@ __global__ void __launch_bounds__(kPolyThreads) polyrigid_bwd_kernel(Gather gath
         for (int w = 1; w < kPolyWarps; ++w) v += red[w][i];
         row[i] = v;
     }
+}
+
+// Per-pixel motion Jacobian (DESIGN.md 6j), full H x W grids only: img [B][H*W] (polyrigid_fwd_kernel's bits), J [B][K][H*W][6]
+// with J[b][k][n][i] = poly_jac_entry of ray n against T [Bm][K][6][12] (the tangents dM_k / d xi_ki), and rects [B][K][4] int32
+// {w0, w1, h0, h1}: the bounding rectangle of the pixels whose ray had an in-volume sample with w_k != 0, grown with one integer
+// atomicMin / atomicMax per (CTA, k) (order-free, so every output repeats bit for bit; polyrigid_rects_empty_kernel runs first).
+// Each warp's 8 x 4 pixel bundle (tiled_ray_index) stages its J rows of one k in shared memory, so that the stores are runs of
+// 8 consecutive pixels (192 B) instead of 24 B per thread.
+template <int KP, class Gather>
+__global__ void __launch_bounds__(kPolyThreads) polyrigid_jac_kernel(Gather gather, VolDims dims, PolyLattice lat,
+                                                                     const float* __restrict__ M, const float* __restrict__ T, int Bm,
+                                                                     int K, const float* __restrict__ src, const float* __restrict__ tgt,
+                                                                     const float* __restrict__ raylen, float* __restrict__ img,
+                                                                     float* __restrict__ J, int* __restrict__ rects, int H, int W,
+                                                                     float shift, float eps, int P, const float* __restrict__ alpha_range)
+{
+    __shared__ float sM[KP * 12];
+    __shared__ float sT[KP * 72];
+    __shared__ float2 stage[kPolyWarps][32 * 3];
+    __shared__ int red[kPolyWarps][KP][4];
+    const int b = blockIdx.y;
+    const float* Tb = T + (Bm == 1 ? 0 : (int64_t)b * K * 72);
+    for (int i = threadIdx.x; i < KP * 72; i += blockDim.x) sT[i] = i < K * 72 ? __ldg(Tb + i) : 0.0f;
+    load_maps<KP>(sM, M, Bm, K, b);   // its __syncthreads covers sT too
+    const int64_t N = (int64_t)H * W;
+    const int64_t n = tiled_ray_index(N, W);
+    float A[KP][3], Bv[KP][3];
+    unsigned touched = 0u;
+    float LS = 0.0f;
+    Ray ray;
+#pragma unroll
+    for (int a = 0; a < 3; ++a) ray.s[a] = ray.d[a] = ray.inv[a] = 0.0f;
+#pragma unroll
+    for (int k = 0; k < KP; ++k)
+#pragma unroll
+        for (int a = 0; a < 3; ++a) A[k][a] = Bv[k][a] = 0.0f;
+    if (n >= 0) {
+        const int64_t r = (int64_t)b * N + n;
+        ray = load_ray(src, tgt, b, r, eps);
+        const float amin = __ldg(alpha_range), amax = __ldg(alpha_range + 1);
+        const float step = (amax - amin) / (float)(P - 1);
+        const float L = __ldg(raylen + r);
+        img[r] = polyrigid_ray_jac<KP>(gather, dims, lat, sM, ray, shift, P, amin, amax, A, Bv, touched) * (L * step);
+        LS = L * step;
+    }
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int tiles_x = (W + 15) / 16;
+    const int px0 = (blockIdx.x % tiles_x) * 16 + (warp & 1) * 8, py0 = (int)(blockIdx.x / tiles_x) * 8 + (warp >> 1) * 4;
+    const int px = px0 + (lane & 7), py = py0 + (lane >> 3);
+#pragma unroll
+    for (int k = 0; k < KP; ++k) {
+        const bool hit = n >= 0 && ((touched >> k) & 1u);
+        const int w0 = __reduce_min_sync(0xffffffffu, hit ? px : INT_MAX), w1 = __reduce_max_sync(0xffffffffu, hit ? px : -1);
+        const int h0 = __reduce_min_sync(0xffffffffu, hit ? py : INT_MAX), h1 = __reduce_max_sync(0xffffffffu, hit ? py : -1);
+        if (lane == 0) {
+            red[warp][k][0] = w0;
+            red[warp][k][1] = w1;
+            red[warp][k][2] = h0;
+            red[warp][k][3] = h1;
+        }
+    }
+    // stage[warp] holds the bundle's 4 rows x 8 pixels x 6 floats of one k: float2 j = row * 24 + pixel * 3 + i / 2
+    float* st = reinterpret_cast<float*>(stage[warp]);
+#pragma unroll
+    for (int k = 0; k < KP; ++k) {
+        if (k >= K) break;
+#pragma unroll
+        for (int i = 0; i < 6; ++i) st[lane * 6 + i] = poly_jac_entry(A[k], Bv[k], ray, sT + (k * 6 + i) * 12, LS);
+        __syncwarp();
+        float* Jk = J + ((int64_t)b * K + k) * N * 6;
+#pragma unroll
+        for (int q = 0; q < 3; ++q) {
+            const int j = lane + 32 * q, row = j / 24, c = j % 24;
+            const int x = px0 + c / 3, y = py0 + row;
+            if (x < W && y < H) reinterpret_cast<float2*>(Jk + ((int64_t)y * W + x) * 6)[c % 3] = stage[warp][j];
+        }
+        __syncwarp();
+    }
+    __syncthreads();
+    if (threadIdx.x < K) {
+        const int k = threadIdx.x;
+        int r[4] = {red[0][k][0], red[0][k][1], red[0][k][2], red[0][k][3]};
+#pragma unroll
+        for (int w = 1; w < kPolyWarps; ++w) {
+            r[0] = min(r[0], red[w][k][0]);
+            r[1] = max(r[1], red[w][k][1]);
+            r[2] = min(r[2], red[w][k][2]);
+            r[3] = max(r[3], red[w][k][3]);
+        }
+        if (r[0] <= r[1]) {
+            int* rk = rects + ((int64_t)b * K + k) * 4;
+            atomicMin(rk, r[0]);
+            atomicMax(rk + 1, r[1]);
+            atomicMin(rk + 2, r[2]);
+            atomicMax(rk + 3, r[3]);
+        }
+    }
+}
+
+// every rectangle empty: {W, -1, H, -1}
+__global__ void __launch_bounds__(256) polyrigid_rects_empty_kernel(int* __restrict__ rects, int n, int H, int W)
+{
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n) reinterpret_cast<int4*>(rects)[i] = make_int4(W, -1, H, -1);
 }
 
 // One CTA per output value: g_M [Bm][K][12], then g_src [B][3], then g_alpha_range [2].  Each adds its column of the partial rows
@@ -208,6 +315,19 @@ cudaError_t run_bwd(const Gather& gather, const PolyCall& c, const float* gout, 
     return cudaGetLastError();
 }
 
+template <int KP, class Gather>
+cudaError_t run_jac(const Gather& gather, const PolyCall& c, const float* T, float* img, float* J, int* rects, int H)
+{
+    const PolyLattice lat = make_lattice(c.weights, c.g0, c.g1, c.g2, c.dims);
+    const int n = c.B * c.K;
+    polyrigid_rects_empty_kernel<<<(unsigned)((n + 255) / 256), 256, 0, c.stream>>>(rects, n, H, c.W);
+    cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return e;
+    polyrigid_jac_kernel<KP, Gather><<<tiled_ray_grid(c.B, c.N, c.W), kPolyThreads, 0, c.stream>>>(
+        gather, c.dims, lat, c.M, T, c.Bm, c.K, c.src, c.tgt, c.raylen, img, J, rects, H, c.W, c.shift, c.eps, c.P, c.alpha_range);
+    return cudaGetLastError();
+}
+
 // f(gather) with the gather policy of the volume the caller gave: the packed-corner copy when there is one, the plain volume
 // otherwise; vol_type 0 = fp32, B200DRR_VOL_F16, B200DRR_VOL_BF16
 template <class F>
@@ -246,6 +366,18 @@ cudaError_t launch_polyrigid_bwd(const void* vol, const void* packed, int vol_ty
     return with_gather(vol, packed, vol_type, [&](auto gather) {
         return K <= 4 ? run_bwd<4>(gather, c, gout, g_src, g_tgt, g_raylen, g_M, g_alpha_range, scratch)
                       : run_bwd<8>(gather, c, gout, g_src, g_tgt, g_raylen, g_M, g_alpha_range, scratch);
+    });
+}
+
+cudaError_t launch_polyrigid_jac(const void* vol, const void* packed, int vol_type, VolDims dims, const float* src, const float* tgt,
+                                 const float* raylen, const float* M, int Bm, int K, const float* weights, int g0, int g1, int g2,
+                                 const float* T, float* img, float* J, int* rects, int B, int H, int W, float shift, float eps,
+                                 int n_points, const float* alpha_range, cudaStream_t stream)
+{
+    const PolyCall c{dims, src, tgt, raylen, M, Bm, K, weights, g0, g1, g2, B, (int64_t)H * W, W, shift, eps, n_points, alpha_range,
+                     stream};
+    return with_gather(vol, packed, vol_type, [&](auto gather) {
+        return K <= 4 ? run_jac<4>(gather, c, T, img, J, rects, H) : run_jac<8>(gather, c, T, img, J, rects, H);
     });
 }
 

@@ -300,4 +300,74 @@ B200_HD float poly_gM_entry(const float A[3], const float Bv[3], const Ray& ray,
     return j < 3 ? fmaf(A[i], ray.s[j], Bv[i] * ray.d[j]) : A[i];
 }
 
+// Per-pixel motion Jacobian of one ray (DESIGN.md 6j): polyrigid_ray_fwd's march, the same samples through the same arithmetic,
+// so the returned sum is its result bit for bit, that also keeps, per in-volume sample,
+//   A_k += w_k G_m,   B_k += alpha_m w_k G_m          (polyrigid_ray_bwd's A_k, B_k without the factor L step)
+// and sets bit k of `touched` where w_k != 0.  The rays do not depend on the motions, so there are no camera or range terms.
+template <int KP, class Gather>
+B200_HD float polyrigid_ray_jac(const Gather& gather, const VolDims& dims, const PolyLattice& lat, const float* M, const Ray& ray,
+                                float shift, int P, float amin, float amax, float A[][3], float Bv[][3], unsigned& touched)
+{
+    const PixLine pl = make_pixline(ray, dims, shift, 0);
+    const float range = amax - amin;
+    const float lstep = 1.0f / (float)(P - 1);
+    const float kb = shift - 0.5f;
+    int m_lo, m_hi;
+    poly_sample_range(pl, lat, amin, range, P, m_lo, m_hi);
+#pragma unroll
+    for (int k = 0; k < KP; ++k)
+#pragma unroll
+        for (int a = 0; a < 3; ++a) A[k][a] = Bv[k][a] = 0.0f;
+    touched = 0u;
+    float acc = 0.0f;
+    for (int m = m_lo; m <= m_hi; ++m) {
+        const float alpha = add_rn(mul_rn(linspace01(m, P, lstep), range), amin);
+        float pix[3], w[KP];
+#pragma unroll
+        for (int a = 0; a < 3; ++a) pix[a] = fmaf(alpha, pl.dp[a], pl.p0[a]);
+        const bool blended = poly_weights<KP, false>(lat, pix, w, nullptr);
+        if (blended) {
+            const float x[3] = {pix[0] - kb, pix[1] - kb, pix[2] - kb};
+            float disp[3] = {0.0f, 0.0f, 0.0f};
+#pragma unroll
+            for (int k = 0; k < KP; ++k) {
+                float o[3];
+                poly_offset(M + 12 * k, x, o);
+#pragma unroll
+                for (int a = 0; a < 3; ++a) disp[a] = fmaf(w[k], o[a], disp[a]);
+            }
+#pragma unroll
+            for (int a = 0; a < 3; ++a) pix[a] += disp[a];
+        }
+        // a sample outside the padded volume adds +0.0f in the forward, which leaves acc unchanged
+        if (!inside_padded(pix, dims)) continue;
+        const Corner8 c8 = gather(dims, pix);
+        acc += lerp8(c8);
+        if (!blended) continue;
+        float val, G[3];
+        tri_value_grad(c8.v, c8.f, val, G);
+#pragma unroll
+        for (int k = 0; k < KP; ++k) {
+            touched |= w[k] != 0.0f ? 1u << k : 0u;
+#pragma unroll
+            for (int a = 0; a < 3; ++a) {
+                const float wG = w[k] * G[a];
+                A[k][a] += wG;
+                Bv[k][a] = fmaf(alpha, wG, Bv[k][a]);
+            }
+        }
+    }
+    return acc;
+}
+
+// Column i of structure k for one ray: LS sum_e dI/dM_k[e] T_ki[e], dI/dM_k from A_k, B_k as poly_gM_entry lays it out and
+// T_ki [12] = dM_k / d xi_ki (row-major 3 x 4), LS = L step.  So sum_n g_n J_n = g_M : T with g_M b200drr_polyrigid_bwd's.
+B200_HD float poly_jac_entry(const float A[3], const float Bv[3], const Ray& ray, const float* Tki, float LS)
+{
+    float s = 0.0f;
+#pragma unroll
+    for (int e = 0; e < 12; ++e) s = fmaf(poly_gM_entry(A, Bv, ray, e), Tki[e], s);
+    return LS * s;
+}
+
 }  // namespace b200drr

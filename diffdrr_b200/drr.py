@@ -224,6 +224,22 @@ class DRR(nn.Module):
                                 convention=convention, degrees=degrees, calibration=calibration, n_points=n_points,
                                 alphamin=alphamin, alphamax=alphamax, **kwargs)
 
+    def polyrigid_jacobian(self, *args, motions, weights, parameterization: str = None, convention: str = None,
+                           degrees: bool = False, calibration: RigidTransform = None, n_points: int = 500, alphamin=None,
+                           alphamax=None, return_footprints: bool = False, **kwargs):
+        """(img, J): the render_polyrigid image (B, 1, H, W), bit for bit, and its per-pixel Jacobian J (B, K, H, W, 6) with
+        respect to the increment xi_k = (omega, v) of each motion (DESIGN.md 6j), from one march.  xi_k is a left increment about
+        the pivot c_k in world coordinates, X_k(xi) = T(c_k) exp(xi^) T(-c_k) X_k, c_k the weight-weighted centroid of channel k of
+        the lattice (polyrigid.polyrigid_pivots).  Columns: the rotation's three, then the translation's three.  return_footprints
+        adds rects (B, K, 4) int32 {w0, w1, h0, h1}: J[:, k] is zero outside rectangle k.  Arguments as in render_polyrigid; the
+        same set is supported except p_subsample and patch_size, and anything else raises before any launch.  Detached results;
+        no host sync once the lattice has been seen."""
+        from .polyrigid import polyrigid_jacobian
+
+        return polyrigid_jacobian(self, *args, motions=motions, weights=weights, parameterization=parameterization,
+                                  convention=convention, degrees=degrees, calibration=calibration, n_points=n_points,
+                                  alphamin=alphamin, alphamax=alphamax, return_footprints=return_footprints, **kwargs)
+
     def render_deformed(self, *args, field, parameterization: str = None, convention: str = None, degrees: bool = False,
                         calibration: RigidTransform = None, n_points: int = 500, alphamin=None, alphamax=None, **kwargs):
         """Deformable DRR (DESIGN.md 6i) -> (B, 1, H, W): the volume under a dense displacement field, marched with the Trilinear

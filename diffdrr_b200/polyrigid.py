@@ -16,7 +16,7 @@ from torch.autograd.function import once_differentiable
 from . import _lib
 from .pose import RigidTransform
 from .renderers import _VOL16, Trilinear, _check_vol16, _dims_tensor, _get_alpha_minmax, _ptr, _stream, _vol_entry
-from .structures import _batch_size, _camera_pose, _label_tuple, _motion_matrices, _rigid_inverse
+from .structures import _batch_size, _camera_pose, _label_tuple, _motion_matrices, _rigid_inverse, _translation, twist_matrix
 
 MAX_STRUCTURES = 8
 _weights_cache = None   # (key, weak reference to the mask, lattice) of the last polyrigid_weights call
@@ -216,3 +216,85 @@ def render_polyrigid(drr, *args, motions, weights, parameterization=None, conven
         out = torch.cat([march(t, i, None) for t, i in zip(target.chunk(drr.n_patches, dim=1), img.chunk(drr.n_patches, dim=-1))],
                         dim=-1)
     return drr.reshape_transform(out, batch_size=B)
+
+
+def polyrigid_pivots(drr, weights):
+    """(K, 3) float64 world points: the weight-weighted centroid of each channel's lattice nodes, the centre about which
+    polyrigid_jacobian and PolyrigidLevenbergMarquardt turn structure k.  Node i of axis a sits at voxel coordinate
+    (i + 1/2) D_a / g_a - 1/2 (render_polyrigid's lattice convention), mapped to world by drr.affine.  A channel whose weights are
+    all zero gets the volume's centre.  Torch ops only, no host sync."""
+    K, g = weights.shape[0], weights.shape[1:]
+    D = drr.density.shape
+    w = weights.detach().double()
+    axes = [(torch.arange(g[a], dtype=torch.float64, device=w.device) + 0.5) * (D[a] / g[a]) - 0.5 for a in range(3)]
+    total = w.sum((1, 2, 3))
+    centroid = torch.stack([(w.sum(tuple(b + 1 for b in range(3) if b != a)) * axes[a]).sum(-1) for a in range(3)], -1)
+    centre = torch.stack([torch.full((), (d - 1) / 2, dtype=torch.float64, device=w.device) for d in D])   # no host-to-device copy
+    p = torch.where((total > 0)[:, None], centroid / torch.where(total > 0, total, 1.0)[:, None], centre)
+    A = drr._affine.reshape(4, 4).double()
+    return p @ A[:3, :3].mT + A[:3, 3]
+
+
+def polyrigid_tangents(drr, X, pivots):
+    """T (Bm, K, 6, 3, 4) fp32: the derivatives dM_k / d xi_ki at xi = 0 of the voxel maps M_k = A^-1 X_k(xi)^-1 A (voxel_maps) under
+    the left increment X_k(xi) = T(c_k) exp(xi_k^) T(-c_k) X_k about pivot c_k (structures.apply_increments).  X (K, 4, 4) -> Bm = 1,
+    or (B, K, 4, 4); pivots (K, 3) float64.  X_k(xi)^-1 = X_k^-1 T(c_k) exp(-xi_k^) T(-c_k), and the derivative is linear in the
+    generator: T_i = -(A^-1 X_k^-1 T(c_k) E_i T(-c_k) A)[:3], E_i = twist_matrix(e_i), in closed form in float64."""
+    A = drr._affine.reshape(4, 4).double()
+    Ainv = torch.linalg.inv_ex(A).inverse
+    X = X.detach().double()
+    X = X if X.dim() == 4 else X[None]
+    E = twist_matrix(torch.eye(6, dtype=torch.float64, device=X.device))                  # (6, 4, 4)
+    left = Ainv @ _rigid_inverse(X) @ _translation(pivots)                                 # (Bm, K, 4, 4)
+    right = _translation(-pivots) @ A                                                      # (K, 4, 4)
+    T = -(left[:, :, None] @ E @ right[None, :, None])                                     # (Bm, K, 6, 4, 4)
+    return T[..., :3, :].float().contiguous()
+
+
+def polyrigid_jacobian(drr, *args, motions, weights, parameterization=None, convention=None, degrees=False, calibration=None,
+                       n_points=500, alphamin=None, alphamax=None, return_footprints=False, **kwargs):
+    """See DRR.polyrigid_jacobian."""
+    det = drr.detector
+    if det.n_subsample is not None or drr.patch_size is not None:
+        raise NotImplementedError("polyrigid_jacobian covers the full detector only, not p_subsample or patch_size: the Jacobian "
+                                  "kernel marches full H x W grids")
+    X, B, K = check_supported(drr, args, parameterization, motions, weights, kwargs)
+    vol, r = drr.density, drr.renderer
+    H, W = det.height, det.width
+    with torch.no_grad():
+        wpacked = _packed_weights(drr, weights)
+        P = _camera_pose(args, B, parameterization, convention, degrees)
+        source, target = drr.detector(RigidTransform(P), calibration)
+        raylen = (target - source).norm(dim=-1)
+        source, target = drr.affine_inverse(source), drr.affine_inverse(target)
+        if vol.dtype in _VOL16:
+            _check_vol16(vol, source, target)
+        M = voxel_maps(drr, X)
+        M = (M if M.dim() == 4 else M[None]).contiguous()
+        T = polyrigid_tangents(drr, X, polyrigid_pivots(drr, weights))
+        packed = r._packed_volume(vol)
+        dims = _dims_tensor(vol.shape, source.device, source.dtype)
+        if alphamin is None or alphamax is None:   # the batch-global range of the rays, as render_polyrigid
+            amin, amax = _get_alpha_minmax(source, target, dims, r.voxel_shift, r.eps)
+            lo, hi = amin.min(), amax.max()
+        else:
+            lo, hi = alphamin, alphamax
+        arange = torch.stack([torch.as_tensor(lo, dtype=torch.float32, device=vol.device),
+                              torch.as_tensor(hi, dtype=torch.float32, device=vol.device)])
+        src = source.reshape(B, 3).contiguous().float()
+        tgt = target.contiguous().float()
+        raylen = raylen.reshape(B, H * W).contiguous().float()
+        volc = vol.contiguous()
+        img = torch.empty(B, H * W, dtype=torch.float32, device=vol.device)
+        J = torch.empty(B, K, H * W, 6, dtype=torch.float32, device=vol.device)
+        rects = torch.empty(B, K, 4, dtype=torch.int32, device=vol.device)
+        lib = _lib.load()
+        fn, head, name = _vol_entry(lib, "b200drr_polyrigid_jac", volc)
+        head = (_ptr(volc) if packed is None else None, _ptr(packed), *head[1:])
+        with torch.cuda.device(vol.device):
+            _lib.check(fn(*head, *vol.shape, _ptr(src), _ptr(tgt), _ptr(raylen), _ptr(M), M.shape[0], K, _ptr(wpacked),
+                          *weights.shape[1:], _ptr(T), _ptr(img), _ptr(J), _ptr(rects), B, H, W, float(r.voxel_shift), float(r.eps),
+                          int(n_points), _ptr(arange), _stream()), name)
+    img = drr.reshape_transform(img.view(B, 1, H * W), batch_size=B)
+    J = J.view(B, K, H, W, 6)
+    return (img, J, rects) if return_footprints else (img, J)

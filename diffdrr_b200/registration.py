@@ -188,6 +188,28 @@ def ncc_normal_structures_equations(x, t, J, rects, eps, weight, A, g):
                                                  torch.cuda.current_stream(x.device).cuda_stream), "b200drr_ncc_normal_structures")
 
 
+def _motion_lm_update(X, A, g, damping, pivots, shared, loss, trial_loss):
+    """The damped solve, update and accept of the motion Levenberg-Marquardt steps (StructuresLevenbergMarquardt,
+    PolyrigidLevenbergMarquardt): solve (A + lambda diag A) delta = -g in float64, move every structure by the left increment
+    delta_k = (omega, v) about its pivot, X_k <- T(c_k) exp(delta_k^) T(-c_k) X_k, and keep the trial where its true loss
+    trial_loss(X_trial) (B,) is below `loss` (B,) (lambda / 10 on accept, x 10 on reject).  Shared motions (K, 4, 4): one system,
+    the mean over the views, and one decision on the mean loss.  X is updated in place -> (damping, loss after the step)."""
+    from .structures import apply_increments
+
+    if shared:
+        A, g = A.mean(0, keepdim=True), g.mean(0, keepdim=True)
+    D = torch.diag_embed(torch.diagonal(A, dim1=-2, dim2=-1).clamp_min(1e-12))
+    delta = torch.linalg.solve_ex(A + damping[:, None, None] * D, -g.unsqueeze(-1))[0].squeeze(-1)
+    X_t = apply_increments(X.detach(), delta.reshape(*X.shape[:-2], 6), pivots)   # (..., K, 6): (omega, v) per k
+    trial = trial_loss(X_t)
+    if shared:
+        loss, trial = loss.mean(), trial.mean()
+    accept = trial < loss  # a NaN trial is rejected
+    X.copy_(torch.where(accept.reshape(-1, *[1] * (X.dim() - 1)), X_t, X))
+    damping = torch.where(accept, damping / 10.0, damping * 10.0).clamp(1e-12, 1e12)
+    return damping, torch.where(accept, trial, loss)
+
+
 class StructuresLevenbergMarquardt:
     """Levenberg-Marquardt registration of the K structures of a piecewise-rigid DRR (DRR.render_structures) towards `target`
     on the global NCC of the composite image (the sum of the channels), with the camera pose fixed (DESIGN.md 6g).
@@ -262,23 +284,105 @@ class StructuresLevenbergMarquardt:
     def step(self) -> torch.Tensor:
         """One damped Gauss-Newton step; -> the loss after it: the mean over the views of 1 - NCC (a 0-d tensor) for shared
         motions, the per-pose (B,) losses otherwise."""
-        from .structures import apply_increments, render_structures, structures_jacobian
+        from .structures import render_structures, structures_jacobian
 
         X, drr = self.motions, self.drr
         with torch.no_grad():
             img, J, rects = structures_jacobian(drr, self.rot, self.xyz, motions=X, labels=self.labels, stop_grad=False,
                                                 return_footprints=True, **self.kw)
             A, g = self.normal_equations(img, J, rects)
-            if self.shared:
-                A, g = A.mean(0, keepdim=True), g.mean(0, keepdim=True)
-            D = torch.diag_embed(torch.diagonal(A, dim1=-2, dim2=-1).clamp_min(1e-12))
-            delta = torch.linalg.solve_ex(A + self.damping[:, None, None] * D, -g.unsqueeze(-1))[0].squeeze(-1)
-            X_t = apply_increments(X.detach(), delta.reshape(*X.shape[:-2], 6), self.pivots)   # (..., K, 6): (omega, v) per k
-            loss = self._loss(img)
-            trial = self._loss(render_structures(drr, self.rot, self.xyz, motions=X_t, labels=self.labels, **self.kw))
-            if self.shared:
-                loss, trial = loss.mean(), trial.mean()
-            accept = trial < loss  # a NaN trial is rejected
-            X.copy_(torch.where(accept.reshape(-1, *[1] * (X.dim() - 1)), X_t, X))
-            self.damping = torch.where(accept, self.damping / 10.0, self.damping * 10.0).clamp(1e-12, 1e12)
-            return torch.where(accept, trial, loss)
+            trial = lambda X_t: self._loss(render_structures(drr, self.rot, self.xyz, motions=X_t, labels=self.labels,  # noqa: E731
+                                                             **self.kw))
+            self.damping, loss = _motion_lm_update(X, A, g, self.damping, self.pivots, self.shared, self._loss(img), trial)
+            return loss
+
+
+class PolyrigidLevenbergMarquardt:
+    """Levenberg-Marquardt registration of the K motions of a blended-rigid DRR (DRR.render_polyrigid) towards `target` on the
+    global NCC of the image, with the camera pose fixed (DESIGN.md 6j).
+
+    The unknowns are the motions: `motions` (K, 4, 4), shared by the B views, or (B, K, 4, 4), one set per pose; a tensor fp32 on
+    the density's device, updated in place by step().  `weights` is render_polyrigid's lattice.  Each step takes one
+    DRR.polyrigid_jacobian (one march: the image, the per-pixel columns of every motion and their footprints), forms the
+    Gauss-Newton system of the z-normalised residual block by block over the footprints (b200drr_ncc_normal_structures), solves
+    (A + lambda diag A) delta = -g in float64, and renders one trial image with render_polyrigid.  delta_k = (omega, v) moves
+    structure k as
+        X_k <- T(c_k) exp(delta_k^) T(-c_k) X_k,
+    a left increment about the pivot c_k, the weight-weighted centroid of channel k's lattice (polyrigid.polyrigid_pivots).  The
+    trial is kept if its true loss is lower (lambda / 10 on accept, x 10 on reject).  Shared motions: one system, the mean over
+    the views, and one decision per step on the mean loss.  Per-pose motions: B independent systems and decisions.  The sampling
+    range is Trilinear's batch-global one unless alphamin / alphamax fix it; its dependence on the motions is nil (the rays do not
+    move), so the model is the image's full derivative.  No host sync once the lattice has been seen.
+
+    Only the global NCC is modelled: `loss` None (NormalizedCrossCorrelation2d(eps=eps)) or a NormalizedCrossCorrelation2d
+    without patch_size; anything else raises TypeError here."""
+
+    def __init__(self, drr, rot: torch.Tensor, xyz: torch.Tensor, motions: torch.Tensor, weights: torch.Tensor, target: torch.Tensor,
+                 parameterization: str = "euler_angles", convention: str | None = None, degrees: bool = False, calibration=None,
+                 n_points: int = 500, alphamin=None, alphamax=None, loss=None, damping: float = 1e-3, eps: float = 1e-5):
+        from .metrics import NormalizedCrossCorrelation2d
+        from .polyrigid import check_supported, polyrigid_pivots
+        from .structures import _batch_size
+
+        if loss is None:
+            loss = NormalizedCrossCorrelation2d(eps=eps)
+        elif type(loss) is not NormalizedCrossCorrelation2d or loss.patch_size is not None:
+            raise TypeError(f"PolyrigidLevenbergMarquardt models the global NCC only: NormalizedCrossCorrelation2d without "
+                            f"patch_size (or loss=None), not {type(loss).__name__}"
+                            f"{'' if getattr(loss, 'patch_size', None) is None else f'(patch_size={loss.patch_size})'}; patch-wise, "
+                            f"multiscale and gradient NCC have no block-sparse system here (use a first-order optimizer)")
+        if not torch.is_tensor(motions) or motions.dim() not in (3, 4):
+            raise ValueError(f"motions must be a (K, 4, 4) or (B, K, 4, 4) tensor updated in place, got "
+                             f"{tuple(motions.shape) if torch.is_tensor(motions) else type(motions).__name__}")
+        if not torch.is_tensor(target) or target.dim() != 4 or target.shape[1] != 1:
+            raise ValueError(f"PolyrigidLevenbergMarquardt takes a one-channel target image (B, 1, H, W), got "
+                             f"{tuple(target.shape) if torch.is_tensor(target) else type(target).__name__}")
+        det = drr.detector
+        if det.n_subsample is not None or drr.patch_size is not None:
+            raise NotImplementedError("PolyrigidLevenbergMarquardt covers the full detector only, not p_subsample or patch_size")
+        if tuple(target.shape[-2:]) != (det.height, det.width):
+            raise ValueError(f"the target {tuple(target.shape)} does not match the {det.height} x {det.width} detector")
+        B = _batch_size((rot, xyz), parameterization)
+        if target.shape[0] not in (1, B):
+            raise ValueError(f"the target's batch ({target.shape[0]}) must be 1 or the number of poses ({B})")
+        check_supported(drr, (rot, xyz), parameterization, motions, weights, {})
+        if not (target.is_cuda and target.dtype == torch.float32):
+            raise ValueError("PolyrigidLevenbergMarquardt's normal equations run on the GPU: the target must be a CUDA fp32 tensor")
+        self.drr, self.rot, self.xyz, self.motions, self.weights = drr, rot.detach(), xyz.detach(), motions, weights
+        self.kw = dict(parameterization=parameterization, convention=convention, degrees=degrees, calibration=calibration,
+                       n_points=n_points, alphamin=alphamin, alphamax=alphamax)
+        self.loss, self.eps = loss, float(loss.eps)
+        self.shared = motions.dim() == 3
+        self.target = target.detach().expand(B, 1, det.height, det.width).contiguous()
+        self._t = self.target[:, 0]
+        self.pivots = polyrigid_pivots(drr, weights)
+        self.damping = torch.full((1 if self.shared else B,), float(damping), dtype=torch.float64, device=motions.device)
+
+    def _loss(self, img):
+        """(B,) 1 - NCC of each view."""
+        return 1.0 - self.loss(self.target, img)
+
+    def normal_equations(self, img, J, rects):
+        """(A (B, 6K, 6K), g (B, 6K)) float64 of each view's Gauss-Newton model of 1 - NCC (weight 1 / (H W)) at the image `img`
+        (B, 1, H, W) with Jacobian J (B, K, H, W, 6) and footprints rects (B, K, 4)."""
+        B, K, H, W = img.shape[0], J.shape[1], self._t.shape[-2], self._t.shape[-1]
+        x = img.reshape(B, H, W).contiguous()
+        A = torch.zeros(B, 6 * K, 6 * K, dtype=torch.float64, device=img.device)
+        g = torch.zeros(B, 6 * K, dtype=torch.float64, device=img.device)
+        ncc_normal_structures_equations(x, self._t, J, rects, self.eps, 1.0 / (H * W), A, g)
+        return A, g
+
+    def step(self) -> torch.Tensor:
+        """One damped Gauss-Newton step; -> the loss after it: the mean over the views of 1 - NCC (a 0-d tensor) for shared
+        motions, the per-pose (B,) losses otherwise."""
+        from .polyrigid import polyrigid_jacobian, render_polyrigid
+
+        X, drr = self.motions, self.drr
+        with torch.no_grad():
+            img, J, rects = polyrigid_jacobian(drr, self.rot, self.xyz, motions=X, weights=self.weights, return_footprints=True,
+                                               **self.kw)
+            A, g = self.normal_equations(img, J, rects)
+            trial = lambda X_t: self._loss(render_polyrigid(drr, self.rot, self.xyz, motions=X_t, weights=self.weights,  # noqa: E731
+                                                            **self.kw))
+            self.damping, loss = _motion_lm_update(X, A, g, self.damping, self.pivots, self.shared, self._loss(img), trial)
+            return loss

@@ -726,6 +726,30 @@ int b200drr_polyrigid_bwd_v16(const void *vol, const void *packed, int vol_type,
                               int n_points, const float *alpha_range, void *stream);
 
 /*
+ * Per-pixel motion Jacobian of the blended-rigid render (DESIGN.md 6j), for Gauss-Newton / Levenberg-Marquardt on the motions.
+ * Arguments as b200drr_polyrigid_fwd's, on a full row-major H x W grid only (N = H * W, H, W > 0).  Per pose b, structure k,
+ * pixel n and parameter i < 6:
+ *     J[b][k][n][i] = raylen * step * sum_e dout/dM_k[e] T[bm][k][i][e],
+ * dout/dM_k (e = 4 r + c of the row-major 3 x 4 map) the ray's derivative that b200drr_polyrigid_bwd sums into g_M, and
+ * T [Bm][K][6][12] fp32 the tangents dM_k / d xi_ki of the caller's parameters (Bm as for M).  So sum_n gout_n J[b][k][n][.] is
+ * g_M : T to fp32 reordering.  Outputs, all OVERWRITTEN: img [B][H*W], b200drr_polyrigid_fwd's out bit for bit; J [B][K][H*W][6];
+ * rects [B][K][4] int32 {w0, w1, h0, h1} (inclusive; empty as {W, -1, H, -1}), the bounding rectangle of the pixels whose ray had
+ * a sample inside the padded volume with w_k != 0: J[b][k] is zero outside it (the contract of
+ * b200drr_ncc_normal_structures, which takes J with strides {K*H*W*6, H*W*6, 6, 1} and rects with S = K).  The entry sets the
+ * rects empty on the stream, then grows them with integer atomic min / max, which do not depend on order: every output repeats
+ * bit for bit.  A null pointer, H * W = 0 or a bad vol_type returns B200DRR_EINVAL, K > 8 B200DRR_EUNSUPPORTED, without touching
+ * CUDA.  The _v16 twin reads a 16-bit volume and equals the fp32 call on the up-cast volume.  The library allocates nothing.
+ */
+int b200drr_polyrigid_jac(const float *vol, const float *packed, int D0, int D1, int D2, const float *src, const float *tgt,
+                          const float *raylen, const float *M, int Bm, int K, const float *weights, int g0, int g1, int g2,
+                          const float *T, float *img, float *J, int32_t *rects, int B, int H, int W, float voxel_shift, float eps,
+                          int n_points, const float *alpha_range, void *stream);
+int b200drr_polyrigid_jac_v16(const void *vol, const void *packed, int vol_type, int D0, int D1, int D2, const float *src,
+                              const float *tgt, const float *raylen, const float *M, int Bm, int K, const float *weights, int g0,
+                              int g1, int g2, const float *T, float *img, float *J, int32_t *rects, int B, int H, int W,
+                              float voxel_shift, float eps, int n_points, const float *alpha_range, void *stream);
+
+/*
  * Deformable trilinear render (DESIGN.md 6i).  The rays and samples are b200drr_trilinear_fwd's; every sample is pulled back
  * through a dense displacement field u given in voxel-index units on a lattice over the volume:
  *     y_m = x_m + u(x_m),      out = raylen * step * sum_m tri(V, y_m).

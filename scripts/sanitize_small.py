@@ -139,4 +139,16 @@ for kw, dtype in ((dict(), torch.float32), (dict(p_subsample=0.37), torch.float3
         img.sum().backward()
         torch.cuda.synchronize()
         print("deform", kw, dtype, shape, "ok", float(img.sum()), float(r.grad.abs().max()), float(u.grad.abs().max()))
+# blended-rigid motion Jacobian (polyrigid.cu: polyrigid_jac_kernel): the 23 x 23 detector (partial 16 x 8 tiles and partial warp
+# bundles), K = 3, per-pose and shared motions, fp32 and bf16 densities
+for dtype in (torch.float32, torch.bfloat16):
+    drr = DRR(synthetic.make_subject(vol), **synthetic.detector_kwargs(23), renderer="trilinear").to(dev)
+    drr.density = drr.density.to(dtype)
+    W = torch.rand(3, 7, 5, 9, device=dev) / 3
+    for shape in ((rot.shape[0], 3, 6), (3, 6)):
+        xi = (torch.rand(*shape, device=dev) - 0.5) * torch.tensor([0.1, 0.1, 0.1, 8.0, 8.0, 8.0], device=dev)
+        img, J, rects = drr.polyrigid_jacobian(rot, xyz, motions=se3_exp(xi), weights=W, n_points=64, return_footprints=True,
+                                               parameterization="euler_angles", convention="ZXY")
+        torch.cuda.synchronize()
+        print("polyrigid_jac", dtype, shape, "ok", float(img.sum()), float(J.abs().max()), rects.tolist())
 print("done")

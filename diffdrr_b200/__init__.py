@@ -13,6 +13,7 @@ from .metrics import (  # noqa: F401,E402
     DoubleGeodesicSE3, GradientNormalizedCrossCorrelation2d, LogGeodesicSE3, MultiscaleNormalizedCrossCorrelation2d,
     MutualInformation, NormalizedCrossCorrelation2d, Sobel)
 from .registration import (  # noqa: F401,E402
-    LevenbergMarquardt, PolyrigidLevenbergMarquardt, Registration, StructuresLevenbergMarquardt)
+    DeformableLevenbergMarquardt, LevenbergMarquardt, PolyrigidLevenbergMarquardt, Registration, StructuresLevenbergMarquardt)
 from .structures import structures_jacobian  # noqa: F401,E402
 from .polyrigid import polyrigid_jacobian, polyrigid_weights  # noqa: F401,E402
+from .deform import deformed_jvp  # noqa: F401,E402

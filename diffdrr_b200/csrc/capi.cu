@@ -1119,6 +1119,31 @@ int b200drr_deform_bwd_v16(const void* vol, const void* packed, int vol_type, in
                                  (cudaStream_t)stream));
 }
 
+int b200drr_deform_jvp(const float* vol, const float* packed, int D0, int D1, int D2, const float* src, const float* tgt,
+                       const float* raylen, const float* field, int Bf, int g0, int g1, int g2, const float* tangent, float* img,
+                       float* jv, int B, int64_t N, int H, int W, float voxel_shift, float eps, int n_points, const float* alpha_range,
+                       void* stream)
+{
+    if (!tangent || !jv || ((uintptr_t)tangent & 15u) != 0) return B200DRR_EINVAL;
+    if (const int bad = deform_bad(vol, packed, D0, D1, D2, src, tgt, raylen, field, Bf, g0, g1, g2, B, N, H, W, n_points, alpha_range))
+        return bad;
+    return ret(launch_deform_jvp(vol, packed, 0, mk(D0, D1, D2), src, tgt, raylen, field, Bf, g0, g1, g2, tangent, img, jv, B, N, W,
+                                 voxel_shift, eps, n_points, alpha_range, (cudaStream_t)stream));
+}
+
+int b200drr_deform_jvp_v16(const void* vol, const void* packed, int vol_type, int D0, int D1, int D2, const float* src, const float* tgt,
+                           const float* raylen, const float* field, int Bf, int g0, int g1, int g2, const float* tangent, float* img,
+                           float* jv, int B, int64_t N, int H, int W, float voxel_shift, float eps, int n_points,
+                           const float* alpha_range, void* stream)
+{
+    if (!tangent || !jv || ((uintptr_t)tangent & 15u) != 0 || (vol_type != B200DRR_VOL_F16 && vol_type != B200DRR_VOL_BF16))
+        return B200DRR_EINVAL;
+    if (const int bad = deform_bad(vol, packed, D0, D1, D2, src, tgt, raylen, field, Bf, g0, g1, g2, B, N, H, W, n_points, alpha_range))
+        return bad;
+    return ret(launch_deform_jvp(vol, packed, vol_type, mk(D0, D1, D2), src, tgt, raylen, field, Bf, g0, g1, g2, tangent, img, jv, B, N,
+                                 W, voxel_shift, eps, n_points, alpha_range, (cudaStream_t)stream));
+}
+
 #ifdef B200DRR_EXPERIMENTS
 int b200drr_x_transpose_volume(const float* vol, int D0, int D1, int D2, int axis, float* out, void* stream)
 {

@@ -4,6 +4,8 @@
 // g_src and the range partials go through one row of partial sums per backward CTA, added in a fixed order by
 // polyrigid_finish_kernel (polyrigid.cu), and g_tgt / g_raylen are per ray, so all of them repeat bit for bit.  The field gradient
 // is the one output accumulated with atomics (vector reductions, one per lattice node and flush): it repeats to fp32 reordering.
+// The tangent (JVP) kernel writes one image value and one directional derivative per ray, with no shared memory and no atomics,
+// so both repeat bit for bit.
 #include "deform_math.cuh"
 #include "kernels.h"
 
@@ -81,6 +83,33 @@ __global__ void __launch_bounds__(kDeformThreads) deform_bwd_kernel(Gather gathe
     }
 }
 
+// jv[r] = L step sum_m G_m . v(x_m) along the tangent `tan` (deform_ray_jvp); img (may be null) = deform_fwd_kernel's out bit for bit
+template <class Gather>
+__global__ void __launch_bounds__(kDeformThreads) deform_jvp_kernel(Gather gather, VolDims dims, PolyLattice lat, PolyLattice tan,
+                                                                    int Bf, const float* __restrict__ src, const float* __restrict__ tgt,
+                                                                    const float* __restrict__ raylen, float* __restrict__ img,
+                                                                    float* __restrict__ jv, int64_t N, int W, float shift, float eps,
+                                                                    int P, const float* __restrict__ alpha_range)
+{
+    const int b = blockIdx.y;
+    const int64_t n = tiled_ray_index(N, W);
+    if (n < 0) return;
+    if (Bf != 1) {
+        const int64_t nodes = (int64_t)lat.g[0] * lat.g[1] * lat.g[2];
+        lat.w += b * nodes;
+        tan.w += b * nodes;
+    }
+    const int64_t r = (int64_t)b * N + n;
+    const Ray ray = load_ray(src, tgt, b, r, eps);
+    const float amin = __ldg(alpha_range), amax = __ldg(alpha_range + 1);
+    const float step = (amax - amin) / (float)(P - 1);
+    float acc;
+    const float d = deform_ray_jvp(gather, dims, lat, tan, ray, shift, P, amin, amax, acc);
+    const float Ls = __ldg(raylen + r) * step;
+    jv[r] = d * Ls;
+    if (img) img[r] = acc * Ls;
+}
+
 int64_t deform_scratch_floats(int B, int64_t N, int W)
 {
     const dim3 grid = tiled_ray_grid(B, N, W);
@@ -107,6 +136,16 @@ cudaError_t run_fwd(const Gather& gather, const DeformCall& c, float* out)
     const PolyLattice lat = make_lattice(c.field, c.g0, c.g1, c.g2, c.dims);
     deform_fwd_kernel<Gather><<<tiled_ray_grid(c.B, c.N, c.W), kDeformThreads, 0, c.stream>>>(
         gather, c.dims, lat, c.Bf, c.src, c.tgt, c.raylen, out, c.N, c.W, c.shift, c.eps, c.P, c.alpha_range);
+    return cudaGetLastError();
+}
+
+template <class Gather>
+cudaError_t run_jvp(const Gather& gather, const DeformCall& c, const float* tangent, float* img, float* jv)
+{
+    const PolyLattice lat = make_lattice(c.field, c.g0, c.g1, c.g2, c.dims);
+    const PolyLattice tan = make_lattice(tangent, c.g0, c.g1, c.g2, c.dims);
+    deform_jvp_kernel<Gather><<<tiled_ray_grid(c.B, c.N, c.W), kDeformThreads, 0, c.stream>>>(
+        gather, c.dims, lat, tan, c.Bf, c.src, c.tgt, c.raylen, img, jv, c.N, c.W, c.shift, c.eps, c.P, c.alpha_range);
     return cudaGetLastError();
 }
 
@@ -166,6 +205,15 @@ cudaError_t launch_deform_bwd(const void* vol, const void* packed, int vol_type,
     return with_gather(vol, packed, vol_type, [&](auto gather) {
         return run_bwd(gather, c, gout, g_src, g_tgt, g_raylen, g_field, g_alpha_range, scratch);
     });
+}
+
+cudaError_t launch_deform_jvp(const void* vol, const void* packed, int vol_type, VolDims dims, const float* src, const float* tgt,
+                              const float* raylen, const float* field, int Bf, int g0, int g1, int g2, const float* tangent, float* img,
+                              float* jv, int B, int64_t N, int W, float shift, float eps, int n_points, const float* alpha_range,
+                              cudaStream_t stream)
+{
+    const DeformCall c{dims, src, tgt, raylen, field, Bf, g0, g1, g2, B, N, W, shift, eps, n_points, alpha_range, stream};
+    return with_gather(vol, packed, vol_type, [&](auto gather) { return run_jvp(gather, c, tangent, img, jv); });
 }
 
 }  // namespace b200drr

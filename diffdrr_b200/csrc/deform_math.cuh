@@ -8,7 +8,8 @@
 // interpolates it.  With u = 0 the displacement is exactly 0.0f and the march is trilinear_ray_fwd bit for bit.
 //
 // The backward scatters d I / d u into a lattice gradient with one vector reduction per lattice node and flush (deform_red4): the
-// field gradient repeats only to fp32 reordering of those adds.  Every other output is a per-ray value.
+// field gradient repeats only to fp32 reordering of those adds.  Every other output is a per-ray value.  The tangent march
+// (deform_ray_jvp) is the scatter's transpose: the image's derivative along a field direction, one value per ray.
 #pragma once
 
 #include "polyrigid_math.cuh"
@@ -169,6 +170,46 @@ B200_HD TriGrad deform_ray_bwd(const Gather& gather, const VolDims& dims, const 
     out.ga0 = -gLv + gLs * E0;
     out.ga1 = gLv + gLs * E1;
     return out;
+}
+
+// Directional derivative of one ray along a field tangent v (DESIGN.md 6k): deform_ray_fwd's march, the same samples through the
+// same arithmetic, that also sums
+//   jv = sum_m G_m . v(x_m),      G_m = grad tri(V)(y_m)
+// over exactly the samples where deform_ray_bwd adds its field term (x_m inside the lattice's support, y_m inside the padded
+// volume), so L step jv is the transpose of that scatter.  tan: lat's geometry, w = this pose's tangent [g0][g1][g2][4] (lane 3
+// ignored).  img receives the forward's sum bit for bit (a skipped sample adds +0.0f there, which leaves it unchanged).  Multiply
+// both by raylen * step outside.
+template <class Gather>
+B200_HD float deform_ray_jvp(const Gather& gather, const VolDims& dims, const PolyLattice& lat, const PolyLattice& tan, const Ray& ray,
+                             float shift, int P, float amin, float amax, float& img)
+{
+    const PixLine pl = make_pixline(ray, dims, shift, 0);
+    const float range = amax - amin;
+    const float lstep = 1.0f / (float)(P - 1);
+    int m_lo, m_hi;
+    poly_sample_range(pl, lat, amin, range, P, m_lo, m_hi);
+    float acc = 0.0f, jv = 0.0f;
+    for (int m = m_lo; m <= m_hi; ++m) {
+        const float alpha = add_rn(mul_rn(linspace01(m, P, lstep), range), amin);
+        float pix[3], u[4], v[4];
+#pragma unroll
+        for (int a = 0; a < 3; ++a) pix[a] = fmaf(alpha, pl.dp[a], pl.p0[a]);
+        const bool moved = poly_weights<4, false>(lat, pix, u, nullptr);
+        if (moved) {
+            poly_weights<4, false>(tan, pix, v, nullptr);
+#pragma unroll
+            for (int a = 0; a < 3; ++a) pix[a] += u[a];
+        }
+        if (!inside_padded(pix, dims)) continue;
+        const Corner8 c8 = gather(dims, pix);
+        acc += lerp8(c8);
+        if (!moved) continue;
+        float val, G[3];
+        tri_value_grad(c8.v, c8.f, val, G);
+        jv = fmaf(G[0], v[0], fmaf(G[1], v[1], fmaf(G[2], v[2], jv)));
+    }
+    img = acc;
+    return jv;
 }
 
 }  // namespace b200drr

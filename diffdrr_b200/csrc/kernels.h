@@ -313,5 +313,10 @@ cudaError_t launch_deform_bwd(const void* vol, const void* packed, int vol_type,
                               const float* raylen, const float* field, int Bf, int g0, int g1, int g2, const float* gout, float* g_src,
                               float* g_tgt, float* g_raylen, float* g_field, float* g_alpha_range, float* scratch, int B, int64_t N,
                               int W, float shift, float eps, int n_points, const float* alpha_range, cudaStream_t stream);
+// the image's derivative along a field tangent [Bf][g0][g1][g2][4] (voxel units): jv [B][N]; img [B][N] (may be null) = the forward
+cudaError_t launch_deform_jvp(const void* vol, const void* packed, int vol_type, VolDims dims, const float* src, const float* tgt,
+                              const float* raylen, const float* field, int Bf, int g0, int g1, int g2, const float* tangent, float* img,
+                              float* jv, int B, int64_t N, int W, float shift, float eps, int n_points, const float* alpha_range,
+                              cudaStream_t stream);
 
 }  // namespace b200drr

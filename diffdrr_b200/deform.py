@@ -112,10 +112,11 @@ def voxel_field(drr, field):
     return torch.nn.functional.pad(u, (0, 1)).contiguous()
 
 
-def render_deformed(drr, *args, field, parameterization=None, convention=None, degrees=False, calibration=None, n_points=500,
-                    alphamin=None, alphamax=None, **kwargs):
-    """See DRR.render_deformed."""
-    B = check_supported(drr, args, parameterization, field, kwargs)
+def _marches(drr, args, B, parameterization, convention, degrees, calibration, alphamin, alphamax):
+    """The rays of a deformable render in voxel-index space -> (source (B, 1, 3), [(target, raylen, alpha_range, grid), ...]): one
+    march for the full or sub-sampled detector, one per patch for patch_size (as DRR.render), each with its own sampling range
+    (the batch-global range of its rays, as Trilinear.forward, unless alphamin / alphamax fix it) and, for a full detector grid,
+    its (H, W).  Torch ops, differentiable in the camera pose and the calibration."""
     vol, r = drr.density, drr.renderer
     P = _camera_pose(args, B, parameterization, convention, degrees)
     source, target = drr.detector(RigidTransform(P), calibration)
@@ -123,10 +124,8 @@ def render_deformed(drr, *args, field, parameterization=None, convention=None, d
     source, target = drr.affine_inverse(source), drr.affine_inverse(target)
     if vol.dtype in _VOL16:
         _check_vol16(vol, source, target)
-    U = voxel_field(drr, field)
     det = drr.detector
     full_grid = det.n_subsample is None and drr.patch_size is None
-    packed = r._packed_volume(vol)
     dims = _dims_tensor(vol.shape, source.device, source.dtype)
 
     def march(tgt, lens, grid):
@@ -137,12 +136,85 @@ def render_deformed(drr, *args, field, parameterization=None, convention=None, d
             lo, hi = alphamin, alphamax
         alpha_range = torch.stack([torch.as_tensor(lo, dtype=torch.float32, device=vol.device),
                                    torch.as_tensor(hi, dtype=torch.float32, device=vol.device)])
-        return _DeformFunction.apply(vol, packed, source, tgt, lens, U, alpha_range, float(r.voxel_shift), float(r.eps),
-                                     int(n_points), grid)
+        return tgt, lens, alpha_range, grid
 
     if drr.patch_size is None:
-        out = march(target, img, (det.height, det.width) if full_grid else None)
-    else:   # serial patches with a range each, as DRR.render
-        out = torch.cat([march(t, i, None) for t, i in zip(target.chunk(drr.n_patches, dim=1), img.chunk(drr.n_patches, dim=-1))],
-                        dim=-1)
+        return source, [march(target, img, (det.height, det.width) if full_grid else None)]
+    return source, [march(t, i, None) for t, i in zip(target.chunk(drr.n_patches, dim=1), img.chunk(drr.n_patches, dim=-1))]
+
+
+def render_deformed(drr, *args, field, parameterization=None, convention=None, degrees=False, calibration=None, n_points=500,
+                    alphamin=None, alphamax=None, **kwargs):
+    """See DRR.render_deformed."""
+    B = check_supported(drr, args, parameterization, field, kwargs)
+    vol, r = drr.density, drr.renderer
+    source, marches = _marches(drr, args, B, parameterization, convention, degrees, calibration, alphamin, alphamax)
+    U = voxel_field(drr, field)
+    packed = r._packed_volume(vol)
+    outs = [_DeformFunction.apply(vol, packed, source, tgt, lens, U, alpha_range, float(r.voxel_shift), float(r.eps), int(n_points),
+                                  grid) for tgt, lens, alpha_range, grid in marches]
+    out = outs[0] if len(outs) == 1 else torch.cat(outs, dim=-1)   # serial patches with a range each, as DRR.render
     return drr.reshape_transform(out, batch_size=B)
+
+
+def _check_tangent(field, tangent):
+    if not torch.is_tensor(tangent) or tangent.shape != field.shape or tangent.dtype != field.dtype or tangent.device != field.device:
+        got = f"{tangent.dtype} {tuple(tangent.shape)} on {tangent.device}" if torch.is_tensor(tangent) else type(tangent).__name__
+        raise ValueError(f"tangent must be a field of the same shape, dtype and device as `field` ({field.dtype} "
+                         f"{tuple(field.shape)} on {field.device}), got {got}")
+
+
+def field_jvp(drr, packed, source, target, raylen, U, T, alpha_range, n_points, grid, img=None):
+    """The directional derivative of one march along the voxel-unit tangent T (b200drr_deform_jvp): rays in voxel-index space
+    (source (B, 1, 3), target (B, N, 3), raylen (B, 1, N)), U and T the kernels' fields (Bf, g0, g1, g2, 4) -> jv (B, N); `img`
+    (B, N) fp32, if given, receives the march's image.  No autograd."""
+    vol, r = drr.density, drr.renderer
+    B, N = target.shape[0], target.shape[1]
+    H, W = grid if grid is not None and grid[0] * grid[1] == N else (0, 0)
+    src, tgt, lens = source.reshape(B, 3).contiguous().float(), target.contiguous().float(), raylen.reshape(B, N).contiguous().float()
+    jv = torch.empty(B, N, dtype=torch.float32, device=vol.device)
+    lib = _lib.load()
+    fn, head, name = _vol_entry(lib, "b200drr_deform_jvp", vol)
+    head = (_ptr(vol) if packed is None else None, _ptr(packed), *head[1:])
+    with torch.cuda.device(vol.device):
+        _lib.check(fn(*head, *vol.shape, _ptr(src), _ptr(tgt), _ptr(lens), _ptr(U), U.shape[0], *U.shape[1:4], _ptr(T), _ptr(img),
+                      _ptr(jv), B, N, H, W, float(r.voxel_shift), float(r.eps), int(n_points), _ptr(alpha_range), _stream()), name)
+    return jv
+
+
+def field_vjp(drr, packed, source, target, raylen, U, w, alpha_range, n_points, grid, scratch=None):
+    """The transpose of field_jvp: sum_n w_n dI_n / dU as the kernels' field (Bf, g0, g1, g2, 4), voxel units (b200drr_deform_bwd
+    with only g_field wanted).  w (B, N) fp32; scratch: b200drr_deform_scratch_floats floats, allocated here when None."""
+    vol, r = drr.density, drr.renderer
+    B, N = target.shape[0], target.shape[1]
+    H, W = grid if grid is not None and grid[0] * grid[1] == N else (0, 0)
+    src, tgt, lens = source.reshape(B, 3).contiguous().float(), target.contiguous().float(), raylen.reshape(B, N).contiguous().float()
+    lib = _lib.load()
+    if scratch is None:
+        scratch = torch.empty(int(lib.b200drr_deform_scratch_floats(B, N, H, W)), dtype=torch.float32, device=vol.device)
+    g_field = torch.empty_like(U)
+    fn, head, name = _vol_entry(lib, "b200drr_deform_bwd", vol)
+    head = (_ptr(vol) if packed is None else None, _ptr(packed), *head[1:])
+    with torch.cuda.device(vol.device):
+        _lib.check(fn(*head, *vol.shape, _ptr(src), _ptr(tgt), _ptr(lens), _ptr(U), U.shape[0], *U.shape[1:4], _ptr(w.contiguous()),
+                      None, None, None, _ptr(g_field), None, _ptr(scratch), B, N, H, W, float(r.voxel_shift), float(r.eps),
+                      int(n_points), _ptr(alpha_range), _stream()), name)
+    return g_field
+
+
+def deformed_jvp(drr, *args, field, tangent, parameterization=None, convention=None, degrees=False, calibration=None, n_points=500,
+                 alphamin=None, alphamax=None, **kwargs):
+    """See DRR.deformed_jvp."""
+    B = check_supported(drr, args, parameterization, field, kwargs)
+    _check_tangent(field, tangent)
+    vol, r = drr.density, drr.renderer
+    with torch.no_grad():
+        source, marches = _marches(drr, args, B, parameterization, convention, degrees, calibration, alphamin, alphamax)
+        U, T = voxel_field(drr, field), voxel_field(drr, tangent)
+        packed = r._packed_volume(vol)
+        imgs, jvs = [], []
+        for tgt, lens, alpha_range, grid in marches:
+            imgs.append(torch.empty(B, tgt.shape[1], dtype=torch.float32, device=vol.device))
+            jvs.append(field_jvp(drr, packed, source, tgt, lens, U, T, alpha_range, n_points, grid, img=imgs[-1]))
+        img, jv = (x[0] if len(x) == 1 else torch.cat(x, dim=-1) for x in (imgs, jvs))
+        return drr.reshape_transform(img.view(B, 1, -1), batch_size=B), drr.reshape_transform(jv.view(B, 1, -1), batch_size=B)

@@ -258,6 +258,20 @@ class DRR(nn.Module):
                                degrees=degrees, calibration=calibration, n_points=n_points, alphamin=alphamin,
                                alphamax=alphamax, **kwargs)
 
+    def deformed_jvp(self, *args, field, tangent, parameterization: str = None, convention: str = None, degrees: bool = False,
+                     calibration: RigidTransform = None, n_points: int = 500, alphamin=None, alphamax=None, **kwargs):
+        """(img, dimg), both (B, 1, H, W): the render_deformed image, bit for bit, and its directional derivative along the field
+        tangent `tangent` (DESIGN.md 6k), from one march: dimg = d/dh render_deformed(field + h tangent) at h = 0, with the rays
+        and the sampling range held fixed (they do not depend on the field).  tangent: world mm, the same shape, dtype and device
+        as `field`.  Arguments and coverage as in render_deformed (shared or per-pose fields, full, sub-sampled and patched
+        detectors, fp32 / fp16 / bf16 densities); anything else, or a tangent that does not match the field, raises before any
+        launch.  Detached results; no host synchronisation."""
+        from .deform import deformed_jvp
+
+        return deformed_jvp(self, *args, field=field, tangent=tangent, parameterization=parameterization, convention=convention,
+                            degrees=degrees, calibration=calibration, n_points=n_points, alphamin=alphamin, alphamax=alphamax,
+                            **kwargs)
+
     # ---- fused pose-in path (SURVEY.md 8f-2) ------------------------------------------------------------------
     def _pose_in_ok(self, mask_to_channels, kwargs) -> bool:
         """True when the whole pose -> rays -> Siddon chain can run as ONE kernel with in-kernel ray generation."""

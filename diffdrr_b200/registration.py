@@ -386,3 +386,230 @@ class PolyrigidLevenbergMarquardt:
                                                             **self.kw))
             self.damping, loss = _motion_lm_update(X, A, g, self.damping, self.pivots, self.shared, self._loss(img), trial)
             return loss
+
+
+def ncc_z(x, eps):
+    """(z, sigma) of the global NCC per row of x (B, N): z = (x - mean x) / sigma, sigma = sqrt(var x + eps) (population variance,
+    as metrics.NormalizedCrossCorrelation2d.norm); sigma (B, 1)."""
+    mu = x.mean(-1, keepdim=True)
+    sigma = (x.var(-1, keepdim=True, correction=0) + eps).sqrt()
+    return (x - mu) / sigma, sigma
+
+
+def ncc_z_jvp(y, z, sigma):
+    """The Jacobian of z(x) (ncc_z) at the x with (z, sigma), applied to y (B, N): (y - mean y - z <z, y> / N) / sigma.  The
+    matrix is symmetric, so this is also its transpose (DESIGN.md 6k)."""
+    N = y.shape[-1]
+    return (y - y.mean(-1, keepdim=True) - z * (z * y).sum(-1, keepdim=True) / N) / sigma
+
+
+def field_smoothness(U):
+    """R(U) = sum_a mean((U[.., i + 1, ..] - U[.., i, ..])^2) over the three lattice axes, the squared differences of neighbouring
+    nodes; U (S, 3, g0, g1, g2) -> (S,).  Axes of one node contribute nothing."""
+    R = U.new_zeros(U.shape[0])
+    for ax in (2, 3, 4):
+        if U.shape[ax] > 1:
+            R = R + (U.diff(dim=ax) ** 2).flatten(1).mean(1)
+    return R
+
+
+def field_smoothness_grad(U):
+    """dR/dU of field_smoothness, in closed form; U (S, 3, g0, g1, g2).  R is quadratic, so this is also its Hessian applied to U."""
+    G = torch.zeros_like(U)
+    for ax in (2, 3, 4):
+        g = U.shape[ax]
+        if g > 1:
+            d = U.diff(dim=ax)
+            c = d * (2.0 / d[0].numel())
+            G.narrow(ax, 1, g - 1).add_(c)
+            G.narrow(ax, 0, g - 1).sub_(c)
+    return G
+
+
+def batched_cg(H, b, mu, iters):
+    """`iters` conjugate-gradient iterations on the S systems (H + mu_s I) x_s = b_s from x = 0; b (S, ...), mu (S,) and H a
+    symmetric positive semi-definite product (S, ...) -> (S, ...).  A system whose residual vanishes or whose curvature
+    p^T (H + mu I) p is not positive stops where it is: fixed work, no host sync and no NaN."""
+    S = b.shape[0]
+
+    def dot(a, c):
+        return (a * c).reshape(S, -1).sum(1)
+
+    def each(s):
+        return s.reshape(S, *[1] * (b.dim() - 1))
+
+    x, r = torch.zeros_like(b), b.clone()
+    p, rr = r.clone(), dot(r, r)
+    active = rr > 0
+    for _ in range(iters):
+        Ap = H(p) + each(mu.to(b.dtype)) * p
+        pAp = dot(p, Ap)
+        active = active & (pAp > 0) & torch.isfinite(pAp)
+        a = torch.where(active, rr / torch.where(active, pAp, torch.ones_like(pAp)), torch.zeros_like(pAp))
+        on = each(active)
+        x = torch.where(on, x + each(a) * p, x)
+        r = torch.where(on, r - each(a) * Ap, r)
+        rr_new = dot(r, r)
+        beta = torch.where(active, rr_new / torch.where(rr > 0, rr, torch.ones_like(rr)), torch.zeros_like(rr))
+        p = torch.where(on, r + each(beta) * p, p)
+        rr = torch.where(active, rr_new, rr)
+        active = active & (rr > 0)
+    return x
+
+
+class DeformableLevenbergMarquardt:
+    """Levenberg-Marquardt registration of the displacement field of a deformable DRR (DRR.render_deformed) towards `target`, with
+    the camera pose fixed (DESIGN.md 6k).
+
+    The objective is E(U) = mean over the views of (1 - NCC(target, img)) + smoothness R(U), R the squared differences of
+    neighbouring nodes (field_smoothness).  `field` (3, g0, g1, g2) in world mm is shared by the B views (one objective);
+    (B, 3, g0, g1, g2) gives B independent objectives, each with its own view.  It is a fp32 tensor on the density's device,
+    updated in place by step().
+
+    A field has 3 g0 g1 g2 unknowns, far too many for a dense Jacobian, so the Gauss-Newton system is used matrix-free: per view
+    the residual is r = z(img) - z(target) with the global NCC's z, M its Jacobian (ncc_z_jvp), and
+        g = (1/B) sum_b (1/N) J_b^T M_b r_b + smoothness grad R(U),
+        H v = (1/B) sum_b (1/N) J_b^T M_b^2 J_b v + smoothness grad R(v),
+    (1/B dropped for per-pose fields), J v from the tangent march (b200drr_deform_jvp) and J^T w from the field scatter of
+    b200drr_deform_bwd.  Each step runs `cg_iters` conjugate-gradient iterations on (H + mu I) delta = -g from delta = 0
+    (batched_cg: one system for a shared field, B for per-pose ones), renders one trial image at U + delta with render_deformed
+    and keeps it where the true E is lower (mu / 10 on accept, x 10 on reject).  mu is identity damping; the first step sets
+    mu = damping g^T H g / g^T g, so `damping` is dimensionless.  The accepted trial image is the next step's image, so a step
+    costs 2 cg_iters + 1 marches and one forward.  The rays and the sampling range do not depend on the field: the model is the
+    image's full derivative.  No host sync once warm.
+
+    Only the global NCC is modelled: `loss` None (NormalizedCrossCorrelation2d(eps=eps)) or a NormalizedCrossCorrelation2d
+    without patch_size; anything else raises TypeError here.  Full detectors only."""
+
+    def __init__(self, drr, rot: torch.Tensor, xyz: torch.Tensor, field: torch.Tensor, target: torch.Tensor,
+                 smoothness: float = 1e-3, cg_iters: int = 10, parameterization: str = "euler_angles", convention: str | None = None,
+                 degrees: bool = False, calibration=None, n_points: int = 500, alphamin=None, alphamax=None, loss=None,
+                 damping: float = 1e-3, eps: float = 1e-5):
+        from . import _lib
+        from .deform import _marches, check_supported
+        from .metrics import NormalizedCrossCorrelation2d
+        from .structures import _batch_size
+
+        if loss is None:
+            loss = NormalizedCrossCorrelation2d(eps=eps)
+        elif type(loss) is not NormalizedCrossCorrelation2d or loss.patch_size is not None:
+            raise TypeError(f"DeformableLevenbergMarquardt models the global NCC only: NormalizedCrossCorrelation2d without "
+                            f"patch_size (or loss=None), not {type(loss).__name__}"
+                            f"{'' if getattr(loss, 'patch_size', None) is None else f'(patch_size={loss.patch_size})'}; patch-wise, "
+                            f"multiscale and gradient NCC have no Gauss-Newton model here (use a first-order optimizer)")
+        if not torch.is_tensor(target) or target.dim() != 4 or target.shape[1] != 1:
+            raise ValueError(f"DeformableLevenbergMarquardt takes a one-channel target image (B, 1, H, W), got "
+                             f"{tuple(target.shape) if torch.is_tensor(target) else type(target).__name__}")
+        det = drr.detector
+        if det.n_subsample is not None or drr.patch_size is not None:
+            raise NotImplementedError("DeformableLevenbergMarquardt covers the full detector only, not p_subsample or patch_size")
+        if tuple(target.shape[-2:]) != (det.height, det.width):
+            raise ValueError(f"the target {tuple(target.shape)} does not match the {det.height} x {det.width} detector")
+        B = _batch_size((rot, xyz), parameterization)
+        if target.shape[0] not in (1, B):
+            raise ValueError(f"the target's batch ({target.shape[0]}) must be 1 or the number of poses ({B})")
+        check_supported(drr, (rot, xyz), parameterization, field, {})
+        if not (target.is_cuda and target.dtype == torch.float32):
+            raise ValueError("DeformableLevenbergMarquardt runs on the GPU: the target must be a CUDA fp32 tensor")
+        if not (isinstance(cg_iters, int) and cg_iters >= 1):
+            raise ValueError(f"cg_iters must be a positive int, got {cg_iters!r}")
+        self.drr, self.rot, self.xyz, self.field = drr, rot.detach(), xyz.detach(), field
+        self.kw = dict(parameterization=parameterization, convention=convention, degrees=degrees, calibration=calibration,
+                       n_points=n_points, alphamin=alphamin, alphamax=alphamax)
+        self.loss, self.eps = loss, float(loss.eps)
+        self.smoothness, self.cg_iters, self.damping = float(smoothness), cg_iters, float(damping)
+        self.shared = field.dim() == 4
+        self.B, self.N = B, det.height * det.width
+        self.target = target.detach().expand(B, 1, det.height, det.width).contiguous()
+        # the views' residual weights 1 / N, and 1 / B for the mean over the views of a shared field's one objective
+        self._wt = 1.0 / (self.N * (B if self.shared else 1))
+        with torch.no_grad():
+            self._zt = ncc_z(self.target.reshape(B, self.N), self.eps)[0]
+            source, marches = _marches(drr, (self.rot, self.xyz), B, parameterization, convention, degrees, calibration, alphamin,
+                                       alphamax)
+        self._rays = (source, *marches[0])
+        lib = _lib.load()
+        self._scratch = torch.empty(int(lib.b200drr_deform_scratch_floats(B, self.N, det.height, det.width)), dtype=torch.float32,
+                                    device=field.device)
+        self._lin = drr._affine_inverse.reshape(4, 4)[:3, :3].to(field.dtype)
+        self.mu = None     # (S,) identity damping, set on the first step
+        self._img = None   # the image at the current field (B, 1, H, W)
+
+    def _systems(self, U):
+        """U's shape -> (S, 3, g0, g1, g2): one system for a shared field, B for per-pose ones."""
+        return U[None] if self.shared else U
+
+    def _render(self, U):
+        from .deform import render_deformed
+        return render_deformed(self.drr, self.rot, self.xyz, field=U, **self.kw)
+
+    def _objective(self, img, Us):
+        """E of each system (S,) at the image `img` and the system-batched field Us."""
+        ncc = 1.0 - self.loss(self.target, img)
+        return (ncc.mean(0, keepdim=True) if self.shared else ncc) + self.smoothness * field_smoothness(Us)
+
+    def _model(self, Us, img):
+        """(grad, H) of the Gauss-Newton model at the system-batched field Us and its image: grad() -> g (S, 3, g0, g1, g2) (one
+        scatter march) and the product H(v) on the same shape (two marches)."""
+        from .deform import field_jvp, field_vjp, voxel_field
+
+        drr, packed = self.drr, self.drr.renderer._packed_volume(self.drr.density)
+        source, tgt, lens, arange, grid = self._rays
+        n_points = int(self.kw["n_points"])
+        Uv = voxel_field(drr, Us)
+        z, sigma = ncc_z(img.reshape(self.B, self.N), self.eps)
+
+        def JT(w):
+            gv = field_vjp(drr, packed, source, tgt, lens, Uv, w, arange, n_points, grid, scratch=self._scratch)
+            return torch.einsum("ij,bxyzi->bjxyz", self._lin, gv[..., :3])
+
+        def H(v):
+            jv = field_jvp(drr, packed, source, tgt, lens, Uv, voxel_field(drr, v), arange, n_points, grid)
+            return JT(self._wt * ncc_z_jvp(ncc_z_jvp(jv, z, sigma), z, sigma)) + self.smoothness * field_smoothness_grad(v)
+
+        def grad():
+            return JT(self._wt * ncc_z_jvp(z - self._zt, z, sigma)) + self.smoothness * field_smoothness_grad(Us)
+
+        return grad, H
+
+    def _current_image(self):
+        if self._img is None:
+            self._img = self._render(self.field.detach())
+        return self._img
+
+    def gradient(self) -> torch.Tensor:
+        """The model's gradient g at the current field, in the field's shape (world mm)."""
+        with torch.no_grad():
+            grad, _ = self._model(self._systems(self.field.detach()), self._current_image())
+            return grad().reshape(self.field.shape)
+
+    def product(self, v: torch.Tensor) -> torch.Tensor:
+        """The model's Gauss-Newton product H v at the current field, v and H v in the field's shape (world mm)."""
+        with torch.no_grad():
+            _, H = self._model(self._systems(self.field.detach()), self._current_image())
+            return H(self._systems(v)).reshape(self.field.shape)
+
+    def step(self) -> torch.Tensor:
+        """One damped Gauss-Newton step; -> E after it: a 0-d tensor for a shared field, the per-pose (B,) objectives
+        otherwise."""
+        U = self.field
+        with torch.no_grad():
+            img = self._current_image()
+            Us = self._systems(U.detach())
+            grad, H = self._model(Us, img)
+            g, S = grad(), Us.shape[0]
+            if self.mu is None:
+                gg, gHg = (g * g).reshape(S, -1).sum(1), (g * H(g)).reshape(S, -1).sum(1)
+                self.mu = torch.where(gg > 0, self.damping * gHg / torch.where(gg > 0, gg, torch.ones_like(gg)),
+                                      torch.full_like(gg, self.damping)).clamp(1e-12, 1e12)
+            delta = batched_cg(H, -g, self.mu, self.cg_iters)
+            Us_t = Us + delta
+            U_t = Us_t.reshape(U.shape)
+            img_t = self._render(U_t)
+            E, E_t = self._objective(img, Us), self._objective(img_t, Us_t)
+            accept = E_t < E  # a NaN trial is rejected
+            U.copy_(torch.where(accept.reshape(-1, *[1] * 4), Us_t, Us).reshape(U.shape))
+            self._img = torch.where(accept.reshape(-1, 1, 1, 1), img_t, img)
+            self.mu = torch.where(accept, self.mu / 10.0, self.mu * 10.0).clamp(1e-12, 1e12)
+            out = torch.where(accept, E_t, E)
+            return out[0] if self.shared else out

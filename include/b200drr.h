@@ -780,6 +780,27 @@ int b200drr_deform_bwd_v16(const void *vol, const void *packed, int vol_type, in
                            float *g_tgt, float *g_raylen, float *g_field, float *g_alpha_range, float *scratch, int B, int64_t N, int H,
                            int W, float voxel_shift, float eps, int n_points, const float *alpha_range, void *stream);
 
+/*
+ * Directional derivative of the deformable render along a field tangent (DESIGN.md 6k), for matrix-free Gauss-Newton on the
+ * field.  Arguments as b200drr_deform_fwd's, plus tangent [Bf][g0][g1][g2][4] in the field's layout (voxel-index units, the same
+ * Bf, 16-byte aligned; lane 3 is ignored).  Per ray, with x_m, y_m = x_m + u(x_m) and step as in b200drr_deform_fwd:
+ *     jv = raylen * step * sum_m grad tri(V)(y_m) . v(x_m),
+ * summed over the samples whose x_m lies inside the lattice's support and whose y_m lies inside the padded volume: the image's
+ * derivative along v with the rays and the sampling range held fixed.  It is the transpose of b200drr_deform_bwd's field scatter:
+ * sum_n gout_n jv_n = <g_field, tangent> (lanes 0..2) to fp32 reordering.  Outputs, OVERWRITTEN: jv [B][N]; img [B][N] (NULL
+ * skips it), b200drr_deform_fwd's out bit for bit.  One value per ray, no atomics: both repeat bit for bit.  A NULL tangent or
+ * jv, a misaligned tangent or a bad vol_type returns B200DRR_EINVAL, and the field and ray checks are b200drr_deform_fwd's.  The
+ * library allocates nothing.  The _v16 twin reads a 16-bit volume and equals the fp32 call on the up-cast volume.
+ */
+int b200drr_deform_jvp(const float *vol, const float *packed, int D0, int D1, int D2, const float *src, const float *tgt,
+                       const float *raylen, const float *field, int Bf, int g0, int g1, int g2, const float *tangent, float *img,
+                       float *jv, int B, int64_t N, int H, int W, float voxel_shift, float eps, int n_points, const float *alpha_range,
+                       void *stream);
+int b200drr_deform_jvp_v16(const void *vol, const void *packed, int vol_type, int D0, int D1, int D2, const float *src, const float *tgt,
+                           const float *raylen, const float *field, int Bf, int g0, int g1, int g2, const float *tangent, float *img,
+                           float *jv, int B, int64_t N, int H, int W, float voxel_shift, float eps, int n_points,
+                           const float *alpha_range, void *stream);
+
 #ifdef __cplusplus
 }
 #endif

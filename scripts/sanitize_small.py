@@ -151,4 +151,14 @@ for dtype in (torch.float32, torch.bfloat16):
                                                parameterization="euler_angles", convention="ZXY")
         torch.cuda.synchronize()
         print("polyrigid_jac", dtype, shape, "ok", float(img.sum()), float(J.abs().max()), rects.tolist())
+# deformable tangent march (deform.cu: deform_jvp_kernel): the 23 x 23 detector (partial 16 x 8 tiles), p_subsample (128-ray
+# chunks), per-pose and shared fields that pull samples out of the volume and back, fp32 and bf16 densities
+for kw, dtype in ((dict(), torch.float32), (dict(p_subsample=0.37), torch.float32), (dict(), torch.bfloat16)):
+    drr = DRR(synthetic.make_subject(vol), **synthetic.detector_kwargs(23), renderer="trilinear", **kw).to(dev)
+    drr.density = drr.density.to(dtype)
+    for shape in ((rot.shape[0], 3, 7, 5, 9), (3, 7, 5, 9)):
+        u, v = (torch.rand(*shape, device=dev) - 0.5) * 80.0, torch.rand(*shape, device=dev) - 0.5
+        img, dimg = drr.deformed_jvp(rot, xyz, field=u, tangent=v, n_points=64, parameterization="euler_angles", convention="ZXY")
+        torch.cuda.synchronize()
+        print("deform_jvp", kw, dtype, shape, "ok", float(img.sum()), float(dimg.abs().max()))
 print("done")

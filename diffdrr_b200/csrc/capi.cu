@@ -1053,15 +1053,23 @@ int b200drr_polyrigid_jac_v16(const void* vol, const void* packed, int vol_type,
 // ---- deformable (dense displacement field) trilinear render (deform.cu) ------------------------------------------------------------
 namespace {
 // the checks every deform entry point shares; 0 = go on
-int deform_bad(const void* vol, const void* packed, int D0, int D1, int D2, const float* src, const float* tgt, const float* raylen,
-               const float* field, int Bf, int g0, int g1, int g2, int B, int64_t N, int H, int W, int n_points, const float* alpha_range)
+// the geometry and field checks, without the volume
+int deform_geom_bad(int D0, int D1, int D2, const float* src, const float* tgt, const float* raylen, const float* field, int Bf, int g0,
+                    int g1, int g2, int B, int64_t N, int H, int W, int n_points, const float* alpha_range)
 {
-    if ((vol == nullptr) == (packed == nullptr) || !src || !tgt || !raylen || !field || !alpha_range || bad_dims(D0, D1, D2) ||
-        bad_dims(g0, g1, g2) || bad_rays(B, N) || (Bf != 1 && Bf != B) || n_points < 2 || H < 0 || W < 0 ||
-        ((H > 0 || W > 0) && (int64_t)H * W != N) || (((uintptr_t)field | (uintptr_t)packed) & 15u) != 0)
+    if (!src || !tgt || !raylen || !field || !alpha_range || bad_dims(D0, D1, D2) || bad_dims(g0, g1, g2) || bad_rays(B, N) ||
+        (Bf != 1 && Bf != B) || n_points < 2 || H < 0 || W < 0 || ((H > 0 || W > 0) && (int64_t)H * W != N) ||
+        ((uintptr_t)field & 15u) != 0)
         return B200DRR_EINVAL;
     if (too_big(D0, D1, D2) || (int64_t)g0 * g1 * g2 * 4 >= (int64_t)INT32_MAX) return B200DRR_EUNSUPPORTED;
     return 0;
+}
+
+int deform_bad(const void* vol, const void* packed, int D0, int D1, int D2, const float* src, const float* tgt, const float* raylen,
+               const float* field, int Bf, int g0, int g1, int g2, int B, int64_t N, int H, int W, int n_points, const float* alpha_range)
+{
+    if ((vol == nullptr) == (packed == nullptr) || ((uintptr_t)packed & 15u) != 0) return B200DRR_EINVAL;
+    return deform_geom_bad(D0, D1, D2, src, tgt, raylen, field, Bf, g0, g1, g2, B, N, H, W, n_points, alpha_range);
 }
 }  // namespace
 
@@ -1142,6 +1150,17 @@ int b200drr_deform_jvp_v16(const void* vol, const void* packed, int vol_type, in
         return bad;
     return ret(launch_deform_jvp(vol, packed, vol_type, mk(D0, D1, D2), src, tgt, raylen, field, Bf, g0, g1, g2, tangent, img, jv, B, N,
                                  W, voxel_shift, eps, n_points, alpha_range, (cudaStream_t)stream));
+}
+
+int b200drr_deform_bproj(int D0, int D1, int D2, const float* src, const float* tgt, const float* raylen, const float* field, int Bf,
+                         int g0, int g1, int g2, const float* gout, float* g_vol, int B, int64_t N, int H, int W, float voxel_shift,
+                         float eps, int n_points, const float* alpha_range, void* stream)
+{
+    if (!gout || !g_vol) return B200DRR_EINVAL;
+    if (const int bad = deform_geom_bad(D0, D1, D2, src, tgt, raylen, field, Bf, g0, g1, g2, B, N, H, W, n_points, alpha_range))
+        return bad;
+    return ret(launch_deform_bproj(mk(D0, D1, D2), src, tgt, raylen, field, Bf, g0, g1, g2, gout, g_vol, B, N, W, voxel_shift, eps,
+                                   n_points, alpha_range, (cudaStream_t)stream));
 }
 
 #ifdef B200DRR_EXPERIMENTS

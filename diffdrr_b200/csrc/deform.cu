@@ -5,7 +5,8 @@
 // polyrigid_finish_kernel (polyrigid.cu), and g_tgt / g_raylen are per ray, so all of them repeat bit for bit.  The field gradient
 // is the one output accumulated with atomics (vector reductions, one per lattice node and flush): it repeats to fp32 reordering.
 // The tangent (JVP) kernel writes one image value and one directional derivative per ray, with no shared memory and no atomics,
-// so both repeat bit for bit.
+// so both repeat bit for bit.  The backprojection kernel (the forward's transpose in the density) scatters into one volume gradient
+// with scalar reductions, shared and per-pose fields alike: it repeats to fp32 reordering.
 #include "deform_math.cuh"
 #include "kernels.h"
 
@@ -108,6 +109,25 @@ __global__ void __launch_bounds__(kDeformThreads) deform_jvp_kernel(Gather gathe
     const float Ls = __ldg(raylen + r) * step;
     jv[r] = d * Ls;
     if (img) img[r] = acc * Ls;
+}
+
+// g_vol [D0][D1][D2] += the transpose of deform_fwd_kernel in the density, for upstream gradient gout (deform_ray_bproj)
+__global__ void __launch_bounds__(kDeformThreads) deform_bproj_kernel(VolDims dims, PolyLattice lat, int Bf, const float* __restrict__ src,
+                                                                      const float* __restrict__ tgt, const float* __restrict__ raylen,
+                                                                      const float* __restrict__ gout, float* g_vol, int64_t N, int W,
+                                                                      float shift, float eps, int P, const float* __restrict__ alpha_range)
+{
+    const int b = blockIdx.y;
+    const int64_t n = tiled_ray_index(N, W);
+    if (n < 0) return;
+    const int64_t r = (int64_t)b * N + n;
+    const float amin = __ldg(alpha_range), amax = __ldg(alpha_range + 1);
+    const float step = (amax - amin) / (float)(P - 1);
+    const float c = __ldg(gout + r) * __ldg(raylen + r) * step;
+    if (c == 0.0f) return;  // every add would be a zero
+    if (Bf != 1) lat.w += (int64_t)b * lat.g[0] * lat.g[1] * lat.g[2];
+    const Ray ray = load_ray(src, tgt, b, r, eps);
+    deform_ray_bproj(dims, lat, ray, shift, P, amin, amax, c, g_vol);
 }
 
 int64_t deform_scratch_floats(int B, int64_t N, int W)
@@ -214,6 +234,19 @@ cudaError_t launch_deform_jvp(const void* vol, const void* packed, int vol_type,
 {
     const DeformCall c{dims, src, tgt, raylen, field, Bf, g0, g1, g2, B, N, W, shift, eps, n_points, alpha_range, stream};
     return with_gather(vol, packed, vol_type, [&](auto gather) { return run_jvp(gather, c, tangent, img, jv); });
+}
+
+cudaError_t launch_deform_bproj(VolDims dims, const float* src, const float* tgt, const float* raylen, const float* field, int Bf, int g0,
+                                int g1, int g2, const float* gout, float* g_vol, int B, int64_t N, int W, float shift, float eps,
+                                int n_points, const float* alpha_range, cudaStream_t stream)
+{
+    const size_t bytes = sizeof(float) * (size_t)dims.d[0] * dims.d[1] * dims.d[2];
+    const cudaError_t e = cudaMemsetAsync(g_vol, 0, bytes, stream);
+    if (e != cudaSuccess) return e;
+    const PolyLattice lat = make_lattice(field, g0, g1, g2, dims);
+    deform_bproj_kernel<<<tiled_ray_grid(B, N, W), kDeformThreads, 0, stream>>>(dims, lat, Bf, src, tgt, raylen, gout, g_vol, N, W, shift,
+                                                                                eps, n_points, alpha_range);
+    return cudaGetLastError();
 }
 
 }  // namespace b200drr

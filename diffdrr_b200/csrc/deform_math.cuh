@@ -9,7 +9,9 @@
 //
 // The backward scatters d I / d u into a lattice gradient with one vector reduction per lattice node and flush (deform_red4): the
 // field gradient repeats only to fp32 reordering of those adds.  Every other output is a per-ray value.  The tangent march
-// (deform_ray_jvp) is the scatter's transpose: the image's derivative along a field direction, one value per ray.
+// (deform_ray_jvp) is the scatter's transpose: the image's derivative along a field direction, one value per ray.  The
+// backprojection (deform_ray_bproj) is the forward's transpose in the density: 8 scalar reductions per in-volume sample into a
+// volume gradient, with no density read.
 #pragma once
 
 #include "polyrigid_math.cuh"
@@ -210,6 +212,50 @@ B200_HD float deform_ray_jvp(const Gather& gather, const VolDims& dims, const Po
     }
     img = acc;
     return jv;
+}
+
+// Transpose of deform_ray_fwd in the density (DESIGN.md 6l): deform_ray_fwd's samples, through the same arithmetic, each adding
+//   g_vol[corner] += c tri_weight(corner, y_m)
+// to the in-bounds corners of the cell around y_m, for every y_m inside the padded volume (x_m inside the lattice's support or
+// not: u = 0 there and y_m = x_m).  The cell and the fractions are gather8's, the weights trilinear_ray_bwd_g's product, so with
+// u = 0 every add is that kernel's volume-gradient add bit for bit.  c = gout raylen step; no density is read.
+B200_HD void deform_ray_bproj(const VolDims& dims, const PolyLattice& lat, const Ray& ray, float shift, int P, float amin, float amax,
+                              float c, float* g_vol)
+{
+    const PixLine pl = make_pixline(ray, dims, shift, 0);
+    const float range = amax - amin;
+    const float lstep = 1.0f / (float)(P - 1);
+    int m_lo, m_hi;
+    poly_sample_range(pl, lat, amin, range, P, m_lo, m_hi);
+    for (int m = m_lo; m <= m_hi; ++m) {
+        const float alpha = add_rn(mul_rn(linspace01(m, P, lstep), range), amin);
+        float pix[3], u[4];
+#pragma unroll
+        for (int a = 0; a < 3; ++a) pix[a] = fmaf(alpha, pl.dp[a], pl.p0[a]);
+        if (poly_weights<4, false>(lat, pix, u, nullptr)) {
+#pragma unroll
+            for (int a = 0; a < 3; ++a) pix[a] += u[a];
+        }
+        if (!inside_padded(pix, dims)) continue;
+        float f[3], e[3];
+        int i0[3];
+#pragma unroll
+        for (int a = 0; a < 3; ++a) {
+            const float fl = floorf(pix[a]);
+            f[a] = pix[a] - fl;
+            e[a] = 1.0f - f[a];
+            i0[a] = (int)fl;
+        }
+        const int64_t base = ((int64_t)i0[0] * dims.d[1] + i0[1]) * dims.d[2] + i0[2];
+#pragma unroll
+        for (int k = 0; k < 8; ++k) {
+            const int x = i0[0] + (k & 1), y = i0[1] + ((k >> 1) & 1), z = i0[2] + ((k >> 2) & 1);
+            if ((unsigned)x < (unsigned)dims.d[0] && (unsigned)y < (unsigned)dims.d[1] && (unsigned)z < (unsigned)dims.d[2]) {
+                const float w = ((k & 1) ? f[0] : e[0]) * (((k >> 1) & 1) ? f[1] : e[1]) * (((k >> 2) & 1) ? f[2] : e[2]);
+                red_add(g_vol + base + corner_off(dims, k), c * w);
+            }
+        }
+    }
 }
 
 }  // namespace b200drr

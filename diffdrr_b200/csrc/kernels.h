@@ -318,5 +318,9 @@ cudaError_t launch_deform_jvp(const void* vol, const void* packed, int vol_type,
                               const float* raylen, const float* field, int Bf, int g0, int g1, int g2, const float* tangent, float* img,
                               float* jv, int B, int64_t N, int W, float shift, float eps, int n_points, const float* alpha_range,
                               cudaStream_t stream);
+// the forward's transpose in the density: g_vol [D0][D1][D2], zeroed here, += sum over the rays of gout * d out / d V
+cudaError_t launch_deform_bproj(VolDims dims, const float* src, const float* tgt, const float* raylen, const float* field, int Bf, int g0,
+                                int g1, int g2, const float* gout, float* g_vol, int B, int64_t N, int W, float shift, float eps,
+                                int n_points, const float* alpha_range, cudaStream_t stream);
 
 }  // namespace b200drr

@@ -6,6 +6,9 @@ lattice over the volume (polyrigid.py's convention: node i of axis a at voxel co
 zero outside the lattice).  The kernels take u in voxel-index units, channel-last and padded to 4 channels; that conversion is
 torch ops here, so autograd carries the kernel's field gradient (include/b200drr.h: b200drr_deform_bwd) back to the world-mm field
 and on to whatever produced it.  Nothing is cached and nothing is read on the host: the field changes every optimiser step.
+
+A density passed as `density=` may require grad (fp32): its gradient is the forward's transpose in the density, a backprojection
+along the warped samples (b200drr_deform_bproj; DESIGN.md 6l), for motion-compensated reconstruction.
 """
 from __future__ import annotations
 
@@ -18,8 +21,9 @@ from .renderers import _VOL16, Trilinear, _check_vol16, _dims_tensor, _get_alpha
 from .structures import _batch_size, _camera_pose
 
 
-def check_supported(drr, args, parameterization, field, kwargs):
-    """Refuse, before any launch, what the deformable render does not cover: -> B."""
+def check_supported(drr, args, parameterization, field, kwargs, density=None):
+    """Refuse, before any launch, what the deformable render does not cover: -> B.  density: the volume rendered in place of
+    drr.density (render_deformed's density=), or None."""
     r = drr.renderer
     if not isinstance(r, Trilinear):
         raise NotImplementedError(f"render_deformed supports the Trilinear renderer, not {type(r).__name__}: the displacement field "
@@ -39,11 +43,21 @@ def check_supported(drr, args, parameterization, field, kwargs):
     if 4 * g0 * g1 * g2 >= 2**31 - 1:
         raise NotImplementedError(f"render_deformed takes a lattice below 2^31 floats per pose (4 channels), got {(g0, g1, g2)}")
     vol = drr.density
+    if density is not None:   # the module keeps the geometry (affine, dims); the volume fitted through it is passed in
+        if not torch.is_tensor(density) or density.shape != vol.shape or density.device != vol.device:
+            got = f"{tuple(density.shape)} on {density.device}" if torch.is_tensor(density) else type(density).__name__
+            raise ValueError(f"density must be a tensor of drr.density's shape {tuple(vol.shape)} on its device {vol.device}, got "
+                             f"{got}")
+        vol = density
     if vol.dtype not in (torch.float32, *_VOL16) or vol.dim() != 3 or vol.numel() >= 2**31 - 1:
         raise NotImplementedError(f"render_deformed needs a 3-D fp32 / fp16 / bf16 density below 2^31 voxels, got {vol.dtype} "
                                   f"{tuple(vol.shape)}")
-    if vol.requires_grad:
-        raise NotImplementedError("render_deformed produces no volume gradient: the density must not require grad")
+    if vol.requires_grad and density is None:
+        raise NotImplementedError("render_deformed produces no volume gradient to drr.density: the density must not require grad "
+                                  "(pass the volume to fit as density= instead)")
+    if vol.requires_grad and vol.dtype != torch.float32:
+        raise NotImplementedError(f"render_deformed produces no volume gradient to a {vol.dtype} density: 16-bit volumes are static "
+                                  "densities (optimise an fp32 volume for volume gradients)")
     if not vol.is_cuda:
         raise _lib.B200DRRError(f"diffdrr_b200 renderers run on CUDA devices only (density is on {vol.device}); there is no CPU "
                                 "fallback")
@@ -87,12 +101,21 @@ class _DeformFunction(torch.autograd.Function):
         B, N = tgt.shape[0], tgt.shape[1]
         dev = vol.device
         gout = gout.reshape(B, N).contiguous().float()
+        lib = _lib.load()
+        g_vol = None
+        if ctx.needs_input_grad[0]:   # the forward's transpose in the density: a backprojection, no density read
+            g_vol = torch.empty(vol.shape, dtype=torch.float32, device=dev)
+            with torch.cuda.device(dev):
+                _lib.check(lib.b200drr_deform_bproj(*vol.shape, _ptr(src), _ptr(tgt), _ptr(raylen), _ptr(field), field.shape[0],
+                                                    *field.shape[1:4], _ptr(gout), _ptr(g_vol), B, N, H, W, voxel_shift, eps,
+                                                    n_points, _ptr(arange), _stream()), "b200drr_deform_bproj")
+        if not any(ctx.needs_input_grad[2:7]):   # a reconstruction step: the density is the only input that wants a gradient
+            return g_vol, None, None, None, None, None, None, None, None, None, None
         g_src = torch.empty(B, 3, dtype=torch.float32, device=dev)
         g_tgt = torch.empty(B, N, 3, dtype=torch.float32, device=dev)
         g_raylen = torch.empty(B, N, dtype=torch.float32, device=dev)
         g_field = torch.empty_like(field) if ctx.needs_input_grad[5] else None   # NULL: the kernel skips the scatter
         g_range = torch.empty(2, dtype=torch.float32, device=dev)
-        lib = _lib.load()
         scratch = torch.empty(int(lib.b200drr_deform_scratch_floats(B, N, H, W)), dtype=torch.float32, device=dev)
         fn, head, name = _vol_entry(lib, "b200drr_deform_bwd", vol)
         head = (_ptr(vol) if packed is None else None, _ptr(packed), *head[1:])
@@ -100,7 +123,7 @@ class _DeformFunction(torch.autograd.Function):
             _lib.check(fn(*head, *vol.shape, _ptr(src), _ptr(tgt), _ptr(raylen), _ptr(field), field.shape[0], *field.shape[1:4],
                           _ptr(gout), _ptr(g_src), _ptr(g_tgt), _ptr(g_raylen), _ptr(g_field), _ptr(g_range), _ptr(scratch),
                           B, N, H, W, voxel_shift, eps, n_points, _ptr(arange), _stream()), name)
-        return None, None, g_src.view(source_shape), g_tgt, g_raylen.view(img_shape), g_field, g_range, None, None, None, None
+        return g_vol, None, g_src.view(source_shape), g_tgt, g_raylen.view(img_shape), g_field, g_range, None, None, None, None
 
 
 def voxel_field(drr, field):
@@ -112,12 +135,13 @@ def voxel_field(drr, field):
     return torch.nn.functional.pad(u, (0, 1)).contiguous()
 
 
-def _marches(drr, args, B, parameterization, convention, degrees, calibration, alphamin, alphamax):
+def _marches(drr, args, B, parameterization, convention, degrees, calibration, alphamin, alphamax, vol=None):
     """The rays of a deformable render in voxel-index space -> (source (B, 1, 3), [(target, raylen, alpha_range, grid), ...]): one
     march for the full or sub-sampled detector, one per patch for patch_size (as DRR.render), each with its own sampling range
     (the batch-global range of its rays, as Trilinear.forward, unless alphamin / alphamax fix it) and, for a full detector grid,
-    its (H, W).  Torch ops, differentiable in the camera pose and the calibration."""
-    vol, r = drr.density, drr.renderer
+    its (H, W).  Torch ops, differentiable in the camera pose and the calibration.  vol: the density rendered (default
+    drr.density)."""
+    vol, r = drr.density if vol is None else vol, drr.renderer
     P = _camera_pose(args, B, parameterization, convention, degrees)
     source, target = drr.detector(RigidTransform(P), calibration)
     img = (target - source).norm(dim=-1).unsqueeze(1)
@@ -144,11 +168,11 @@ def _marches(drr, args, B, parameterization, convention, degrees, calibration, a
 
 
 def render_deformed(drr, *args, field, parameterization=None, convention=None, degrees=False, calibration=None, n_points=500,
-                    alphamin=None, alphamax=None, **kwargs):
+                    alphamin=None, alphamax=None, density=None, **kwargs):
     """See DRR.render_deformed."""
-    B = check_supported(drr, args, parameterization, field, kwargs)
-    vol, r = drr.density, drr.renderer
-    source, marches = _marches(drr, args, B, parameterization, convention, degrees, calibration, alphamin, alphamax)
+    B = check_supported(drr, args, parameterization, field, kwargs, density=density)
+    vol, r = drr.density if density is None else density, drr.renderer
+    source, marches = _marches(drr, args, B, parameterization, convention, degrees, calibration, alphamin, alphamax, vol=vol)
     U = voxel_field(drr, field)
     packed = r._packed_volume(vol)
     outs = [_DeformFunction.apply(vol, packed, source, tgt, lens, U, alpha_range, float(r.voxel_shift), float(r.eps), int(n_points),

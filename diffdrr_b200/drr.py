@@ -241,7 +241,8 @@ class DRR(nn.Module):
                                   alphamin=alphamin, alphamax=alphamax, return_footprints=return_footprints, **kwargs)
 
     def render_deformed(self, *args, field, parameterization: str = None, convention: str = None, degrees: bool = False,
-                        calibration: RigidTransform = None, n_points: int = 500, alphamin=None, alphamax=None, **kwargs):
+                        calibration: RigidTransform = None, n_points: int = 500, alphamin=None, alphamax=None, density=None,
+                        **kwargs):
         """Deformable DRR (DESIGN.md 6i) -> (B, 1, H, W): the volume under a dense displacement field, marched with the Trilinear
         renderer's rays and samples.
 
@@ -249,14 +250,21 @@ class DRR(nn.Module):
         (the rendered density at world point p is the CT density at p + u(p)) on a lattice over the volume whose node i of axis a
         sits at voxel coordinate (i + 1/2) D_a / g_a - 1/2, interpolated trilinearly and zero outside the lattice.  It may
         require grad.  The camera pose `*args`, calibration, n_points and alphamin / alphamax mean what they do in forward.
-        Gradients reach the field, the camera pose and the calibration; the density gets none.  Supported: Trilinear with default
-        options, fp32 / fp16 / bf16 densities, the full detector, p_subsample and patch_size; anything else raises before any
-        launch.  No host synchronisation."""
+
+        density: a volume rendered in place of self.density (the reconstruction idiom: the module keeps the geometry, the fitted
+        volume is passed in), of self.density's shape and on its device (ValueError otherwise), fp32 / fp16 / bf16.  An fp32
+        density may require grad: its gradient is the render's transpose in the density, a backprojection along the warped
+        samples (DESIGN.md 6l), so a volume can be fitted to projections taken under known per-view motion (motion-compensated
+        reconstruction), alone or jointly with the field and the camera.
+
+        Gradients reach the field, the camera pose, the calibration and a `density=` volume that requires grad; self.density gets
+        none (it must not require grad).  Supported: Trilinear with default options, fp32 / fp16 / bf16 densities, the full
+        detector, p_subsample and patch_size; anything else raises before any launch.  No host synchronisation."""
         from .deform import render_deformed
 
         return render_deformed(self, *args, field=field, parameterization=parameterization, convention=convention,
                                degrees=degrees, calibration=calibration, n_points=n_points, alphamin=alphamin,
-                               alphamax=alphamax, **kwargs)
+                               alphamax=alphamax, density=density, **kwargs)
 
     def deformed_jvp(self, *args, field, tangent, parameterization: str = None, convention: str = None, degrees: bool = False,
                      calibration: RigidTransform = None, n_points: int = 500, alphamin=None, alphamax=None, **kwargs):

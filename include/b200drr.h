@@ -761,7 +761,8 @@ int b200drr_polyrigid_jac_v16(const void *vol, const void *packed, int vol_type,
  * g_tgt [B][N][3], g_raylen [B][N], g_alpha_range [2] (as b200drr_polyrigid_bwd's) and g_field, the field's layout, 16-byte
  * aligned; lane 3 is written 0.  The entry zeroes g_field on the stream and then adds every ray's contribution with vector atomics,
  * so g_field repeats only to fp32 reordering; every other output repeats bit for bit (sums over rays taken from scratch,
- * b200drr_deform_scratch_floats(B, N, H, W) floats, in a fixed order).  g_field == NULL skips the scatter.  No volume gradient.
+ * b200drr_deform_scratch_floats(B, N, H, W) floats, in a fixed order).  g_field == NULL skips the scatter.  The volume gradient is
+ * b200drr_deform_bproj's.
  * The library allocates nothing.  The _v16 twins read a 16-bit volume and equal the fp32 call on the up-cast volume.
  */
 int64_t b200drr_deform_scratch_floats(int B, int64_t N, int H, int W);
@@ -800,6 +801,23 @@ int b200drr_deform_jvp_v16(const void *vol, const void *packed, int vol_type, in
                            const float *raylen, const float *field, int Bf, int g0, int g1, int g2, const float *tangent, float *img,
                            float *jv, int B, int64_t N, int H, int W, float voxel_shift, float eps, int n_points,
                            const float *alpha_range, void *stream);
+
+/*
+ * Backprojection through the deformable render (DESIGN.md 6l): the transpose of b200drr_deform_fwd in the density, for
+ * reconstruction through known (or jointly fitted) displacement fields.  For a fixed camera and field the render is linear in V:
+ *     out = raylen * step * sum_m tri(V, y_m),      y_m = x_m + u(x_m),
+ * so the gradient of sum(gout * out) with respect to V is
+ *     g_vol[corner] = sum over rays and samples of gout * raylen * step * tri_weight(corner, y_m),
+ * over every y_m inside the padded volume (x_m inside the lattice's support or not).  The samples, the field and the range are
+ * b200drr_deform_fwd's; no density is read, so there is no volume argument and no _v16 twin.  gout [B][N]; g_vol [D0][D1][D2],
+ * OVERWRITTEN: the entry zeroes it on the stream, then every pose (shared or per-pose field) adds into it with scalar atomics, so
+ * it repeats only to fp32 reordering.  A NULL gout or g_vol returns B200DRR_EINVAL, and the field and ray checks are
+ * b200drr_deform_fwd's (the field 16-byte aligned, fewer than 2^31 floats per pose), all before touching CUDA.  The library
+ * allocates nothing.
+ */
+int b200drr_deform_bproj(int D0, int D1, int D2, const float *src, const float *tgt, const float *raylen, const float *field, int Bf,
+                         int g0, int g1, int g2, const float *gout, float *g_vol, int B, int64_t N, int H, int W, float voxel_shift,
+                         float eps, int n_points, const float *alpha_range, void *stream);
 
 #ifdef __cplusplus
 }

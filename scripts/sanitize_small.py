@@ -161,4 +161,18 @@ for kw, dtype in ((dict(), torch.float32), (dict(p_subsample=0.37), torch.float3
         img, dimg = drr.deformed_jvp(rot, xyz, field=u, tangent=v, n_points=64, parameterization="euler_angles", convention="ZXY")
         torch.cuda.synchronize()
         print("deform_jvp", kw, dtype, shape, "ok", float(img.sum()), float(dimg.abs().max()))
+# deformable density backprojection (deform.cu: deform_bproj_kernel): the 23 x 23 detector (partial 16 x 8 tiles), p_subsample
+# (128-ray chunks) and patches, per-pose and shared fields that pull samples out of the volume and back, the density alone and
+# jointly with the field
+for kw in (dict(), dict(p_subsample=0.37), dict(patch_size=8, height=24)):
+    kw = dict(kw)
+    drr = DRR(synthetic.make_subject(vol), **synthetic.detector_kwargs(kw.pop("height", 23)), renderer="trilinear", **kw).to(dev)
+    for shape in ((rot.shape[0], 3, 7, 5, 9), (3, 7, 5, 9)):
+        for joint in (False, True):
+            u = ((torch.rand(*shape, device=dev) - 0.5) * 80.0).requires_grad_(joint)
+            V = drr.density.detach().clone().requires_grad_(True)
+            img = drr.render_deformed(rot, xyz, field=u, n_points=64, density=V, parameterization="euler_angles", convention="ZXY")
+            img.sum().backward()
+            torch.cuda.synchronize()
+            print("deform_bproj", kw, shape, joint, "ok", float(img.sum()), float(V.grad.abs().max()))
 print("done")

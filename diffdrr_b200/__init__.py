@@ -17,3 +17,4 @@ from .registration import (  # noqa: F401,E402
 from .structures import structures_jacobian  # noqa: F401,E402
 from .polyrigid import polyrigid_jacobian, polyrigid_weights  # noqa: F401,E402
 from .deform import deformed_jvp  # noqa: F401,E402
+from .svf import exp_velocity  # noqa: F401,E402

@@ -377,6 +377,13 @@ _SIGNATURES = {
         ctypes.c_int, ctypes.c_int, ctypes.c_int, _c_float_p, _c_float_p, _c_float_p, _c_float_p, ctypes.c_int, ctypes.c_int,
         ctypes.c_int, ctypes.c_int, _c_float_p, _c_float_p, ctypes.c_int, ctypes.c_int64, ctypes.c_int, ctypes.c_int, ctypes.c_float,
         ctypes.c_float, ctypes.c_int, _c_float_p, ctypes.c_void_p]),
+    # scaling and squaring of a stationary velocity field
+    "b200drr_svf_square": (ctypes.c_int, [
+        _c_float_p, _c_float_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int,
+        ctypes.c_float, ctypes.c_void_p]),
+    "b200drr_svf_square_bwd": (ctypes.c_int, [
+        _c_float_p, _c_float_p, _c_float_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int,
+        ctypes.c_int, ctypes.c_float, ctypes.c_void_p]),
 }
 
 # entry points of rejected experiments (include/b200drr_experimental.h): bound only when the experimental build is loaded

@@ -1163,6 +1163,35 @@ int b200drr_deform_bproj(int D0, int D1, int D2, const float* src, const float* 
                                    n_points, alpha_range, (cudaStream_t)stream));
 }
 
+// ---- scaling and squaring of a stationary velocity field (svf.cu) ------------------------------------------------------------------
+namespace {
+// the checks both svf entry points share; 0 = go on
+int svf_bad(const float* field, const float* out, int Bf, int g0, int g1, int g2, int D0, int D1, int D2, float scale)
+{
+    if (!field || !out || Bf <= 0 || bad_dims(g0, g1, g2) || bad_dims(D0, D1, D2) || !(scale > 0.0f) ||
+        (((uintptr_t)field | (uintptr_t)out) & 15u) != 0)
+        return B200DRR_EINVAL;
+    if ((int64_t)g0 * g1 * g2 * 4 >= (int64_t)INT32_MAX) return B200DRR_EUNSUPPORTED;
+    return 0;
+}
+}  // namespace
+
+int b200drr_svf_square(const float* field, float* out, int Bf, int g0, int g1, int g2, int D0, int D1, int D2, float scale, void* stream)
+{
+    if (const int bad = svf_bad(field, out, Bf, g0, g1, g2, D0, D1, D2, scale)) return bad;
+    if (field == out) return B200DRR_EINVAL;
+    return ret(launch_svf_square(field, out, Bf, g0, g1, g2, mk(D0, D1, D2), scale, (cudaStream_t)stream));
+}
+
+int b200drr_svf_square_bwd(const float* field, const float* gout, float* gin, int Bf, int g0, int g1, int g2, int D0, int D1, int D2,
+                           float scale, void* stream)
+{
+    if (!gout || (((uintptr_t)gout & 15u) != 0)) return B200DRR_EINVAL;
+    if (const int bad = svf_bad(field, gin, Bf, g0, g1, g2, D0, D1, D2, scale)) return bad;
+    if (gin == field || gin == gout) return B200DRR_EINVAL;
+    return ret(launch_svf_square_bwd(field, gout, gin, Bf, g0, g1, g2, mk(D0, D1, D2), scale, (cudaStream_t)stream));
+}
+
 #ifdef B200DRR_EXPERIMENTS
 int b200drr_x_transpose_volume(const float* vol, int D0, int D1, int D2, int axis, float* out, void* stream)
 {

@@ -323,4 +323,11 @@ cudaError_t launch_deform_bproj(VolDims dims, const float* src, const float* tgt
                                 int g1, int g2, const float* gout, float* g_vol, int B, int64_t N, int W, float shift, float eps,
                                 int n_points, const float* alpha_range, cudaStream_t stream);
 
+// scaling-and-squaring steps of a stationary velocity field (svf.cu).  field / out / gout / gin: [Bf][g0][g1][g2][4], 16-byte
+// aligned; out = one squaring step of field with scale s, gin = its adjoint applied to gout (zeroed on the stream first)
+cudaError_t launch_svf_square(const float* field, float* out, int Bf, int g0, int g1, int g2, VolDims dims, float scale,
+                              cudaStream_t stream);
+cudaError_t launch_svf_square_bwd(const float* field, const float* gout, float* gin, int Bf, int g0, int g1, int g2, VolDims dims,
+                                  float scale, cudaStream_t stream);
+
 }  // namespace b200drr

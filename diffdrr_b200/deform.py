@@ -171,9 +171,15 @@ def render_deformed(drr, *args, field, parameterization=None, convention=None, d
                     alphamin=None, alphamax=None, density=None, **kwargs):
     """See DRR.render_deformed."""
     B = check_supported(drr, args, parameterization, field, kwargs, density=density)
-    vol, r = drr.density if density is None else density, drr.renderer
+    vol = drr.density if density is None else density
+    return render_voxel_field(drr, args, B, voxel_field(drr, field), parameterization, convention, degrees, calibration, n_points,
+                              alphamin, alphamax, vol)
+
+
+def render_voxel_field(drr, args, B, U, parameterization, convention, degrees, calibration, n_points, alphamin, alphamax, vol):
+    """render_deformed after its checks, for the kernels' field U (Bf, g0, g1, g2, 4) in voxel units (voxel_field's output)."""
+    r = drr.renderer
     source, marches = _marches(drr, args, B, parameterization, convention, degrees, calibration, alphamin, alphamax, vol=vol)
-    U = voxel_field(drr, field)
     packed = r._packed_volume(vol)
     outs = [_DeformFunction.apply(vol, packed, source, tgt, lens, U, alpha_range, float(r.voxel_shift), float(r.eps), int(n_points),
                                   grid) for tgt, lens, alpha_range, grid in marches]

@@ -206,12 +206,17 @@ class DRR(nn.Module):
 
     def render_polyrigid(self, *args, motions, weights, parameterization: str = None, convention: str = None,
                          degrees: bool = False, calibration: RigidTransform = None, n_points: int = 500, alphamin=None,
-                         alphamax=None, **kwargs):
-        """Blended-rigid (skinned) DRR (DESIGN.md 6h) -> (B, 1, H, W): the volume deformed by K rigid motions that smooth weights
+                         alphamax=None, blend: str = "linear", steps: int = 10, **kwargs):
+        """Blended-rigid (skinned) DRR (DESIGN.md 6h, 6m) -> (B, 1, H, W): the volume deformed by K rigid motions that smooth weights
         blend into one continuous map, marched with the Trilinear renderer's rays and samples.
 
-        Every sample x reads the density at x + sum_k w_k(x) (M_k x - x), M_k the voxel-space form of X_k^-1: linear blend skinning
-        of the pull-back, rigid wherever one weight is 1 and the identity where all are 0.  motions: (K, 4, 4) shared by the poses
+        blend="linear" (the default): every sample x reads the density at x + sum_k w_k(x) (M_k x - x), M_k the voxel-space form of
+        X_k^-1: linear blend skinning of the pull-back, rigid wherever one weight is 1 and the identity where all are 0.  Between
+        structures with a large relative rotation it loses volume.  blend="log_euclidean": the pull-back is exp(v), v(x) =
+        sum_k w_k(x) log(M_k) [x; 1] on the weight lattice's nodes, exponentiated by `steps` squarings (1..16; DESIGN.md 6m) and
+        marched as render_deformed marches a field: invertible, volume-preserving between structures, and rigid wherever one
+        weight is 1 (up to the squaring's error, which falls 4x per step).  It keeps `steps` lattice-sized fields for the
+        backward.  motions: (K, 4, 4) shared by the poses
         or (B, K, 4, 4) world motions x -> X x as in render_structures (a tensor or a RigidTransform; it may require grad).
         weights: (K, g0, g1, g2) fp32 lattice over the volume with values in [0, 1] and sum_k <= 1, e.g. from
         polyrigid.polyrigid_weights; K <= 8.  The camera pose `*args`, calibration, n_points and alphamin / alphamax mean what they
@@ -222,7 +227,7 @@ class DRR(nn.Module):
 
         return render_polyrigid(self, *args, motions=motions, weights=weights, parameterization=parameterization,
                                 convention=convention, degrees=degrees, calibration=calibration, n_points=n_points,
-                                alphamin=alphamin, alphamax=alphamax, **kwargs)
+                                alphamin=alphamin, alphamax=alphamax, blend=blend, steps=steps, **kwargs)
 
     def polyrigid_jacobian(self, *args, motions, weights, parameterization: str = None, convention: str = None,
                            degrees: bool = False, calibration: RigidTransform = None, n_points: int = 500, alphamin=None,

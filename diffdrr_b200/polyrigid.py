@@ -181,11 +181,20 @@ def voxel_maps(drr, X):
 
 
 def render_polyrigid(drr, *args, motions, weights, parameterization=None, convention=None, degrees=False, calibration=None,
-                     n_points=500, alphamin=None, alphamax=None, **kwargs):
+                     n_points=500, alphamin=None, alphamax=None, blend="linear", steps=10, **kwargs):
     """See DRR.render_polyrigid."""
+    if blend not in ("linear", "log_euclidean"):
+        raise ValueError(f"blend must be 'linear' or 'log_euclidean', got {blend!r}")
+    if blend == "log_euclidean":
+        from . import svf
+
+        svf.check_steps(steps)
     X, B, K = check_supported(drr, args, parameterization, motions, weights, kwargs)
     vol, r = drr.density, drr.renderer
     wpacked = _packed_weights(drr, weights)
+    if blend == "log_euclidean":   # the lattice check above is the linear blend's; the packed copy is not used
+        return svf.render_log_euclidean(drr, args, X, B, weights, steps, parameterization, convention, degrees, calibration,
+                                        n_points, alphamin, alphamax)
     P = _camera_pose(args, B, parameterization, convention, degrees)
     source, target = drr.detector(RigidTransform(P), calibration)
     img = (target - source).norm(dim=-1).unsqueeze(1)

@@ -819,6 +819,27 @@ int b200drr_deform_bproj(int D0, int D1, int D2, const float *src, const float *
                          int g0, int g1, int g2, const float *gout, float *g_vol, int B, int64_t N, int H, int W, float voxel_shift,
                          float eps, int n_points, const float *alpha_range, void *stream);
 
+/*
+ * Scaling and squaring of a stationary velocity field (DESIGN.md 6m): N calls compose exp(v) ~ (id + v / 2^N)^(2^N).
+ * field, out: [Bf][g0][g1][g2][4] fp32, channel-last, voxel-index units, lane 3 zero (b200drr_deform_fwd's field layout; node i
+ * of axis a at voxel coordinate (i + 1/2) D_a / g_a - 1/2 of a D0 x D1 x D2 volume), 16-byte aligned, not aliased.  One step:
+ *     out(x) = s field(x) + s U(x + s field(x)),
+ * U the trilinear interpolant of field with lattice coordinates clamped to the node range per axis; s = scale, 1 / 2^N on the
+ * first step (folding v / 2^N into it) and 1 on the others.  out is OVERWRITTEN, every node once: it repeats bit for bit.
+ *
+ * b200drr_svf_square_bwd: the step's adjoint for an upstream gradient gout on out, into gin (the field's layout, OVERWRITTEN: the
+ * entry zeroes it on the stream): node x gets s gout(x) + s^2 J_U(y)^T gout(x), y = x + s field(x), J_U the interpolant's spatial
+ * gradient (zero along a clamped axis), and each corner node c of y's cell gets s w_c(y) gout(x).  Vector reductions: gin repeats
+ * only to fp32 reordering.  gout, gin 16-byte aligned, gin aliasing neither input.
+ *
+ * A NULL pointer, a non-positive size, a scale that is not positive, a misaligned or aliased array returns B200DRR_EINVAL, and a
+ * lattice of 2^31 floats or more per pose B200DRR_EUNSUPPORTED, all before touching CUDA.  The library allocates nothing.
+ */
+int b200drr_svf_square(const float *field, float *out, int Bf, int g0, int g1, int g2, int D0, int D1, int D2, float scale,
+                       void *stream);
+int b200drr_svf_square_bwd(const float *field, const float *gout, float *gin, int Bf, int g0, int g1, int g2, int D0, int D1, int D2,
+                           float scale, void *stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -13,8 +13,9 @@ from .metrics import (  # noqa: F401,E402
     DoubleGeodesicSE3, GradientNormalizedCrossCorrelation2d, LogGeodesicSE3, MultiscaleNormalizedCrossCorrelation2d,
     MutualInformation, NormalizedCrossCorrelation2d, Sobel)
 from .registration import (  # noqa: F401,E402
-    DeformableLevenbergMarquardt, LevenbergMarquardt, PolyrigidLevenbergMarquardt, Registration, StructuresLevenbergMarquardt)
+    DeformableLevenbergMarquardt, DiffeomorphicLevenbergMarquardt, LevenbergMarquardt, PolyrigidLevenbergMarquardt, Registration,
+    StructuresLevenbergMarquardt)
 from .structures import structures_jacobian  # noqa: F401,E402
 from .polyrigid import polyrigid_jacobian, polyrigid_weights  # noqa: F401,E402
 from .deform import deformed_jvp  # noqa: F401,E402
-from .svf import exp_velocity  # noqa: F401,E402
+from .svf import exp_velocity, exp_velocity_jvp  # noqa: F401,E402

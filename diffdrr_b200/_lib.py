@@ -384,6 +384,9 @@ _SIGNATURES = {
     "b200drr_svf_square_bwd": (ctypes.c_int, [
         _c_float_p, _c_float_p, _c_float_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int,
         ctypes.c_int, ctypes.c_float, ctypes.c_void_p]),
+    "b200drr_svf_square_jvp": (ctypes.c_int, [
+        _c_float_p, _c_float_p, _c_float_p, _c_float_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int,
+        ctypes.c_int, ctypes.c_int, ctypes.c_float, ctypes.c_void_p]),
 }
 
 # entry points of rejected experiments (include/b200drr_experimental.h): bound only when the experimental build is loaded

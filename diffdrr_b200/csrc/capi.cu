@@ -1165,7 +1165,7 @@ int b200drr_deform_bproj(int D0, int D1, int D2, const float* src, const float* 
 
 // ---- scaling and squaring of a stationary velocity field (svf.cu) ------------------------------------------------------------------
 namespace {
-// the checks both svf entry points share; 0 = go on
+// the checks every svf entry point shares; 0 = go on
 int svf_bad(const float* field, const float* out, int Bf, int g0, int g1, int g2, int D0, int D1, int D2, float scale)
 {
     if (!field || !out || Bf <= 0 || bad_dims(g0, g1, g2) || bad_dims(D0, D1, D2) || !(scale > 0.0f) ||
@@ -1190,6 +1190,15 @@ int b200drr_svf_square_bwd(const float* field, const float* gout, float* gin, in
     if (const int bad = svf_bad(field, gin, Bf, g0, g1, g2, D0, D1, D2, scale)) return bad;
     if (gin == field || gin == gout) return B200DRR_EINVAL;
     return ret(launch_svf_square_bwd(field, gout, gin, Bf, g0, g1, g2, mk(D0, D1, D2), scale, (cudaStream_t)stream));
+}
+
+int b200drr_svf_square_jvp(const float* field, const float* tangent, float* tout, float* out, int Bf, int g0, int g1, int g2, int D0,
+                           int D1, int D2, float scale, void* stream)
+{
+    if (!tangent || (((uintptr_t)tangent | (uintptr_t)out) & 15u) != 0) return B200DRR_EINVAL;
+    if (const int bad = svf_bad(field, tout, Bf, g0, g1, g2, D0, D1, D2, scale)) return bad;
+    if (tout == field || tout == tangent || out == field || out == tangent || out == tout) return B200DRR_EINVAL;
+    return ret(launch_svf_square_jvp(field, tangent, tout, out, Bf, g0, g1, g2, mk(D0, D1, D2), scale, (cudaStream_t)stream));
 }
 
 #ifdef B200DRR_EXPERIMENTS

@@ -329,5 +329,8 @@ cudaError_t launch_svf_square(const float* field, float* out, int Bf, int g0, in
                               cudaStream_t stream);
 cudaError_t launch_svf_square_bwd(const float* field, const float* gout, float* gin, int Bf, int g0, int g1, int g2, VolDims dims,
                                   float scale, cudaStream_t stream);
+// tout = the step's tangent along `tangent` (same layout); out (may be null) = the step itself, launch_svf_square's out bit for bit
+cudaError_t launch_svf_square_jvp(const float* field, const float* tangent, float* tout, float* out, int Bf, int g0, int g1, int g2,
+                                  VolDims dims, float scale, cudaStream_t stream);
 
 }  // namespace b200drr

@@ -1,7 +1,7 @@
 // svf.cu -- scaling-and-squaring steps of a stationary velocity field and their adjoint for sm_90a (math in svf_math.cuh).
 // One thread per lattice node and pose, 256 threads per CTA over the flattened [Bf][g0][g1][g2] nodes, so a warp reads 32
-// consecutive float4 nodes along axis 2.  The forward writes each node once (bit for bit repeatable); the adjoint adds 9 vector
-// reductions per node into a gradient the launcher zeroes first, so it repeats to fp32 reordering.
+// consecutive float4 nodes along axis 2.  The forward and the tangent write each node once (bit for bit repeatable); the adjoint
+// adds 9 vector reductions per node into a gradient the launcher zeroes first, so it repeats to fp32 reordering.
 #include "kernels.h"
 #include "svf_math.cuh"
 
@@ -50,6 +50,19 @@ __global__ void __launch_bounds__(kSvfThreads) svf_square_bwd_kernel(PolyLattice
     svf_square_node_bwd(lat, node, s, gp, gin + 4 * b * nodes);
 }
 
+__global__ void __launch_bounds__(kSvfThreads) svf_square_jvp_kernel(PolyLattice lat, PolyLattice tan, int64_t total, float s,
+                                                                      float4* __restrict__ tout, float4* __restrict__ out)
+{
+    int64_t b;
+    int node[3];
+    if (!svf_index(lat, total, b, node)) return;
+    const int64_t nodes = (int64_t)lat.g[0] * lat.g[1] * lat.g[2];
+    lat.w += b * nodes;
+    tan.w += b * nodes;
+    const int64_t x = b * nodes + svf_node(lat, node[0], node[1], node[2]);
+    tout[x] = svf_square_node_jvp(lat, tan, node, s, out ? out + x : nullptr);
+}
+
 cudaError_t launch_svf_square(const float* field, float* out, int Bf, int g0, int g1, int g2, VolDims dims, float scale,
                               cudaStream_t stream)
 {
@@ -69,6 +82,17 @@ cudaError_t launch_svf_square_bwd(const float* field, const float* gout, float* 
     const PolyLattice lat = make_lattice(field, g0, g1, g2, dims);
     svf_square_bwd_kernel<<<(unsigned)((total + kSvfThreads - 1) / kSvfThreads), kSvfThreads, 0, stream>>>(lat, total, scale,
                                                                                                             (const float4*)gout, gin);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_svf_square_jvp(const float* field, const float* tangent, float* tout, float* out, int Bf, int g0, int g1, int g2,
+                                  VolDims dims, float scale, cudaStream_t stream)
+{
+    const PolyLattice lat = make_lattice(field, g0, g1, g2, dims);
+    const PolyLattice tan = make_lattice(tangent, g0, g1, g2, dims);
+    const int64_t total = (int64_t)Bf * g0 * g1 * g2;
+    svf_square_jvp_kernel<<<(unsigned)((total + kSvfThreads - 1) / kSvfThreads), kSvfThreads, 0, stream>>>(lat, tan, total, scale,
+                                                                                                            (float4*)tout, (float4*)out);
     return cudaGetLastError();
 }
 

@@ -114,4 +114,32 @@ B200_HD void svf_square_node_bwd(const PolyLattice& lat, const int node[3], floa
     }
 }
 
+// The tangent of one squaring step at one node: for a tangent t on u (lat_t: this pose's tangent, lat_u's geometry), -> t'(x) =
+//   s t(x) + s^2 J_U(y) t(x) + s sum_c w_c(y) t(c)          (lane 3 zero),
+// y, its cell and J_U those of svf_square_node_bwd, one cell for u and for t: term by term the transpose of that adjoint, and no
+// reductions, so the tangent repeats bit for bit.  out_u (nullable) receives u'(x) by svf_square_node's own arithmetic.
+B200_HD float4 svf_square_node_jvp(const PolyLattice& lat_u, const PolyLattice& lat_t, const int node[3], float s, float4* out_u)
+{
+    const int64_t x = svf_node(lat_u, node[0], node[1], node[2]);
+    const float4 u = ldg4(lat_u.w + x);
+    const float4 tx = ldg4(lat_t.w + x);
+    float q[3], U[3], J[3][3], T[3];
+    svf_target(lat_u, node, u, s, q);
+    const SvfCell c = svf_cell(lat_u, q);
+    svf_lookup<true>(lat_u, c, U, J);
+    svf_lookup<false>(lat_t, c, T, nullptr);   // sum_c w_c(y) t(c)
+    if (out_u) *out_u = svf_square_node(lat_u, node, s);
+    const float t[3] = {tx.x, tx.y, tx.z};
+    const float ss = s * s;
+    float o[3];
+#pragma unroll
+    for (int i = 0; i < 3; ++i) o[i] = fmaf(ss, fmaf(J[i][0], t[0], fmaf(J[i][1], t[1], J[i][2] * t[2])), s * (t[i] + T[i]));
+    float4 r;
+    r.x = o[0];
+    r.y = o[1];
+    r.z = o[2];
+    r.w = 0.0f;
+    return r;
+}
+
 }  // namespace b200drr

@@ -577,6 +577,10 @@ class DeformableLevenbergMarquardt:
             self._img = self._render(self.field.detach())
         return self._img
 
+    def _keep(self, accept, img_t, img):
+        """The next step's image: the trial's for the accepted systems (accept (S,)), the current one's for the others."""
+        return torch.where(accept.reshape(-1, 1, 1, 1), img_t, img)
+
     def gradient(self) -> torch.Tensor:
         """The model's gradient g at the current field, in the field's shape (world mm)."""
         with torch.no_grad():
@@ -609,7 +613,86 @@ class DeformableLevenbergMarquardt:
             E, E_t = self._objective(img, Us), self._objective(img_t, Us_t)
             accept = E_t < E  # a NaN trial is rejected
             U.copy_(torch.where(accept.reshape(-1, *[1] * 4), Us_t, Us).reshape(U.shape))
-            self._img = torch.where(accept.reshape(-1, 1, 1, 1), img_t, img)
+            self._img = self._keep(accept, img_t, img)
             self.mu = torch.where(accept, self.mu / 10.0, self.mu * 10.0).clamp(1e-12, 1e12)
             out = torch.where(accept, E_t, E)
             return out[0] if self.shared else out
+
+
+class DiffeomorphicLevenbergMarquardt(DeformableLevenbergMarquardt):
+    """Levenberg-Marquardt registration of a stationary velocity field V towards `target`, rendered through its exponential:
+    render_deformed(field=exp_velocity(drr, V, steps)), with the camera pose fixed (DESIGN.md 6n).  The map exp(V) stays
+    invertible however large the step, where DeformableLevenbergMarquardt's displacement can fold.
+
+    The objective is E(V) = mean over the views of (1 - NCC(target, img)) + smoothness R(V), R = field_smoothness of the velocity.
+    `velocity` (3, g0, g1, g2) in world mm is shared by the B views (one objective); (B, 3, g0, g1, g2) gives B independent
+    objectives.  It is a fp32 tensor on the density's device, updated in place by step().
+
+    The Gauss-Newton model is DeformableLevenbergMarquardt's with the Jacobian of the march chained to that of the exponential:
+    J v = J_render J_exp v, J_exp v from the tangent squarings (b200drr_svf_square_jvp) over the levels of the current V, and
+    J^T w through the field scatter, then the squarings' adjoints (b200drr_svf_square_bwd) over the same levels, whose exact
+    transpose the tangent is.  Everything between the kernels stays in voxel units.  step(), the batched conjugate gradients, the
+    damping and the accept / reject rule are DeformableLevenbergMarquardt's; the levels of the current V (steps fields of
+    Bf g0 g1 g2 16 bytes) are computed once with its image and kept with the accepted trial's, so a step costs 2 cg_iters + 1
+    marches, 2 cg_iters steps small lattice launches and one forward.  No autograd and no host sync once warm.
+
+    The refusals are DeformableLevenbergMarquardt's, plus exp_velocity's for the velocity and for `steps` (1..16)."""
+
+    def __init__(self, drr, rot: torch.Tensor, xyz: torch.Tensor, velocity: torch.Tensor, target: torch.Tensor, steps: int = 10,
+                 smoothness: float = 1e-3, cg_iters: int = 10, parameterization: str = "euler_angles", convention: str | None = None,
+                 degrees: bool = False, calibration=None, n_points: int = 500, alphamin=None, alphamax=None, loss=None,
+                 damping: float = 1e-3, eps: float = 1e-5):
+        from .svf import check_velocity
+
+        check_velocity(drr, velocity, steps)
+        super().__init__(drr, rot, xyz, velocity, target, smoothness=smoothness, cg_iters=cg_iters,
+                         parameterization=parameterization, convention=convention, degrees=degrees, calibration=calibration,
+                         n_points=n_points, alphamin=alphamin, alphamax=alphamax, loss=loss, damping=damping, eps=eps)
+        self.steps, self._dims = steps, tuple(drr.density.shape)
+        self._exp = None     # (levels, exp) of the current velocity, the kernels' fields in voxel units
+        self._trial = None   # (levels, exp) of the last render
+
+    def _render(self, V):
+        from .deform import render_voxel_field, voxel_field
+        from .svf import square_chain
+
+        self._trial = square_chain(voxel_field(self.drr, V), self.steps, self._dims)
+        if self._img is None:   # the current velocity's image (_current_image), not a trial's
+            self._exp = self._trial
+        kw = self.kw
+        return render_voxel_field(self.drr, (self.rot, self.xyz), self.B, self._trial[1], kw["parameterization"], kw["convention"],
+                                  kw["degrees"], kw["calibration"], kw["n_points"], kw["alphamin"], kw["alphamax"],
+                                  self.drr.density)
+
+    def _keep(self, accept, img_t, img):
+        on = accept.reshape(-1, 1, 1, 1, 1)
+        (levels_t, phi_t), (levels, phi) = self._trial, self._exp
+        self._exp = ([torch.where(on, a, b) for a, b in zip(levels_t, levels)], torch.where(on, phi_t, phi))
+        return super()._keep(accept, img_t, img)
+
+    def _model(self, Vs, img):
+        """(grad, H) of the Gauss-Newton model at the system-batched velocity Vs and its image, through the levels of the current
+        velocity: grad() one scatter march and `steps` adjoint squarings, H(v) two marches and 2 steps lattice launches."""
+        from .deform import field_jvp, field_vjp, voxel_field
+        from .svf import square_chain_bwd, square_chain_jvp
+
+        drr, packed = self.drr, self.drr.renderer._packed_volume(self.drr.density)
+        source, tgt, lens, arange, grid = self._rays
+        n_points = int(self.kw["n_points"])
+        levels, phi = self._exp
+        z, sigma = ncc_z(img.reshape(self.B, self.N), self.eps)
+
+        def JT(w):
+            gphi = field_vjp(drr, packed, source, tgt, lens, phi, w, arange, n_points, grid, scratch=self._scratch)
+            gv = square_chain_bwd(levels, gphi, self._dims)
+            return torch.einsum("ij,bxyzi->bjxyz", self._lin, gv[..., :3])
+
+        def H(v):
+            dphi = square_chain_jvp(levels, voxel_field(drr, v), self._dims)[1]
+            jv = field_jvp(drr, packed, source, tgt, lens, phi, dphi, arange, n_points, grid)
+            return JT(self._wt * ncc_z_jvp(ncc_z_jvp(jv, z, sigma), z, sigma)) + self.smoothness * field_smoothness_grad(v)
+
+        def grad():
+            return JT(self._wt * ncc_z_jvp(z - self._zt, z, sigma)) + self.smoothness * field_smoothness_grad(Vs)
+
+        return grad, H

@@ -26,43 +26,106 @@ def _aligned(t):
     return t if t.data_ptr() % 16 == 0 else t.clone()
 
 
+def _scale(k, steps):
+    """Step k's s: 1 / 2^steps on the first step (it folds v / 2^steps in), 1 on the others."""
+    return 2.0**-steps if k == 0 else 1.0
+
+
+def square_chain(U, steps, dims):
+    """The kernels' field U (Bf, g0, g1, g2, 4), voxel units -> (levels, exp(U)): `steps` squaring launches on a volume of shape
+    dims, levels the inputs of the steps (levels[0] is U).  No autograd."""
+    levels = [_aligned(U)]
+    lib = _lib.load()
+    with torch.cuda.device(U.device):
+        for k in range(steps):
+            out = torch.empty_like(levels[0])
+            _lib.check(lib.b200drr_svf_square(_ptr(levels[-1]), _ptr(out), U.shape[0], *U.shape[1:4], *dims, _scale(k, steps),
+                                              _stream()), "b200drr_svf_square")
+            levels.append(out)
+    return levels[:-1], levels[-1]
+
+
+def square_chain_bwd(levels, g, dims):
+    """The adjoint of square_chain: an upstream gradient g on exp(U) -> the gradient on U, the steps' adjoints in reverse over
+    square_chain's levels.  No autograd."""
+    steps = len(levels)
+    g = _aligned(g)
+    lib = _lib.load()
+    with torch.cuda.device(g.device):
+        for k in reversed(range(steps)):
+            gin = torch.empty_like(levels[0])
+            _lib.check(lib.b200drr_svf_square_bwd(_ptr(levels[k]), _ptr(g), _ptr(gin), g.shape[0], *g.shape[1:4], *dims,
+                                                  _scale(k, steps), _stream()), "b200drr_svf_square_bwd")
+            g = gin
+    return g
+
+
+def square_chain_jvp(levels, T, dims, steps=None):
+    """The tangent T (voxel units, U's layout) pushed through the squarings, one b200drr_svf_square_jvp per step -> (exp(U) or
+    None, the tangent of exp(U)).  levels: square_chain's levels, read as they are (steps = len(levels), exp(U) not returned); or,
+    with `steps` given, [U] alone: each launch then also writes the next level, b200drr_svf_square's bits, so the primal and the
+    tangent share the `steps` launches and exp(U) is returned.  The exact transpose of square_chain_bwd over the same levels.  No
+    autograd."""
+    carry = steps is not None
+    levels, steps = [_aligned(levels[0])] if carry else list(levels), steps if carry else len(levels)
+    T = _aligned(T)
+    lib = _lib.load()
+    with torch.cuda.device(T.device):
+        for k in range(steps):
+            tout = torch.empty_like(levels[0])
+            out = torch.empty_like(levels[0]) if carry else None
+            _lib.check(lib.b200drr_svf_square_jvp(_ptr(levels[k]), _ptr(T), _ptr(tout), _ptr(out), T.shape[0], *T.shape[1:4], *dims,
+                                                  _scale(k, steps), _stream()), "b200drr_svf_square_jvp")
+            if carry:
+                levels.append(out)
+            T = tout
+    return (levels[-1] if carry else None), T
+
+
 class _SquaringFunction(torch.autograd.Function):
     """The kernels' field U (Bf, g0, g1, g2, 4), voxel units -> exp(U) in the same layout, by `steps` squaring launches on a volume
-    of shape dims.  Saves the input of every step (steps fields of U's size) for the backward."""
+    of shape dims (square_chain).  Saves the input of every step (steps fields of U's size) for the backward (square_chain_bwd)."""
 
     @staticmethod
     def forward(ctx, U, steps, dims):
-        levels = [_aligned(U)]
-        lib = _lib.load()
-        with torch.cuda.device(U.device):
-            for k in range(steps):
-                out = torch.empty_like(levels[0])
-                _lib.check(lib.b200drr_svf_square(_ptr(levels[-1]), _ptr(out), U.shape[0], *U.shape[1:4], *dims,
-                                                  2.0**-steps if k == 0 else 1.0, _stream()), "b200drr_svf_square")
-                levels.append(out)
-        ctx.save_for_backward(*levels[:-1])
-        ctx.consts = (steps, dims)
-        return levels[-1]
+        levels, out = square_chain(U, steps, dims)
+        ctx.save_for_backward(*levels)
+        ctx.consts = dims
+        return out
 
     @staticmethod
     @once_differentiable
     def backward(ctx, g):
-        levels = ctx.saved_tensors
-        steps, dims = ctx.consts
-        g = _aligned(g)
-        lib = _lib.load()
-        with torch.cuda.device(g.device):
-            for k in reversed(range(steps)):
-                gin = torch.empty_like(levels[0])
-                _lib.check(lib.b200drr_svf_square_bwd(_ptr(levels[k]), _ptr(g), _ptr(gin), g.shape[0], *g.shape[1:4], *dims,
-                                                      2.0**-steps if k == 0 else 1.0, _stream()), "b200drr_svf_square_bwd")
-                g = gin
-        return g, None, None
+        return square_chain_bwd(ctx.saved_tensors, g, ctx.consts), None, None
 
 
 def check_steps(steps):
     if isinstance(steps, bool) or not isinstance(steps, int) or not 1 <= steps <= MAX_STEPS:
         raise ValueError(f"steps must be an int in 1..{MAX_STEPS} (the number of squarings), got {steps!r}")
+
+
+def check_velocity(drr, velocity, steps):
+    """exp_velocity's refusals, before any launch."""
+    check_steps(steps)
+    if not torch.is_tensor(velocity) or velocity.dtype != torch.float32 or velocity.dim() not in (4, 5) or \
+            velocity.shape[-4] != 3 or min(velocity.shape[-3:]) < 1 or (velocity.dim() == 5 and velocity.shape[0] < 1):
+        got = f"{velocity.dtype} {tuple(velocity.shape)}" if torch.is_tensor(velocity) else type(velocity).__name__
+        raise ValueError(f"velocity must be an fp32 velocity lattice (3, g0, g1, g2) or (B, 3, g0, g1, g2), got {got}")
+    g0, g1, g2 = velocity.shape[-3:]
+    if 4 * g0 * g1 * g2 >= 2**31 - 1:
+        raise NotImplementedError(f"exp_velocity takes a lattice below 2^31 floats per pose (4 channels), got {(g0, g1, g2)}")
+    if not velocity.is_cuda:
+        raise _lib.B200DRRError(f"diffdrr_b200 runs on CUDA devices only (velocity is on {velocity.device}); there is no CPU "
+                                "fallback")
+    if velocity.device != drr.density.device:
+        raise ValueError(f"velocity must be on the density's device {drr.density.device}, not {velocity.device}")
+
+
+def _world(drr, phi, dim):
+    """The kernels' field (Bf, g0, g1, g2, 4), voxel units -> world mm (Bf, 3, g0, g1, g2), or (3, g0, g1, g2) for dim 4."""
+    lin = drr._affine.reshape(4, 4)[:3, :3]
+    u = torch.einsum("ij,bxyzj->bixyz", lin, phi[..., :3])
+    return u if dim == 5 else u[0]
 
 
 def exp_velocity(drr, velocity, steps=10):
@@ -77,23 +140,24 @@ def exp_velocity(drr, velocity, steps=10):
     Differentiable in the velocity (b200drr_svf_square_bwd; the gradient repeats to fp32 reordering).  Autograd keeps the input
     of every step, `steps` fields of Bf * g0 * g1 * g2 * 16 bytes (4.2 MB per 64^3 field and step).  A velocity that is not
     fp32, of the wrong rank or channel count, on the CPU or another device, or a steps outside 1..16 raises before any launch."""
-    check_steps(steps)
-    if not torch.is_tensor(velocity) or velocity.dtype != torch.float32 or velocity.dim() not in (4, 5) or \
-            velocity.shape[-4] != 3 or min(velocity.shape[-3:]) < 1 or (velocity.dim() == 5 and velocity.shape[0] < 1):
-        got = f"{velocity.dtype} {tuple(velocity.shape)}" if torch.is_tensor(velocity) else type(velocity).__name__
-        raise ValueError(f"velocity must be an fp32 velocity lattice (3, g0, g1, g2) or (B, 3, g0, g1, g2), got {got}")
-    g0, g1, g2 = velocity.shape[-3:]
-    if 4 * g0 * g1 * g2 >= 2**31 - 1:
-        raise NotImplementedError(f"exp_velocity takes a lattice below 2^31 floats per pose (4 channels), got {(g0, g1, g2)}")
-    if not velocity.is_cuda:
-        raise _lib.B200DRRError(f"diffdrr_b200 runs on CUDA devices only (velocity is on {velocity.device}); there is no CPU "
-                                "fallback")
-    if velocity.device != drr.density.device:
-        raise ValueError(f"velocity must be on the density's device {drr.density.device}, not {velocity.device}")
+    check_velocity(drr, velocity, steps)
     phi = _SquaringFunction.apply(voxel_field(drr, velocity), steps, tuple(drr.density.shape))
-    lin = drr._affine.reshape(4, 4)[:3, :3]
-    u = torch.einsum("ij,bxyzj->bixyz", lin, phi[..., :3])
-    return u if velocity.dim() == 5 else u[0]
+    return _world(drr, phi, velocity.dim())
+
+
+def exp_velocity_jvp(drr, velocity, tangent, steps=10):
+    """exp_velocity and its directional derivative along a velocity tangent (DESIGN.md 6n) -> (u, du), both world mm in the
+    velocity's shape: u = exp_velocity(drr, velocity, steps), bit for bit, and du = d/de exp_velocity(drr, velocity + e tangent,
+    steps) at e = 0.  One b200drr_svf_square_jvp launch per step carries the primal and the tangent together.  tangent: a tensor
+    of the velocity's shape, dtype and device.  No autograd: the results do not require grad.  The refusals are exp_velocity's
+    and DRR.deformed_jvp's tangent checks, before any launch."""
+    from .deform import _check_tangent
+
+    check_velocity(drr, velocity, steps)
+    _check_tangent(velocity, tangent)
+    with torch.no_grad():
+        phi, dphi = square_chain_jvp([voxel_field(drr, velocity)], voxel_field(drr, tangent), tuple(drr.density.shape), steps=steps)
+        return _world(drr, phi, velocity.dim()), _world(drr, dphi, velocity.dim())
 
 
 def se3_log_matrix(X):

@@ -840,6 +840,20 @@ int b200drr_svf_square(const float *field, float *out, int Bf, int g0, int g1, i
 int b200drr_svf_square_bwd(const float *field, const float *gout, float *gin, int Bf, int g0, int g1, int g2, int D0, int D1, int D2,
                            float scale, void *stream);
 
+/*
+ * Forward-mode derivative of one squaring step (DESIGN.md 6n), for Gauss-Newton on a velocity field: the step's tangent along a
+ * tangent t on field (the field's layout and units, the same Bf, lane 3 ignored).  With y = x + s field(x) and its clamped cell as
+ * in b200drr_svf_square_bwd,
+ *     tout(x) = s t(x) + s^2 J_U(y) t(x) + s sum_c w_c(y) t(c),
+ * the exact transpose of that adjoint: <gout, tout> = <gin, t> (lanes 0..2) to fp32 reordering.  out (NULL skips it) receives
+ * b200drr_svf_square's out bit for bit, so a chain of calls carries the primal and the tangent together.  tout and out are
+ * OVERWRITTEN, every node once, lane 3 zero: both repeat bit for bit.  tangent, tout and out 16-byte aligned, tout and out
+ * aliasing neither input nor each other.  The refusals are b200drr_svf_square's, plus a NULL tangent (B200DRR_EINVAL), all before
+ * touching CUDA.  The library allocates nothing.
+ */
+int b200drr_svf_square_jvp(const float *field, const float *tangent, float *tout, float *out /* nullable */, int Bf, int g0, int g1,
+                           int g2, int D0, int D1, int D2, float scale, void *stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -175,4 +175,19 @@ for kw in (dict(), dict(p_subsample=0.37), dict(patch_size=8, height=24)):
             img.sum().backward()
             torch.cuda.synchronize()
             print("deform_bproj", kw, shape, joint, "ok", float(img.sum()), float(V.grad.abs().max()))
+# tangent of a squaring step (svf.cu: svf_square_jvp_kernel) and the velocity LM over it: a 7 x 5 x 9 lattice (partial CTA), shared
+# and per-pose velocities large enough that many lookups clamp, with and without the primal output
+from diffdrr_b200 import DiffeomorphicLevenbergMarquardt, exp_velocity_jvp  # noqa: E402
+
+drr = DRR(synthetic.make_subject(vol), **synthetic.detector_kwargs(23), renderer="trilinear").to(dev)
+for shape in ((rot.shape[0], 3, 7, 5, 9), (3, 7, 5, 9)):
+    v, t = (torch.rand(*shape, device=dev) - 0.5) * 80.0, torch.rand(*shape, device=dev) - 0.5
+    u, du = exp_velocity_jvp(drr, v, t, steps=4)
+    with torch.no_grad():
+        target = drr.render_deformed(rot, xyz, field=u, n_points=64, parameterization="euler_angles", convention="ZXY")
+    lm = DiffeomorphicLevenbergMarquardt(drr, rot, xyz, torch.zeros_like(v), target, steps=4, cg_iters=2, n_points=64,
+                                         parameterization="euler_angles", convention="ZXY")
+    E = lm.step()
+    torch.cuda.synchronize()
+    print("svf_jvp", shape, "ok", float(du.abs().max()), E.tolist())
 print("done")

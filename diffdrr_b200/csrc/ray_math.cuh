@@ -1507,6 +1507,24 @@ struct GatherPacked16 {
     }
 };
 
+// f(gather) with the gather policy of the volume the caller gave: the packed-corner copy when there is one, the plain volume
+// otherwise; vol_type 0 = fp32, B200DRR_VOL_F16, B200DRR_VOL_BF16.  Host launch code of the warped kernels (polyrigid.cu,
+// deform.cu), so not part of the host emulation.
+#if defined(__CUDACC__)
+template <class F>
+cudaError_t with_gather(const void* vol, const void* packed, int vol_type, F&& f)
+{
+    switch (vol_type) {
+    case 0: return packed ? f(GatherPacked{(const float4*)packed}) : f(GatherPlainT<float>{(const float*)vol});
+    case 1:
+        return packed ? f(GatherPacked16<VoxF16>{(const Cell16<VoxF16>*)packed}) : f(GatherPlainT<VoxF16>{(const VoxF16*)vol});
+    case 2:
+        return packed ? f(GatherPacked16<VoxBF16>{(const Cell16<VoxBF16>*)packed}) : f(GatherPlainT<VoxBF16>{(const VoxBF16*)vol});
+    }
+    return cudaErrorInvalidValue;
+}
+#endif
+
 B200_HD bool outside_padded(const float pix[3], const VolDims& dims)
 {
     return pix[0] <= -1.0f || pix[1] <= -1.0f || pix[2] <= -1.0f || pix[0] >= (float)dims.d[0] ||

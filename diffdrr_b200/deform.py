@@ -21,19 +21,37 @@ from .renderers import _VOL16, Trilinear, _check_vol16, _dims_tensor, _get_alpha
 from .structures import _batch_size, _camera_pose
 
 
+def _check_renderer(drr, name, warp, kwargs):
+    """The warped renders' (render_polyrigid, render_deformed: `name`) refusals of the renderer and its options, before any launch.
+    warp: what bends the rays, for the message."""
+    r = drr.renderer
+    if not isinstance(r, Trilinear):
+        raise NotImplementedError(f"{name} supports the Trilinear renderer, not {type(r).__name__}: {warp} bends the rays inside "
+                                  "the volume, and Siddon's voxel walk follows straight lines")
+    if r.mode != "bilinear" or not isinstance(r.reducefn, str) or r.reducefn != "sum":
+        raise NotImplementedError(f"{name} supports Trilinear with its default options (mode='bilinear', reducefn='sum')")
+    if kwargs.get("align_corners", False) or kwargs.get("mask") is not None or kwargs.get("mask_to_channels", False) or \
+            set(kwargs) - {"align_corners", "mask", "mask_to_channels"}:
+        raise NotImplementedError(f"{name} takes no renderer options besides n_points, alphamin and alphamax, got {sorted(kwargs)}")
+
+
+def _check_density(vol, name, no_grad):
+    """The warped renders' refusals of the density `vol`, before any launch: no_grad is the message refusing a density that
+    requires grad, or None where the render has a gradient for it."""
+    if vol.dtype not in (torch.float32, *_VOL16) or vol.dim() != 3 or vol.numel() >= 2**31 - 1:
+        raise NotImplementedError(f"{name} needs a 3-D fp32 / fp16 / bf16 density below 2^31 voxels, got {vol.dtype} "
+                                  f"{tuple(vol.shape)}")
+    if vol.requires_grad and no_grad is not None:
+        raise NotImplementedError(no_grad)
+    if not vol.is_cuda:
+        raise _lib.B200DRRError(f"diffdrr_b200 renderers run on CUDA devices only (density is on {vol.device}); there is no CPU "
+                                "fallback")
+
+
 def check_supported(drr, args, parameterization, field, kwargs, density=None):
     """Refuse, before any launch, what the deformable render does not cover: -> B.  density: the volume rendered in place of
     drr.density (render_deformed's density=), or None."""
-    r = drr.renderer
-    if not isinstance(r, Trilinear):
-        raise NotImplementedError(f"render_deformed supports the Trilinear renderer, not {type(r).__name__}: the displacement field "
-                                  "bends the rays inside the volume, and Siddon's voxel walk follows straight lines")
-    if r.mode != "bilinear" or not isinstance(r.reducefn, str) or r.reducefn != "sum":
-        raise NotImplementedError("render_deformed supports Trilinear with its default options (mode='bilinear', reducefn='sum')")
-    if kwargs.get("align_corners", False) or kwargs.get("mask") is not None or kwargs.get("mask_to_channels", False) or \
-            set(kwargs) - {"align_corners", "mask", "mask_to_channels"}:
-        raise NotImplementedError(f"render_deformed takes no renderer options besides n_points, alphamin and alphamax, got "
-                                  f"{sorted(kwargs)}")
+    _check_renderer(drr, "render_deformed", "the displacement field", kwargs)
     B = _batch_size(args, parameterization)
     if not torch.is_tensor(field) or field.dtype != torch.float32 or field.dim() not in (4, 5) or field.shape[-4] != 3 or \
             (field.dim() == 5 and field.shape[0] != B) or min(field.shape[-3:]) < 1:
@@ -49,21 +67,29 @@ def check_supported(drr, args, parameterization, field, kwargs, density=None):
             raise ValueError(f"density must be a tensor of drr.density's shape {tuple(vol.shape)} on its device {vol.device}, got "
                              f"{got}")
         vol = density
-    if vol.dtype not in (torch.float32, *_VOL16) or vol.dim() != 3 or vol.numel() >= 2**31 - 1:
-        raise NotImplementedError(f"render_deformed needs a 3-D fp32 / fp16 / bf16 density below 2^31 voxels, got {vol.dtype} "
-                                  f"{tuple(vol.shape)}")
-    if vol.requires_grad and density is None:
-        raise NotImplementedError("render_deformed produces no volume gradient to drr.density: the density must not require grad "
-                                  "(pass the volume to fit as density= instead)")
-    if vol.requires_grad and vol.dtype != torch.float32:
-        raise NotImplementedError(f"render_deformed produces no volume gradient to a {vol.dtype} density: 16-bit volumes are static "
-                                  "densities (optimise an fp32 volume for volume gradients)")
-    if not vol.is_cuda:
-        raise _lib.B200DRRError(f"diffdrr_b200 renderers run on CUDA devices only (density is on {vol.device}); there is no CPU "
-                                "fallback")
+    if density is None:
+        no_grad = ("render_deformed produces no volume gradient to drr.density: the density must not require grad (pass the volume "
+                   "to fit as density= instead)")
+    elif vol.dtype != torch.float32:
+        no_grad = (f"render_deformed produces no volume gradient to a {vol.dtype} density: 16-bit volumes are static densities "
+                   "(optimise an fp32 volume for volume gradients)")
+    else:
+        no_grad = None
+    _check_density(vol, "render_deformed", no_grad)
     if field.device != vol.device:
         raise ValueError(f"field must be on the density's device {vol.device}, not {field.device}")
     return B
+
+
+def _launch_args(name, vol, packed, source, target, raylen, grid):
+    """The leading arguments of a warped-render entry point `name` (b200drr_polyrigid_*, b200drr_deform_*) -> (entry point: `name`
+    or its 16-bit twin, its (vol, packed[, vol_type]) with exactly one of the two arrays passed, its name, (src (B, 3), tgt
+    (B, N, 3), raylen (B, N)) contiguous fp32, (H, W) of a full detector grid or (0, 0) for any other ray set)."""
+    B, N = target.shape[0], target.shape[1]
+    fn, head, name = _vol_entry(_lib.load(), name, vol)
+    head = (_ptr(vol) if packed is None else None, _ptr(packed), *head[1:])
+    rays = (source.reshape(B, 3).contiguous().float(), target.contiguous().float(), raylen.reshape(B, N).contiguous().float())
+    return fn, head, name, rays, (grid if grid is not None and grid[0] * grid[1] == N else (0, 0))
 
 
 class _DeformFunction(torch.autograd.Function):
@@ -73,19 +99,12 @@ class _DeformFunction(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, volume, packed, source, target, img, field, alpha_range, voxel_shift, eps, n_points, grid):
-        B, N = target.shape[0], target.shape[1]
         vol = volume.contiguous()
-        src = source.reshape(B, 3).contiguous().float()
-        tgt = target.contiguous().float()
-        raylen = img.reshape(B, N).contiguous().float()
+        fn, head, name, (src, tgt, raylen), (H, W) = _launch_args("b200drr_deform_fwd", vol, packed, source, target, img, grid)
+        B, N = tgt.shape[0], tgt.shape[1]
         field = field.contiguous()
         arange = alpha_range.detach().to(device=vol.device, dtype=torch.float32).contiguous()
-        H, W = grid if grid is not None and grid[0] * grid[1] == N else (0, 0)
         out = torch.empty(B, N, dtype=torch.float32, device=vol.device)
-        lib = _lib.load()
-        # (vol, packed[, vol_type]): exactly one of the two arrays is passed
-        fn, head, name = _vol_entry(lib, "b200drr_deform_fwd", vol)
-        head = (_ptr(vol) if packed is None else None, _ptr(packed), *head[1:])
         geom = (*vol.shape, _ptr(src), _ptr(tgt), _ptr(raylen), _ptr(field), field.shape[0], *field.shape[1:4])
         with torch.cuda.device(vol.device):
             _lib.check(fn(*head, *geom, _ptr(out), B, N, H, W, voxel_shift, eps, n_points, _ptr(arange), _stream()), name)
@@ -117,8 +136,7 @@ class _DeformFunction(torch.autograd.Function):
         g_field = torch.empty_like(field) if ctx.needs_input_grad[5] else None   # NULL: the kernel skips the scatter
         g_range = torch.empty(2, dtype=torch.float32, device=dev)
         scratch = torch.empty(int(lib.b200drr_deform_scratch_floats(B, N, H, W)), dtype=torch.float32, device=dev)
-        fn, head, name = _vol_entry(lib, "b200drr_deform_bwd", vol)
-        head = (_ptr(vol) if packed is None else None, _ptr(packed), *head[1:])
+        fn, head, name, _, _ = _launch_args("b200drr_deform_bwd", vol, packed, src, tgt, raylen, (H, W))
         with torch.cuda.device(dev):
             _lib.check(fn(*head, *vol.shape, _ptr(src), _ptr(tgt), _ptr(raylen), _ptr(field), field.shape[0], *field.shape[1:4],
                           _ptr(gout), _ptr(g_src), _ptr(g_tgt), _ptr(g_raylen), _ptr(g_field), _ptr(g_range), _ptr(scratch),
@@ -136,11 +154,12 @@ def voxel_field(drr, field):
 
 
 def _marches(drr, args, B, parameterization, convention, degrees, calibration, alphamin, alphamax, vol=None):
-    """The rays of a deformable render in voxel-index space -> (source (B, 1, 3), [(target, raylen, alpha_range, grid), ...]): one
-    march for the full or sub-sampled detector, one per patch for patch_size (as DRR.render), each with its own sampling range
-    (the batch-global range of its rays, as Trilinear.forward, unless alphamin / alphamax fix it) and, for a full detector grid,
-    its (H, W).  Torch ops, differentiable in the camera pose and the calibration.  vol: the density rendered (default
-    drr.density)."""
+    """The rays of a warped render in voxel-index space -> (source (B, 1, 3), marches of (target, raylen, alpha_range, grid)): a
+    list of one march for the full or sub-sampled detector, or for patch_size (as DRR.render) an iterator of one march per patch
+    whose range is built when the iterator reaches it.  Each march has its own sampling range (the batch-global range of its rays,
+    as Trilinear.forward, unless alphamin / alphamax fix it) and, for a full detector grid, its (H, W).  Torch ops, differentiable
+    in the camera pose and the calibration; the order in which the ranges and the marches are built is the order in which
+    autograd sums their fp32 contributions to the camera gradient.  vol: the density rendered (default drr.density)."""
     vol, r = drr.density if vol is None else vol, drr.renderer
     P = _camera_pose(args, B, parameterization, convention, degrees)
     source, target = drr.detector(RigidTransform(P), calibration)
@@ -164,7 +183,7 @@ def _marches(drr, args, B, parameterization, convention, degrees, calibration, a
 
     if drr.patch_size is None:
         return source, [march(target, img, (det.height, det.width) if full_grid else None)]
-    return source, [march(t, i, None) for t, i in zip(target.chunk(drr.n_patches, dim=1), img.chunk(drr.n_patches, dim=-1))]
+    return source, (march(t, i, None) for t, i in zip(target.chunk(drr.n_patches, dim=1), img.chunk(drr.n_patches, dim=-1)))
 
 
 def render_deformed(drr, *args, field, parameterization=None, convention=None, degrees=False, calibration=None, n_points=500,
@@ -180,6 +199,7 @@ def render_voxel_field(drr, args, B, U, parameterization, convention, degrees, c
     """render_deformed after its checks, for the kernels' field U (Bf, g0, g1, g2, 4) in voxel units (voxel_field's output)."""
     r = drr.renderer
     source, marches = _marches(drr, args, B, parameterization, convention, degrees, calibration, alphamin, alphamax, vol=vol)
+    marches = list(marches)   # every patch's range before the first march (render_polyrigid builds each just before its march)
     packed = r._packed_volume(vol)
     outs = [_DeformFunction.apply(vol, packed, source, tgt, lens, U, alpha_range, float(r.voxel_shift), float(r.eps), int(n_points),
                                   grid) for tgt, lens, alpha_range, grid in marches]
@@ -199,13 +219,9 @@ def field_jvp(drr, packed, source, target, raylen, U, T, alpha_range, n_points, 
     (source (B, 1, 3), target (B, N, 3), raylen (B, 1, N)), U and T the kernels' fields (Bf, g0, g1, g2, 4) -> jv (B, N); `img`
     (B, N) fp32, if given, receives the march's image.  No autograd."""
     vol, r = drr.density, drr.renderer
-    B, N = target.shape[0], target.shape[1]
-    H, W = grid if grid is not None and grid[0] * grid[1] == N else (0, 0)
-    src, tgt, lens = source.reshape(B, 3).contiguous().float(), target.contiguous().float(), raylen.reshape(B, N).contiguous().float()
+    fn, head, name, (src, tgt, lens), (H, W) = _launch_args("b200drr_deform_jvp", vol, packed, source, target, raylen, grid)
+    B, N = tgt.shape[0], tgt.shape[1]
     jv = torch.empty(B, N, dtype=torch.float32, device=vol.device)
-    lib = _lib.load()
-    fn, head, name = _vol_entry(lib, "b200drr_deform_jvp", vol)
-    head = (_ptr(vol) if packed is None else None, _ptr(packed), *head[1:])
     with torch.cuda.device(vol.device):
         _lib.check(fn(*head, *vol.shape, _ptr(src), _ptr(tgt), _ptr(lens), _ptr(U), U.shape[0], *U.shape[1:4], _ptr(T), _ptr(img),
                       _ptr(jv), B, N, H, W, float(r.voxel_shift), float(r.eps), int(n_points), _ptr(alpha_range), _stream()), name)
@@ -216,15 +232,11 @@ def field_vjp(drr, packed, source, target, raylen, U, w, alpha_range, n_points, 
     """The transpose of field_jvp: sum_n w_n dI_n / dU as the kernels' field (Bf, g0, g1, g2, 4), voxel units (b200drr_deform_bwd
     with only g_field wanted).  w (B, N) fp32; scratch: b200drr_deform_scratch_floats floats, allocated here when None."""
     vol, r = drr.density, drr.renderer
-    B, N = target.shape[0], target.shape[1]
-    H, W = grid if grid is not None and grid[0] * grid[1] == N else (0, 0)
-    src, tgt, lens = source.reshape(B, 3).contiguous().float(), target.contiguous().float(), raylen.reshape(B, N).contiguous().float()
-    lib = _lib.load()
+    fn, head, name, (src, tgt, lens), (H, W) = _launch_args("b200drr_deform_bwd", vol, packed, source, target, raylen, grid)
+    B, N = tgt.shape[0], tgt.shape[1]
     if scratch is None:
-        scratch = torch.empty(int(lib.b200drr_deform_scratch_floats(B, N, H, W)), dtype=torch.float32, device=vol.device)
+        scratch = torch.empty(int(_lib.load().b200drr_deform_scratch_floats(B, N, H, W)), dtype=torch.float32, device=vol.device)
     g_field = torch.empty_like(U)
-    fn, head, name = _vol_entry(lib, "b200drr_deform_bwd", vol)
-    head = (_ptr(vol) if packed is None else None, _ptr(packed), *head[1:])
     with torch.cuda.device(vol.device):
         _lib.check(fn(*head, *vol.shape, _ptr(src), _ptr(tgt), _ptr(lens), _ptr(U), U.shape[0], *U.shape[1:4], _ptr(w.contiguous()),
                       None, None, None, _ptr(g_field), None, _ptr(scratch), B, N, H, W, float(r.voxel_shift), float(r.eps),

@@ -14,9 +14,9 @@ import torch
 from torch.autograd.function import once_differentiable
 
 from . import _lib
-from .pose import RigidTransform
-from .renderers import _VOL16, Trilinear, _check_vol16, _dims_tensor, _get_alpha_minmax, _ptr, _stream, _vol_entry
-from .structures import _batch_size, _camera_pose, _label_tuple, _motion_matrices, _rigid_inverse, _translation, twist_matrix
+from .deform import _check_density, _check_renderer, _launch_args, _marches
+from .renderers import _ptr, _stream, _vol_entry  # noqa: F401  (_vol_entry: the tests call the entry points through this module)
+from .structures import _batch_size, _label_tuple, _motion_matrices, _rigid_inverse, _translation, twist_matrix
 
 MAX_STRUCTURES = 8
 _weights_cache = None   # (key, weak reference to the mask, lattice) of the last polyrigid_weights call
@@ -86,16 +86,7 @@ def _packed_weights(drr, weights):
 
 def check_supported(drr, args, parameterization, motions, weights, kwargs):
     """Refuse, before any launch, what the blended-rigid render does not cover: -> (motion matrices, B, K)."""
-    r = drr.renderer
-    if not isinstance(r, Trilinear):
-        raise NotImplementedError(f"render_polyrigid supports the Trilinear renderer, not {type(r).__name__}: the blended motion bends "
-                                  "the rays inside the volume, and Siddon's voxel walk follows straight lines")
-    if r.mode != "bilinear" or not isinstance(r.reducefn, str) or r.reducefn != "sum":
-        raise NotImplementedError("render_polyrigid supports Trilinear with its default options (mode='bilinear', reducefn='sum')")
-    if kwargs.get("align_corners", False) or kwargs.get("mask") is not None or kwargs.get("mask_to_channels", False) or \
-            set(kwargs) - {"align_corners", "mask", "mask_to_channels"}:
-        raise NotImplementedError(f"render_polyrigid takes no renderer options besides n_points, alphamin and alphamax, got "
-                                  f"{sorted(kwargs)}")
+    _check_renderer(drr, "render_polyrigid", "the blended motion", kwargs)
     if not torch.is_tensor(weights) or weights.dim() != 4 or weights.dtype != torch.float32:
         got = f"{weights.dtype} {tuple(weights.shape)}" if torch.is_tensor(weights) else type(weights).__name__
         raise ValueError(f"weights must be an fp32 lattice (K, g0, g1, g2), got {got}")
@@ -107,14 +98,7 @@ def check_supported(drr, args, parameterization, motions, weights, kwargs):
     B = _batch_size(args, parameterization)
     X = _motion_matrices(motions, K, B)
     vol = drr.density
-    if vol.dtype not in (torch.float32, *_VOL16) or vol.dim() != 3 or vol.numel() >= 2**31 - 1:
-        raise NotImplementedError(f"render_polyrigid needs a 3-D fp32 / fp16 / bf16 density below 2^31 voxels, got {vol.dtype} "
-                                  f"{tuple(vol.shape)}")
-    if vol.requires_grad:
-        raise NotImplementedError("render_polyrigid produces no volume gradient: the density must not require grad")
-    if not vol.is_cuda:
-        raise _lib.B200DRRError(f"diffdrr_b200 renderers run on CUDA devices only (density is on {vol.device}); there is no CPU "
-                                "fallback")
+    _check_density(vol, "render_polyrigid", "render_polyrigid produces no volume gradient: the density must not require grad")
     if X.device != vol.device or weights.device != vol.device:
         raise ValueError(f"motions and weights must be on the density's device {vol.device}, not {X.device} and {weights.device}")
     return X, B, K
@@ -126,19 +110,12 @@ class _PolyrigidFunction(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, volume, packed, source, target, img, M, alpha_range, wpacked, lattice, voxel_shift, eps, n_points, grid):
-        B, N = target.shape[0], target.shape[1]
         vol = volume.contiguous()
-        src = source.reshape(B, 3).contiguous().float()
-        tgt = target.contiguous().float()
-        raylen = img.reshape(B, N).contiguous().float()
+        fn, head, name, (src, tgt, raylen), (H, W) = _launch_args("b200drr_polyrigid_fwd", vol, packed, source, target, img, grid)
+        B, N = tgt.shape[0], tgt.shape[1]
         M = M.contiguous().float()
         arange = alpha_range.detach().to(device=vol.device, dtype=torch.float32).contiguous()
-        H, W = grid if grid is not None and grid[0] * grid[1] == N else (0, 0)
         out = torch.empty(B, N, dtype=torch.float32, device=vol.device)
-        lib = _lib.load()
-        # (vol, packed[, vol_type]): exactly one of the two arrays is passed
-        fn, head, name = _vol_entry(lib, "b200drr_polyrigid_fwd", vol)
-        head = (_ptr(vol) if packed is None else None, _ptr(packed), *head[1:])
         tail = (B, N, H, W, voxel_shift, eps, n_points, _ptr(arange), _stream())
         geom = (*vol.shape, _ptr(src), _ptr(tgt), _ptr(raylen), _ptr(M), M.shape[0], M.shape[1], _ptr(wpacked), *lattice)
         with torch.cuda.device(vol.device):
@@ -162,8 +139,7 @@ class _PolyrigidFunction(torch.autograd.Function):
         g_range = torch.empty(2, dtype=torch.float32, device=dev)
         lib = _lib.load()
         scratch = torch.empty(int(lib.b200drr_polyrigid_scratch_floats(B, N, H, W, M.shape[1])), dtype=torch.float32, device=dev)
-        fn, head, name = _vol_entry(lib, "b200drr_polyrigid_bwd", vol)
-        head = (_ptr(vol) if packed is None else None, _ptr(packed), *head[1:])
+        fn, head, name, _, _ = _launch_args("b200drr_polyrigid_bwd", vol, packed, src, tgt, raylen, (H, W))
         with torch.cuda.device(dev):
             _lib.check(fn(*head, *vol.shape, _ptr(src), _ptr(tgt), _ptr(raylen), _ptr(M), M.shape[0], M.shape[1], _ptr(wpacked),
                           *lattice, _ptr(gout), _ptr(g_src), _ptr(g_tgt), _ptr(g_raylen), _ptr(g_M), _ptr(g_range), _ptr(scratch),
@@ -195,35 +171,13 @@ def render_polyrigid(drr, *args, motions, weights, parameterization=None, conven
     if blend == "log_euclidean":   # the lattice check above is the linear blend's; the packed copy is not used
         return svf.render_log_euclidean(drr, args, X, B, weights, steps, parameterization, convention, degrees, calibration,
                                         n_points, alphamin, alphamax)
-    P = _camera_pose(args, B, parameterization, convention, degrees)
-    source, target = drr.detector(RigidTransform(P), calibration)
-    img = (target - source).norm(dim=-1).unsqueeze(1)
-    source, target = drr.affine_inverse(source), drr.affine_inverse(target)
-    if vol.dtype in _VOL16:
-        _check_vol16(vol, source, target)
+    source, marches = _marches(drr, args, B, parameterization, convention, degrees, calibration, alphamin, alphamax)
     M = voxel_maps(drr, X)
     M = M if M.dim() == 4 else M[None]
-    det = drr.detector
-    full_grid = det.n_subsample is None and drr.patch_size is None
     packed = r._packed_volume(vol)
-    dims = _dims_tensor(vol.shape, source.device, source.dtype)
-
-    def march(tgt, lens, grid):
-        if alphamin is None or alphamax is None:   # the batch-global range of the rays in this call, as Trilinear.forward
-            amin, amax = _get_alpha_minmax(source, tgt, dims, r.voxel_shift, r.eps)
-            lo, hi = amin.min(), amax.max()
-        else:
-            lo, hi = alphamin, alphamax
-        alpha_range = torch.stack([torch.as_tensor(lo, dtype=torch.float32, device=vol.device),
-                                   torch.as_tensor(hi, dtype=torch.float32, device=vol.device)])
-        return _PolyrigidFunction.apply(vol, packed, source, tgt, lens, M, alpha_range, wpacked, tuple(weights.shape[1:]),
-                                        float(r.voxel_shift), float(r.eps), int(n_points), grid)
-
-    if drr.patch_size is None:
-        out = march(target, img, (det.height, det.width) if full_grid else None)
-    else:   # serial patches with a range each, as DRR.render
-        out = torch.cat([march(t, i, None) for t, i in zip(target.chunk(drr.n_patches, dim=1), img.chunk(drr.n_patches, dim=-1))],
-                        dim=-1)
+    outs = [_PolyrigidFunction.apply(vol, packed, source, tgt, lens, M, alpha_range, wpacked, tuple(weights.shape[1:]),
+                                     float(r.voxel_shift), float(r.eps), int(n_points), grid) for tgt, lens, alpha_range, grid in marches]
+    out = outs[0] if len(outs) == 1 else torch.cat(outs, dim=-1)   # serial patches with a range each, as DRR.render
     return drr.reshape_transform(out, batch_size=B)
 
 
@@ -272,34 +226,17 @@ def polyrigid_jacobian(drr, *args, motions, weights, parameterization=None, conv
     H, W = det.height, det.width
     with torch.no_grad():
         wpacked = _packed_weights(drr, weights)
-        P = _camera_pose(args, B, parameterization, convention, degrees)
-        source, target = drr.detector(RigidTransform(P), calibration)
-        raylen = (target - source).norm(dim=-1)
-        source, target = drr.affine_inverse(source), drr.affine_inverse(target)
-        if vol.dtype in _VOL16:
-            _check_vol16(vol, source, target)
+        source, [(target, raylen, arange, grid)] = _marches(drr, args, B, parameterization, convention, degrees, calibration,
+                                                            alphamin, alphamax)
         M = voxel_maps(drr, X)
         M = (M if M.dim() == 4 else M[None]).contiguous()
         T = polyrigid_tangents(drr, X, polyrigid_pivots(drr, weights))
         packed = r._packed_volume(vol)
-        dims = _dims_tensor(vol.shape, source.device, source.dtype)
-        if alphamin is None or alphamax is None:   # the batch-global range of the rays, as render_polyrigid
-            amin, amax = _get_alpha_minmax(source, target, dims, r.voxel_shift, r.eps)
-            lo, hi = amin.min(), amax.max()
-        else:
-            lo, hi = alphamin, alphamax
-        arange = torch.stack([torch.as_tensor(lo, dtype=torch.float32, device=vol.device),
-                              torch.as_tensor(hi, dtype=torch.float32, device=vol.device)])
-        src = source.reshape(B, 3).contiguous().float()
-        tgt = target.contiguous().float()
-        raylen = raylen.reshape(B, H * W).contiguous().float()
         volc = vol.contiguous()
+        fn, head, name, (src, tgt, raylen), _ = _launch_args("b200drr_polyrigid_jac", volc, packed, source, target, raylen, grid)
         img = torch.empty(B, H * W, dtype=torch.float32, device=vol.device)
         J = torch.empty(B, K, H * W, 6, dtype=torch.float32, device=vol.device)
         rects = torch.empty(B, K, 4, dtype=torch.int32, device=vol.device)
-        lib = _lib.load()
-        fn, head, name = _vol_entry(lib, "b200drr_polyrigid_jac", volc)
-        head = (_ptr(volc) if packed is None else None, _ptr(packed), *head[1:])
         with torch.cuda.device(vol.device):
             _lib.check(fn(*head, *vol.shape, _ptr(src), _ptr(tgt), _ptr(raylen), _ptr(M), M.shape[0], K, _ptr(wpacked),
                           *weights.shape[1:], _ptr(T), _ptr(img), _ptr(J), _ptr(rects), B, H, W, float(r.voxel_shift), float(r.eps),

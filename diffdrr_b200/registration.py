@@ -42,6 +42,55 @@ class Registration(nn.Module):
         return self._translation
 
 
+def _damped_solve(A, g, damping):
+    """The Levenberg-Marquardt step delta of (A + lambda diag A) delta = -g, solved per system in float64: A (S, P, P), g (S, P)
+    and lambda = damping (S,) -> delta (S, P).  No host sync."""
+    D = torch.diag_embed(torch.diagonal(A, dim1=-2, dim2=-1).clamp_min(1e-12))
+    return torch.linalg.solve_ex(A + damping[:, None, None] * D, -g.unsqueeze(-1))[0].squeeze(-1)
+
+
+def _next_damping(accept, damping):
+    """The damping after a step: / 10 where the trial was accepted, x 10 where it was rejected, within [1e-12, 1e12]."""
+    return torch.where(accept, damping / 10.0, damping * 10.0).clamp(1e-12, 1e12)
+
+
+def _global_ncc(name, loss, eps):
+    """The loss of the Levenberg-Marquardt solvers that model the global NCC only: None -> NormalizedCrossCorrelation2d(eps=eps);
+    anything but a NormalizedCrossCorrelation2d without patch_size raises TypeError."""
+    from .metrics import NormalizedCrossCorrelation2d
+
+    if loss is None:
+        return NormalizedCrossCorrelation2d(eps=eps)
+    if type(loss) is not NormalizedCrossCorrelation2d or loss.patch_size is not None:
+        raise TypeError(f"{name} models the global NCC only: NormalizedCrossCorrelation2d without patch_size (or loss=None), not "
+                        f"{type(loss).__name__}{'' if getattr(loss, 'patch_size', None) is None else f'(patch_size={loss.patch_size})'}"
+                        f"; patch-wise, multiscale and gradient NCC have no Gauss-Newton model here (use a first-order optimizer)")
+    return loss
+
+
+def _check_target(name, drr, target, args, parameterization, check_supported, full_detector=True):
+    """The refusals of a warped-render Levenberg-Marquardt solver `name` for its target, in order: a one-channel (B, 1, H, W)
+    image, a full detector (where `full_detector`), the detector's H x W, a batch of 1 or the poses' B, then the render's own
+    refusals (`check_supported()`), then a CUDA fp32 tensor -> B."""
+    from .structures import _batch_size
+
+    if not torch.is_tensor(target) or target.dim() != 4 or target.shape[1] != 1:
+        raise ValueError(f"{name} takes a one-channel target image (B, 1, H, W), got "
+                         f"{tuple(target.shape) if torch.is_tensor(target) else type(target).__name__}")
+    det = drr.detector
+    if full_detector and (det.n_subsample is not None or drr.patch_size is not None):
+        raise NotImplementedError(f"{name} covers the full detector only, not p_subsample or patch_size")
+    if tuple(target.shape[-2:]) != (det.height, det.width):
+        raise ValueError(f"the target {tuple(target.shape)} does not match the {det.height} x {det.width} detector")
+    B = _batch_size(args, parameterization)
+    if target.shape[0] not in (1, B):
+        raise ValueError(f"the target's batch ({target.shape[0]}) must be 1 or the number of poses ({B})")
+    check_supported()
+    if not (target.is_cuda and target.dtype == torch.float32):
+        raise ValueError(f"{name} runs on the GPU: the target must be a CUDA fp32 tensor")
+    return B
+
+
 def ncc_normal_equations(x, t, J, strides, patch_size, eps, weight, A, g):
     """A += weight * sum Jz^T Jz, g += weight * sum Jz^T r over every window of every channel of the global (patch_size None) or
     patch-wise NCC between x and t ((B, C, H, W) fp32 CUDA, contiguous), through b200drr_ncc_normal (csrc/ncc_normal.cu).
@@ -153,15 +202,13 @@ class LevenbergMarquardt:
             img, J = drr_jacobian(reg.drr, rot, xyz, stop_grad=False, **kw)
             nr = rot.shape[1]
             A, g = self.normal_equations(img, J)
-            g = g.unsqueeze(-1)
-            D = torch.diag_embed(torch.diagonal(A, dim1=-2, dim2=-1).clamp_min(1e-12))
-            delta = torch.linalg.solve_ex(A + self.damping[:, None, None] * D, -g)[0].squeeze(-1).to(rot.dtype)
+            delta = _damped_solve(A, g, self.damping).to(rot.dtype)
             rot_t, xyz_t = rot + delta[:, :nr], xyz + delta[:, nr:]
             loss, trial = self._loss(img), self._loss(reg.drr(rot_t, xyz_t, **kw))
             accept = trial < loss  # a NaN trial is rejected
             rot.copy_(torch.where(accept[:, None], rot_t, rot))
             xyz.copy_(torch.where(accept[:, None], xyz_t, xyz))
-            self.damping = torch.where(accept, self.damping / 10.0, self.damping * 10.0).clamp(1e-12, 1e12)
+            self.damping = _next_damping(accept, self.damping)
             return torch.where(accept, trial, loss)
 
 
@@ -188,204 +235,143 @@ def ncc_normal_structures_equations(x, t, J, rects, eps, weight, A, g):
                                                  torch.cuda.current_stream(x.device).cuda_stream), "b200drr_ncc_normal_structures")
 
 
-def _motion_lm_update(X, A, g, damping, pivots, shared, loss, trial_loss):
-    """The damped solve, update and accept of the motion Levenberg-Marquardt steps (StructuresLevenbergMarquardt,
-    PolyrigidLevenbergMarquardt): solve (A + lambda diag A) delta = -g in float64, move every structure by the left increment
-    delta_k = (omega, v) about its pivot, X_k <- T(c_k) exp(delta_k^) T(-c_k) X_k, and keep the trial where its true loss
-    trial_loss(X_trial) (B,) is below `loss` (B,) (lambda / 10 on accept, x 10 on reject).  Shared motions (K, 4, 4): one system,
-    the mean over the views, and one decision on the mean loss.  X is updated in place -> (damping, loss after the step)."""
-    from .structures import apply_increments
-
-    if shared:
-        A, g = A.mean(0, keepdim=True), g.mean(0, keepdim=True)
-    D = torch.diag_embed(torch.diagonal(A, dim1=-2, dim2=-1).clamp_min(1e-12))
-    delta = torch.linalg.solve_ex(A + damping[:, None, None] * D, -g.unsqueeze(-1))[0].squeeze(-1)
-    X_t = apply_increments(X.detach(), delta.reshape(*X.shape[:-2], 6), pivots)   # (..., K, 6): (omega, v) per k
-    trial = trial_loss(X_t)
-    if shared:
-        loss, trial = loss.mean(), trial.mean()
-    accept = trial < loss  # a NaN trial is rejected
-    X.copy_(torch.where(accept.reshape(-1, *[1] * (X.dim() - 1)), X_t, X))
-    damping = torch.where(accept, damping / 10.0, damping * 10.0).clamp(1e-12, 1e12)
-    return damping, torch.where(accept, trial, loss)
-
-
-class StructuresLevenbergMarquardt:
-    """Levenberg-Marquardt registration of the K structures of a piecewise-rigid DRR (DRR.render_structures) towards `target`
-    on the global NCC of the composite image (the sum of the channels), with the camera pose fixed (DESIGN.md 6g).
+class _MotionLevenbergMarquardt:
+    """The Levenberg-Marquardt step of the rigid-motion solvers (StructuresLevenbergMarquardt, PolyrigidLevenbergMarquardt) on the
+    global NCC of the composite image, with the camera pose fixed.
 
     The unknowns are the motions: `motions` (K, 4, 4), shared by the B views, or (B, K, 4, 4), one set per pose; a tensor or a
-    Parameter, fp32 on the density's device, updated in place by step().  Each step takes one DRR.structures_jacobian (the full
-    derivative of the image, whatever the renderer's stop_gradients_through_grid_sample), forms the Gauss-Newton system of the
-    z-normalised residual block by block over the structures' footprints (b200drr_ncc_normal_structures), solves
-    (A + lambda diag A) delta = -g in float64, and renders one trial image.  delta_k = (omega, v) moves structure k as
-        X_k <- T(c_k) exp(delta_k^) T(-c_k) X_k
-    (a left increment about the pivot c_k, the world centre of label k's box, structures.structure_pivots; exp is the matrix
-    exponential of the twist, not pose.se3_exp_map's transposed convention).  The trial is kept if its true loss is lower
-    (lambda / 10 on accept, x 10 on reject).  Shared motions: one system, the mean over the views of the per-view systems,
-    modelling the mean of 1 - NCC, and one decision per step on that mean.  Per-pose motions: B independent systems and
-    decisions.  No host sync.
+    Parameter, fp32 on the density's device, updated in place by step().  Each step takes one Jacobian of the image (_jacobian: the
+    image, the per-pixel columns of every motion and their footprints), forms the Gauss-Newton system of the z-normalised residual
+    block by block over the footprints (b200drr_ncc_normal_structures), solves (A + lambda diag A) delta = -g in float64, and
+    renders one trial image (_render).  delta_k = (omega, v) moves structure k as
+        X_k <- T(c_k) exp(delta_k^) T(-c_k) X_k,
+    a left increment about the pivot c_k (exp is the matrix exponential of the twist, not pose.se3_exp_map's transposed
+    convention).  The trial is kept if its true loss is lower (lambda / 10 on accept, x 10 on reject).  Shared motions: one
+    system, the mean over the views of the per-view systems, modelling the mean of 1 - NCC, and one decision per step on that
+    mean.  Per-pose motions: B independent systems and decisions.  No host sync.
 
     Only the global NCC is modelled: `loss` None (NormalizedCrossCorrelation2d(eps=eps)) or a NormalizedCrossCorrelation2d
     without patch_size; anything else raises TypeError here."""
+
+    def __init__(self, drr, rot, xyz, motions, target, parameterization, loss, damping, eps, check_supported, full_detector):
+        name = type(self).__name__
+        loss = _global_ncc(name, loss, eps)
+        if not torch.is_tensor(motions) or motions.dim() not in (3, 4):
+            raise ValueError(f"motions must be a (K, 4, 4) or (B, K, 4, 4) tensor updated in place, got "
+                             f"{tuple(motions.shape) if torch.is_tensor(motions) else type(motions).__name__}")
+        B = _check_target(name, drr, target, (rot, xyz), parameterization, check_supported, full_detector)
+        det = drr.detector
+        self.drr, self.rot, self.xyz, self.motions = drr, rot.detach(), xyz.detach(), motions
+        self.loss, self.eps = loss, float(loss.eps)
+        self.shared = motions.dim() == 3
+        self.target = target.detach().expand(B, 1, det.height, det.width).contiguous()
+        self._t = self.target[:, 0]
+        self.damping = torch.full((1 if self.shared else B,), float(damping), dtype=torch.float64, device=motions.device)
+
+    def _composite(self, img):
+        """The image the loss compares with the target, (B, 1, H, W)."""
+        return img
+
+    def _loss(self, img):
+        """(B,) 1 - NCC of the composite of each view."""
+        return 1.0 - self.loss(self.target, self._composite(img))
+
+    def normal_equations(self, img, J, rects):
+        """(A (B, 6K, 6K), g (B, 6K)) float64 of each view's Gauss-Newton model of 1 - NCC (weight 1 / (H W)) at the image `img`
+        with Jacobian J (B, K, H, W, 6) and footprints rects."""
+        B, K, H, W = img.shape[0], J.shape[1], self._t.shape[-2], self._t.shape[-1]
+        x = self._composite(img).reshape(B, H, W).contiguous()
+        A = torch.zeros(B, 6 * K, 6 * K, dtype=torch.float64, device=img.device)
+        g = torch.zeros(B, 6 * K, dtype=torch.float64, device=img.device)
+        ncc_normal_structures_equations(x, self._t, J, rects, self.eps, 1.0 / (H * W), A, g)
+        return A, g
+
+    def step(self) -> torch.Tensor:
+        """One damped Gauss-Newton step; -> the loss after it: the mean over the views of 1 - NCC (a 0-d tensor) for shared
+        motions, the per-pose (B,) losses otherwise."""
+        from .structures import apply_increments
+
+        X = self.motions
+        with torch.no_grad():
+            img, J, rects = self._jacobian(X)
+            A, g = self.normal_equations(img, J, rects)
+            loss = self._loss(img)
+            if self.shared:
+                A, g = A.mean(0, keepdim=True), g.mean(0, keepdim=True)
+            delta = _damped_solve(A, g, self.damping)
+            X_t = apply_increments(X.detach(), delta.reshape(*X.shape[:-2], 6), self.pivots)   # (..., K, 6): (omega, v) per k
+            trial = self._loss(self._render(X_t))
+            if self.shared:
+                loss, trial = loss.mean(), trial.mean()
+            accept = trial < loss  # a NaN trial is rejected
+            X.copy_(torch.where(accept.reshape(-1, *[1] * (X.dim() - 1)), X_t, X))
+            self.damping = _next_damping(accept, self.damping)
+            return torch.where(accept, trial, loss)
+
+
+class StructuresLevenbergMarquardt(_MotionLevenbergMarquardt):
+    """Levenberg-Marquardt registration of the K structures of a piecewise-rigid DRR (DRR.render_structures) towards `target`
+    on the global NCC of the composite image (the sum of the channels), with the camera pose fixed (DESIGN.md 6g).
+
+    The step is _MotionLevenbergMarquardt's.  The Jacobian is DRR.structures_jacobian's (the full derivative of the image,
+    whatever the renderer's stop_gradients_through_grid_sample), the trial render DRR.render_structures', and the pivot c_k of
+    structure k the world centre of label k's box (structures.structure_pivots)."""
 
     def __init__(self, drr, rot: torch.Tensor, xyz: torch.Tensor, motions: torch.Tensor, labels, target: torch.Tensor,
                  parameterization: str = "euler_angles", convention: str | None = None, degrees: bool = False, calibration=None,
                  background: bool = True, loss=None, damping: float = 1e-3, eps: float = 1e-5):
-        from .metrics import NormalizedCrossCorrelation2d
-        from .structures import _batch_size, _label_tuple, check_supported, structure_pivots
+        from .structures import _label_tuple, check_supported, structure_pivots
 
-        if loss is None:
-            loss = NormalizedCrossCorrelation2d(eps=eps)
-        elif type(loss) is not NormalizedCrossCorrelation2d or loss.patch_size is not None:
-            raise TypeError(f"StructuresLevenbergMarquardt models the global NCC only: NormalizedCrossCorrelation2d without "
-                            f"patch_size (or loss=None), not {type(loss).__name__}"
-                            f"{'' if getattr(loss, 'patch_size', None) is None else f'(patch_size={loss.patch_size})'}; patch-wise, "
-                            f"multiscale and gradient NCC have no block-sparse system here (use a first-order optimizer)")
-        if not torch.is_tensor(motions) or motions.dim() not in (3, 4):
-            raise ValueError(f"motions must be a (K, 4, 4) or (B, K, 4, 4) tensor updated in place, got "
-                             f"{tuple(motions.shape) if torch.is_tensor(motions) else type(motions).__name__}")
-        if not torch.is_tensor(target) or target.dim() != 4 or target.shape[1] != 1:
-            raise ValueError(f"StructuresLevenbergMarquardt takes a one-channel target image (B, 1, H, W) of the composite, got "
-                             f"{tuple(target.shape) if torch.is_tensor(target) else type(target).__name__}")
-        det = drr.detector
-        if tuple(target.shape[-2:]) != (det.height, det.width):
-            raise ValueError(f"the target {tuple(target.shape)} does not match the {det.height} x {det.width} detector")
-        B = _batch_size((rot, xyz), parameterization)
-        if target.shape[0] not in (1, B):
-            raise ValueError(f"the target's batch ({target.shape[0]}) must be 1 or the number of poses ({B})")
-        labels, _, B = check_supported(drr, (rot, xyz), parameterization, motions, _label_tuple(labels), {})
-        if not (target.is_cuda and target.dtype == torch.float32):
-            raise ValueError("StructuresLevenbergMarquardt's normal equations run on the GPU: the target must be a CUDA fp32 tensor")
-        self.drr, self.rot, self.xyz, self.motions, self.labels = drr, rot.detach(), xyz.detach(), motions, labels
+        def check():
+            self.labels = check_supported(drr, (rot, xyz), parameterization, motions, _label_tuple(labels), {})[0]
+
+        super().__init__(drr, rot, xyz, motions, target, parameterization, loss, damping, eps, check, full_detector=False)
         self.kw = dict(parameterization=parameterization, convention=convention, degrees=degrees, calibration=calibration,
                        background=background)
-        self.loss, self.eps = loss, float(loss.eps)
-        self.shared = motions.dim() == 3
-        self.target = target.detach().expand(B, 1, det.height, det.width).contiguous()
-        self._t = self.target[:, 0]
-        self.pivots = structure_pivots(drr, labels)
-        self.damping = torch.full((1 if self.shared else B,), float(damping), dtype=torch.float64, device=motions.device)
+        self.pivots = structure_pivots(drr, self.labels)
 
-    def _loss(self, img):
-        """(B,) 1 - NCC of the composite of each view."""
-        return 1.0 - self.loss(self.target, img.sum(1, keepdim=True))
+    def _composite(self, img):
+        return img.sum(1, keepdim=True)
 
-    def normal_equations(self, img, J, rects):
-        """(A (B, 6K, 6K), g (B, 6K)) float64 of each view's Gauss-Newton model of 1 - NCC (weight 1 / (H W)) at the image `img`
-        (B, S, H, W) with Jacobian J (B, K, H, W, 6) and footprints rects (B, S, 4)."""
-        B, K, H, W = img.shape[0], J.shape[1], self._t.shape[-2], self._t.shape[-1]
-        x = img.sum(1).reshape(B, H, W).contiguous()
-        A = torch.zeros(B, 6 * K, 6 * K, dtype=torch.float64, device=img.device)
-        g = torch.zeros(B, 6 * K, dtype=torch.float64, device=img.device)
-        ncc_normal_structures_equations(x, self._t, J, rects, self.eps, 1.0 / (H * W), A, g)
-        return A, g
+    def _jacobian(self, X):
+        from .structures import structures_jacobian
+        return structures_jacobian(self.drr, self.rot, self.xyz, motions=X, labels=self.labels, stop_grad=False,
+                                   return_footprints=True, **self.kw)
 
-    def step(self) -> torch.Tensor:
-        """One damped Gauss-Newton step; -> the loss after it: the mean over the views of 1 - NCC (a 0-d tensor) for shared
-        motions, the per-pose (B,) losses otherwise."""
-        from .structures import render_structures, structures_jacobian
-
-        X, drr = self.motions, self.drr
-        with torch.no_grad():
-            img, J, rects = structures_jacobian(drr, self.rot, self.xyz, motions=X, labels=self.labels, stop_grad=False,
-                                                return_footprints=True, **self.kw)
-            A, g = self.normal_equations(img, J, rects)
-            trial = lambda X_t: self._loss(render_structures(drr, self.rot, self.xyz, motions=X_t, labels=self.labels,  # noqa: E731
-                                                             **self.kw))
-            self.damping, loss = _motion_lm_update(X, A, g, self.damping, self.pivots, self.shared, self._loss(img), trial)
-            return loss
+    def _render(self, X):
+        from .structures import render_structures
+        return render_structures(self.drr, self.rot, self.xyz, motions=X, labels=self.labels, **self.kw)
 
 
-class PolyrigidLevenbergMarquardt:
+class PolyrigidLevenbergMarquardt(_MotionLevenbergMarquardt):
     """Levenberg-Marquardt registration of the K motions of a blended-rigid DRR (DRR.render_polyrigid) towards `target` on the
     global NCC of the image, with the camera pose fixed (DESIGN.md 6j).
 
-    The unknowns are the motions: `motions` (K, 4, 4), shared by the B views, or (B, K, 4, 4), one set per pose; a tensor fp32 on
-    the density's device, updated in place by step().  `weights` is render_polyrigid's lattice.  Each step takes one
-    DRR.polyrigid_jacobian (one march: the image, the per-pixel columns of every motion and their footprints), forms the
-    Gauss-Newton system of the z-normalised residual block by block over the footprints (b200drr_ncc_normal_structures), solves
-    (A + lambda diag A) delta = -g in float64, and renders one trial image with render_polyrigid.  delta_k = (omega, v) moves
-    structure k as
-        X_k <- T(c_k) exp(delta_k^) T(-c_k) X_k,
-    a left increment about the pivot c_k, the weight-weighted centroid of channel k's lattice (polyrigid.polyrigid_pivots).  The
-    trial is kept if its true loss is lower (lambda / 10 on accept, x 10 on reject).  Shared motions: one system, the mean over
-    the views, and one decision per step on the mean loss.  Per-pose motions: B independent systems and decisions.  The sampling
-    range is Trilinear's batch-global one unless alphamin / alphamax fix it; its dependence on the motions is nil (the rays do not
-    move), so the model is the image's full derivative.  No host sync once the lattice has been seen.
-
-    Only the global NCC is modelled: `loss` None (NormalizedCrossCorrelation2d(eps=eps)) or a NormalizedCrossCorrelation2d
-    without patch_size; anything else raises TypeError here."""
+    The step is _MotionLevenbergMarquardt's.  `weights` is render_polyrigid's lattice.  The Jacobian is DRR.polyrigid_jacobian's
+    (one march: the image, the per-pixel columns of every motion and their footprints), the trial render render_polyrigid's, and
+    the pivot c_k the weight-weighted centroid of channel k's lattice (polyrigid.polyrigid_pivots).  The sampling range is
+    Trilinear's batch-global one unless alphamin / alphamax fix it; its dependence on the motions is nil (the rays do not move),
+    so the model is the image's full derivative.  Full detectors only.  No host sync once the lattice has been seen."""
 
     def __init__(self, drr, rot: torch.Tensor, xyz: torch.Tensor, motions: torch.Tensor, weights: torch.Tensor, target: torch.Tensor,
                  parameterization: str = "euler_angles", convention: str | None = None, degrees: bool = False, calibration=None,
                  n_points: int = 500, alphamin=None, alphamax=None, loss=None, damping: float = 1e-3, eps: float = 1e-5):
-        from .metrics import NormalizedCrossCorrelation2d
         from .polyrigid import check_supported, polyrigid_pivots
-        from .structures import _batch_size
 
-        if loss is None:
-            loss = NormalizedCrossCorrelation2d(eps=eps)
-        elif type(loss) is not NormalizedCrossCorrelation2d or loss.patch_size is not None:
-            raise TypeError(f"PolyrigidLevenbergMarquardt models the global NCC only: NormalizedCrossCorrelation2d without "
-                            f"patch_size (or loss=None), not {type(loss).__name__}"
-                            f"{'' if getattr(loss, 'patch_size', None) is None else f'(patch_size={loss.patch_size})'}; patch-wise, "
-                            f"multiscale and gradient NCC have no block-sparse system here (use a first-order optimizer)")
-        if not torch.is_tensor(motions) or motions.dim() not in (3, 4):
-            raise ValueError(f"motions must be a (K, 4, 4) or (B, K, 4, 4) tensor updated in place, got "
-                             f"{tuple(motions.shape) if torch.is_tensor(motions) else type(motions).__name__}")
-        if not torch.is_tensor(target) or target.dim() != 4 or target.shape[1] != 1:
-            raise ValueError(f"PolyrigidLevenbergMarquardt takes a one-channel target image (B, 1, H, W), got "
-                             f"{tuple(target.shape) if torch.is_tensor(target) else type(target).__name__}")
-        det = drr.detector
-        if det.n_subsample is not None or drr.patch_size is not None:
-            raise NotImplementedError("PolyrigidLevenbergMarquardt covers the full detector only, not p_subsample or patch_size")
-        if tuple(target.shape[-2:]) != (det.height, det.width):
-            raise ValueError(f"the target {tuple(target.shape)} does not match the {det.height} x {det.width} detector")
-        B = _batch_size((rot, xyz), parameterization)
-        if target.shape[0] not in (1, B):
-            raise ValueError(f"the target's batch ({target.shape[0]}) must be 1 or the number of poses ({B})")
-        check_supported(drr, (rot, xyz), parameterization, motions, weights, {})
-        if not (target.is_cuda and target.dtype == torch.float32):
-            raise ValueError("PolyrigidLevenbergMarquardt's normal equations run on the GPU: the target must be a CUDA fp32 tensor")
-        self.drr, self.rot, self.xyz, self.motions, self.weights = drr, rot.detach(), xyz.detach(), motions, weights
+        super().__init__(drr, rot, xyz, motions, target, parameterization, loss, damping, eps,
+                         lambda: check_supported(drr, (rot, xyz), parameterization, motions, weights, {}), full_detector=True)
+        self.weights = weights
         self.kw = dict(parameterization=parameterization, convention=convention, degrees=degrees, calibration=calibration,
                        n_points=n_points, alphamin=alphamin, alphamax=alphamax)
-        self.loss, self.eps = loss, float(loss.eps)
-        self.shared = motions.dim() == 3
-        self.target = target.detach().expand(B, 1, det.height, det.width).contiguous()
-        self._t = self.target[:, 0]
         self.pivots = polyrigid_pivots(drr, weights)
-        self.damping = torch.full((1 if self.shared else B,), float(damping), dtype=torch.float64, device=motions.device)
 
-    def _loss(self, img):
-        """(B,) 1 - NCC of each view."""
-        return 1.0 - self.loss(self.target, img)
+    def _jacobian(self, X):
+        from .polyrigid import polyrigid_jacobian
+        return polyrigid_jacobian(self.drr, self.rot, self.xyz, motions=X, weights=self.weights, return_footprints=True, **self.kw)
 
-    def normal_equations(self, img, J, rects):
-        """(A (B, 6K, 6K), g (B, 6K)) float64 of each view's Gauss-Newton model of 1 - NCC (weight 1 / (H W)) at the image `img`
-        (B, 1, H, W) with Jacobian J (B, K, H, W, 6) and footprints rects (B, K, 4)."""
-        B, K, H, W = img.shape[0], J.shape[1], self._t.shape[-2], self._t.shape[-1]
-        x = img.reshape(B, H, W).contiguous()
-        A = torch.zeros(B, 6 * K, 6 * K, dtype=torch.float64, device=img.device)
-        g = torch.zeros(B, 6 * K, dtype=torch.float64, device=img.device)
-        ncc_normal_structures_equations(x, self._t, J, rects, self.eps, 1.0 / (H * W), A, g)
-        return A, g
-
-    def step(self) -> torch.Tensor:
-        """One damped Gauss-Newton step; -> the loss after it: the mean over the views of 1 - NCC (a 0-d tensor) for shared
-        motions, the per-pose (B,) losses otherwise."""
-        from .polyrigid import polyrigid_jacobian, render_polyrigid
-
-        X, drr = self.motions, self.drr
-        with torch.no_grad():
-            img, J, rects = polyrigid_jacobian(drr, self.rot, self.xyz, motions=X, weights=self.weights, return_footprints=True,
-                                               **self.kw)
-            A, g = self.normal_equations(img, J, rects)
-            trial = lambda X_t: self._loss(render_polyrigid(drr, self.rot, self.xyz, motions=X_t, weights=self.weights,  # noqa: E731
-                                                            **self.kw))
-            self.damping, loss = _motion_lm_update(X, A, g, self.damping, self.pivots, self.shared, self._loss(img), trial)
-            return loss
+    def _render(self, X):
+        from .polyrigid import render_polyrigid
+        return render_polyrigid(self.drr, self.rot, self.xyz, motions=X, weights=self.weights, **self.kw)
 
 
 def ncc_z(x, eps):
@@ -487,32 +473,14 @@ class DeformableLevenbergMarquardt:
                  damping: float = 1e-3, eps: float = 1e-5):
         from . import _lib
         from .deform import _marches, check_supported
-        from .metrics import NormalizedCrossCorrelation2d
-        from .structures import _batch_size
 
-        if loss is None:
-            loss = NormalizedCrossCorrelation2d(eps=eps)
-        elif type(loss) is not NormalizedCrossCorrelation2d or loss.patch_size is not None:
-            raise TypeError(f"DeformableLevenbergMarquardt models the global NCC only: NormalizedCrossCorrelation2d without "
-                            f"patch_size (or loss=None), not {type(loss).__name__}"
-                            f"{'' if getattr(loss, 'patch_size', None) is None else f'(patch_size={loss.patch_size})'}; patch-wise, "
-                            f"multiscale and gradient NCC have no Gauss-Newton model here (use a first-order optimizer)")
-        if not torch.is_tensor(target) or target.dim() != 4 or target.shape[1] != 1:
-            raise ValueError(f"DeformableLevenbergMarquardt takes a one-channel target image (B, 1, H, W), got "
-                             f"{tuple(target.shape) if torch.is_tensor(target) else type(target).__name__}")
-        det = drr.detector
-        if det.n_subsample is not None or drr.patch_size is not None:
-            raise NotImplementedError("DeformableLevenbergMarquardt covers the full detector only, not p_subsample or patch_size")
-        if tuple(target.shape[-2:]) != (det.height, det.width):
-            raise ValueError(f"the target {tuple(target.shape)} does not match the {det.height} x {det.width} detector")
-        B = _batch_size((rot, xyz), parameterization)
-        if target.shape[0] not in (1, B):
-            raise ValueError(f"the target's batch ({target.shape[0]}) must be 1 or the number of poses ({B})")
-        check_supported(drr, (rot, xyz), parameterization, field, {})
-        if not (target.is_cuda and target.dtype == torch.float32):
-            raise ValueError("DeformableLevenbergMarquardt runs on the GPU: the target must be a CUDA fp32 tensor")
+        name = type(self).__name__
+        loss = _global_ncc(name, loss, eps)
+        B = _check_target(name, drr, target, (rot, xyz), parameterization,
+                          lambda: check_supported(drr, (rot, xyz), parameterization, field, {}))
         if not (isinstance(cg_iters, int) and cg_iters >= 1):
             raise ValueError(f"cg_iters must be a positive int, got {cg_iters!r}")
+        det = drr.detector
         self.drr, self.rot, self.xyz, self.field = drr, rot.detach(), xyz.detach(), field
         self.kw = dict(parameterization=parameterization, convention=convention, degrees=degrees, calibration=calibration,
                        n_points=n_points, alphamin=alphamin, alphamax=alphamax)
@@ -548,23 +516,31 @@ class DeformableLevenbergMarquardt:
         ncc = 1.0 - self.loss(self.target, img)
         return (ncc.mean(0, keepdim=True) if self.shared else ncc) + self.smoothness * field_smoothness(Us)
 
+    def _chain(self, Us):
+        """The field map of the model at the system-batched unknowns Us -> (the kernels' field the march is linearised at, the
+        map from a tangent of the unknowns (S, 3, g0, g1, g2) to a tangent of that field, the adjoint of that map): here the field
+        is Us itself in voxel units (voxel_field), and the map is voxel_field, whose adjoint in voxel units is the identity."""
+        from .deform import voxel_field
+
+        return voxel_field(self.drr, Us), lambda v: voxel_field(self.drr, v), lambda g: g
+
     def _model(self, Us, img):
-        """(grad, H) of the Gauss-Newton model at the system-batched field Us and its image: grad() -> g (S, 3, g0, g1, g2) (one
-        scatter march) and the product H(v) on the same shape (two marches)."""
-        from .deform import field_jvp, field_vjp, voxel_field
+        """(grad, H) of the Gauss-Newton model at the system-batched unknowns Us and their image: grad() -> g (S, 3, g0, g1, g2)
+        (one scatter march) and the product H(v) on the same shape (two marches), each through the field map of _chain."""
+        from .deform import field_jvp, field_vjp
 
         drr, packed = self.drr, self.drr.renderer._packed_volume(self.drr.density)
         source, tgt, lens, arange, grid = self._rays
         n_points = int(self.kw["n_points"])
-        Uv = voxel_field(drr, Us)
+        U, tangent, adjoint = self._chain(Us)
         z, sigma = ncc_z(img.reshape(self.B, self.N), self.eps)
 
         def JT(w):
-            gv = field_vjp(drr, packed, source, tgt, lens, Uv, w, arange, n_points, grid, scratch=self._scratch)
+            gv = adjoint(field_vjp(drr, packed, source, tgt, lens, U, w, arange, n_points, grid, scratch=self._scratch))
             return torch.einsum("ij,bxyzi->bjxyz", self._lin, gv[..., :3])
 
         def H(v):
-            jv = field_jvp(drr, packed, source, tgt, lens, Uv, voxel_field(drr, v), arange, n_points, grid)
+            jv = field_jvp(drr, packed, source, tgt, lens, U, tangent(v), arange, n_points, grid)
             return JT(self._wt * ncc_z_jvp(ncc_z_jvp(jv, z, sigma), z, sigma)) + self.smoothness * field_smoothness_grad(v)
 
         def grad():
@@ -614,7 +590,7 @@ class DeformableLevenbergMarquardt:
             accept = E_t < E  # a NaN trial is rejected
             U.copy_(torch.where(accept.reshape(-1, *[1] * 4), Us_t, Us).reshape(U.shape))
             self._img = self._keep(accept, img_t, img)
-            self.mu = torch.where(accept, self.mu / 10.0, self.mu * 10.0).clamp(1e-12, 1e12)
+            self.mu = _next_damping(accept, self.mu)
             out = torch.where(accept, E_t, E)
             return out[0] if self.shared else out
 
@@ -670,29 +646,13 @@ class DiffeomorphicLevenbergMarquardt(DeformableLevenbergMarquardt):
         self._exp = ([torch.where(on, a, b) for a, b in zip(levels_t, levels)], torch.where(on, phi_t, phi))
         return super()._keep(accept, img_t, img)
 
-    def _model(self, Vs, img):
-        """(grad, H) of the Gauss-Newton model at the system-batched velocity Vs and its image, through the levels of the current
-        velocity: grad() one scatter march and `steps` adjoint squarings, H(v) two marches and 2 steps lattice launches."""
-        from .deform import field_jvp, field_vjp, voxel_field
+    def _chain(self, Vs):
+        """The exponential at the current velocity: the march is linearised at exp(V), a velocity tangent goes through the tangent
+        squarings (square_chain_jvp) and a field gradient back through their adjoints (square_chain_bwd), over the levels of the
+        current V."""
+        from .deform import voxel_field
         from .svf import square_chain_bwd, square_chain_jvp
 
-        drr, packed = self.drr, self.drr.renderer._packed_volume(self.drr.density)
-        source, tgt, lens, arange, grid = self._rays
-        n_points = int(self.kw["n_points"])
         levels, phi = self._exp
-        z, sigma = ncc_z(img.reshape(self.B, self.N), self.eps)
-
-        def JT(w):
-            gphi = field_vjp(drr, packed, source, tgt, lens, phi, w, arange, n_points, grid, scratch=self._scratch)
-            gv = square_chain_bwd(levels, gphi, self._dims)
-            return torch.einsum("ij,bxyzi->bjxyz", self._lin, gv[..., :3])
-
-        def H(v):
-            dphi = square_chain_jvp(levels, voxel_field(drr, v), self._dims)[1]
-            jv = field_jvp(drr, packed, source, tgt, lens, phi, dphi, arange, n_points, grid)
-            return JT(self._wt * ncc_z_jvp(ncc_z_jvp(jv, z, sigma), z, sigma)) + self.smoothness * field_smoothness_grad(v)
-
-        def grad():
-            return JT(self._wt * ncc_z_jvp(z - self._zt, z, sigma)) + self.smoothness * field_smoothness_grad(Vs)
-
-        return grad, H
+        return (phi, lambda v: square_chain_jvp(levels, voxel_field(self.drr, v), self._dims)[1],
+                lambda g: square_chain_bwd(levels, g, self._dims))

@@ -248,70 +248,6 @@ _SIGNATURES = {
     "b200drr_mi_bwd": (ctypes.c_int, [
         _c_float_p, _c_float_p, _c_float_p, _c_float_p, _c_float_p, _c_float_p, _c_float_p, _c_float_p, ctypes.c_int,
         ctypes.c_int64, ctypes.c_int, ctypes.c_void_p]),
-    # 16-bit volumes (vol pointer, vol_type, then the fp32 entry point's arguments)
-    "b200drr_siddon_fwd_v16": (ctypes.c_int, [
-        ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, _c_float_p, _c_float_p, _c_float_p, _c_float_p,
-        ctypes.c_int, ctypes.c_int64, ctypes.c_float, ctypes.c_float, ctypes.c_int, ctypes.c_int, ctypes.c_void_p]),
-    "b200drr_siddon_fwd_sens_v16": (ctypes.c_int, [
-        ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, _c_float_p, _c_float_p, _c_float_p, _c_float_p,
-        _c_float_p, ctypes.c_int, ctypes.c_int64, ctypes.c_float, ctypes.c_float, ctypes.c_void_p]),
-    "b200drr_siddon_fwd_sorted_v16": (ctypes.c_int, [
-        ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, _c_float_p, _c_float_p, _c_float_p, _c_float_p,
-        ctypes.c_int, ctypes.c_int64, ctypes.c_float, ctypes.c_float, ctypes.c_void_p]),
-    "b200drr_siddon_fwd_sens_sorted_v16": (ctypes.c_int, [
-        ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, _c_float_p, _c_float_p, _c_float_p, _c_float_p,
-        _c_float_p, ctypes.c_int, ctypes.c_int64, ctypes.c_float, ctypes.c_float, ctypes.c_void_p]),
-    "b200drr_siddon_fwd_grid_v16": (ctypes.c_int, [
-        ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, _c_float_p, _c_float_p, _c_float_p, _c_float_p,
-        ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_float, ctypes.c_float, ctypes.c_int, ctypes.c_void_p]),
-    "b200drr_siddon_fwd_sens_grid_v16": (ctypes.c_int, [
-        ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, _c_float_p, _c_float_p, _c_float_p, _c_float_p,
-        _c_float_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_float, ctypes.c_float, ctypes.c_int, ctypes.c_void_p]),
-    "b200drr_siddon_fwd_brick_v16": (ctypes.c_int, [
-        ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, _c_float_p, _c_float_p, _c_float_p, _c_float_p,
-        _c_float_p, _c_float_p, _c_float_p, _c_float_p, ctypes.c_void_p, ctypes.c_int64, ctypes.c_int, ctypes.c_int, ctypes.c_int,
-        ctypes.c_float, ctypes.c_float, ctypes.c_int, ctypes.c_void_p]),
-    "b200drr_siddon_fwd_brick_subset_v16": (ctypes.c_int, [
-        ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, _c_float_p, _c_float_p, _c_float_p,
-        ctypes.c_void_p, _c_float_p, _c_float_p, ctypes.c_void_p, ctypes.c_int64, ctypes.c_int, ctypes.c_int, ctypes.c_int,
-        ctypes.c_int64, ctypes.c_float, ctypes.c_float, ctypes.c_int, ctypes.c_void_p]),
-    "b200drr_siddon_fwd_pose_v16": (ctypes.c_int, [
-        ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, _c_float_p, _c_float_p, _c_float_p, _c_float_p,
-        _c_float_p, _c_float_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_float, ctypes.c_float, ctypes.c_void_p]),
-    "b200drr_siddon_fwd_sens_pose_v16": (ctypes.c_int, [
-        ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, _c_float_p, _c_float_p, _c_float_p, _c_float_p,
-        _c_float_p, _c_float_p, _c_float_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_float, ctypes.c_float,
-        ctypes.c_void_p]),
-    "b200drr_siddon_fwd_sens_structures_v16": (ctypes.c_int, [
-        ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, _c_float_p, _c_float_p,
-        _c_float_p, _c_float_p, _c_float_p, ctypes.c_void_p, ctypes.c_void_p, _c_float_p, _c_float_p, ctypes.c_int, ctypes.c_int,
-        ctypes.c_int, ctypes.c_int, ctypes.c_float, ctypes.c_float, ctypes.c_void_p]),
-    "b200drr_pack_corners_v16": (ctypes.c_int, [
-        ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p]),
-    "b200drr_trilinear_fwd_v16": (ctypes.c_int, [
-        ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, _c_float_p, _c_float_p, _c_float_p, _c_float_p,
-        ctypes.c_int, ctypes.c_int64, ctypes.c_float, ctypes.c_float, ctypes.c_int, _c_float_p, ctypes.c_int, ctypes.c_int,
-        ctypes.c_void_p]),
-    "b200drr_trilinear_fwd_grid_v16": (ctypes.c_int, [
-        ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, _c_float_p, _c_float_p, _c_float_p, _c_float_p,
-        ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_float, ctypes.c_float, ctypes.c_int, _c_float_p, ctypes.c_int,
-        ctypes.c_void_p]),
-    "b200drr_trilinear_fwd_sens_v16": (ctypes.c_int, [
-        ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, _c_float_p, _c_float_p, _c_float_p, _c_float_p,
-        _c_float_p, ctypes.c_int, ctypes.c_int64, ctypes.c_int, ctypes.c_int, ctypes.c_float, ctypes.c_float, ctypes.c_int,
-        _c_float_p, ctypes.c_int, ctypes.c_void_p]),
-    "b200drr_trilinear_fwd_packed_v16": (ctypes.c_int, [
-        ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, _c_float_p, _c_float_p, _c_float_p, _c_float_p,
-        ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_float, ctypes.c_float, ctypes.c_int, _c_float_p, ctypes.c_int,
-        ctypes.c_void_p]),
-    "b200drr_trilinear_fwd_sens_packed_v16": (ctypes.c_int, [
-        ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, _c_float_p, _c_float_p, _c_float_p, _c_float_p,
-        _c_float_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_float, ctypes.c_float, ctypes.c_int, _c_float_p,
-        ctypes.c_int, ctypes.c_void_p]),
-    "b200drr_trilinear_fwd_sens_pose_v16": (ctypes.c_int, [
-        ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, _c_float_p, _c_float_p, _c_float_p, _c_float_p,
-        _c_float_p, _c_float_p, _c_float_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_float, ctypes.c_float,
-        ctypes.c_int, _c_float_p, ctypes.c_int, ctypes.c_void_p]),
     # blended-rigid (skinned) trilinear render
     "b200drr_polyrigid_weight_floats": (ctypes.c_int64, [ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int]),
     "b200drr_polyrigid_pack_weights": (ctypes.c_int, [
@@ -326,25 +262,11 @@ _SIGNATURES = {
         ctypes.c_int, ctypes.c_int, _c_float_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, _c_float_p, _c_float_p, _c_float_p,
         _c_float_p, _c_float_p, _c_float_p, _c_float_p, ctypes.c_int, ctypes.c_int64, ctypes.c_int, ctypes.c_int, ctypes.c_float,
         ctypes.c_float, ctypes.c_int, _c_float_p, ctypes.c_void_p]),
-    "b200drr_polyrigid_fwd_v16": (ctypes.c_int, [
-        ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, _c_float_p, _c_float_p, _c_float_p,
-        _c_float_p, ctypes.c_int, ctypes.c_int, _c_float_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, _c_float_p, ctypes.c_int,
-        ctypes.c_int64, ctypes.c_int, ctypes.c_int, ctypes.c_float, ctypes.c_float, ctypes.c_int, _c_float_p, ctypes.c_void_p]),
-    "b200drr_polyrigid_bwd_v16": (ctypes.c_int, [
-        ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, _c_float_p, _c_float_p, _c_float_p,
-        _c_float_p, ctypes.c_int, ctypes.c_int, _c_float_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, _c_float_p, _c_float_p,
-        _c_float_p, _c_float_p, _c_float_p, _c_float_p, _c_float_p, ctypes.c_int, ctypes.c_int64, ctypes.c_int, ctypes.c_int,
-        ctypes.c_float, ctypes.c_float, ctypes.c_int, _c_float_p, ctypes.c_void_p]),
     "b200drr_polyrigid_jac": (ctypes.c_int, [
         _c_float_p, _c_float_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, _c_float_p, _c_float_p, _c_float_p, _c_float_p,
         ctypes.c_int, ctypes.c_int, _c_float_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, _c_float_p, _c_float_p, _c_float_p,
         ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_float, ctypes.c_float, ctypes.c_int, _c_float_p,
         ctypes.c_void_p]),
-    "b200drr_polyrigid_jac_v16": (ctypes.c_int, [
-        ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, _c_float_p, _c_float_p, _c_float_p,
-        _c_float_p, ctypes.c_int, ctypes.c_int, _c_float_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, _c_float_p, _c_float_p,
-        _c_float_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_float, ctypes.c_float, ctypes.c_int,
-        _c_float_p, ctypes.c_void_p]),
     # deformable (dense displacement field) trilinear render
     "b200drr_deform_scratch_floats": (ctypes.c_int64, [ctypes.c_int, ctypes.c_int64, ctypes.c_int, ctypes.c_int]),
     "b200drr_deform_fwd": (ctypes.c_int, [
@@ -356,23 +278,10 @@ _SIGNATURES = {
         ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, _c_float_p, _c_float_p, _c_float_p, _c_float_p, _c_float_p,
         _c_float_p, _c_float_p, ctypes.c_int, ctypes.c_int64, ctypes.c_int, ctypes.c_int, ctypes.c_float, ctypes.c_float,
         ctypes.c_int, _c_float_p, ctypes.c_void_p]),
-    "b200drr_deform_fwd_v16": (ctypes.c_int, [
-        ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, _c_float_p, _c_float_p, _c_float_p,
-        _c_float_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, _c_float_p, ctypes.c_int, ctypes.c_int64, ctypes.c_int,
-        ctypes.c_int, ctypes.c_float, ctypes.c_float, ctypes.c_int, _c_float_p, ctypes.c_void_p]),
-    "b200drr_deform_bwd_v16": (ctypes.c_int, [
-        ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, _c_float_p, _c_float_p, _c_float_p,
-        _c_float_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, _c_float_p, _c_float_p, _c_float_p, _c_float_p,
-        _c_float_p, _c_float_p, _c_float_p, ctypes.c_int, ctypes.c_int64, ctypes.c_int, ctypes.c_int, ctypes.c_float, ctypes.c_float,
-        ctypes.c_int, _c_float_p, ctypes.c_void_p]),
     "b200drr_deform_jvp": (ctypes.c_int, [
         _c_float_p, _c_float_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, _c_float_p, _c_float_p, _c_float_p, _c_float_p,
         ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, _c_float_p, _c_float_p, _c_float_p, ctypes.c_int, ctypes.c_int64,
         ctypes.c_int, ctypes.c_int, ctypes.c_float, ctypes.c_float, ctypes.c_int, _c_float_p, ctypes.c_void_p]),
-    "b200drr_deform_jvp_v16": (ctypes.c_int, [
-        ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, _c_float_p, _c_float_p, _c_float_p,
-        _c_float_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, _c_float_p, _c_float_p, _c_float_p, ctypes.c_int,
-        ctypes.c_int64, ctypes.c_int, ctypes.c_int, ctypes.c_float, ctypes.c_float, ctypes.c_int, _c_float_p, ctypes.c_void_p]),
     "b200drr_deform_bproj": (ctypes.c_int, [
         ctypes.c_int, ctypes.c_int, ctypes.c_int, _c_float_p, _c_float_p, _c_float_p, _c_float_p, ctypes.c_int, ctypes.c_int,
         ctypes.c_int, ctypes.c_int, _c_float_p, _c_float_p, ctypes.c_int, ctypes.c_int64, ctypes.c_int, ctypes.c_int, ctypes.c_float,
@@ -388,6 +297,23 @@ _SIGNATURES = {
         _c_float_p, _c_float_p, _c_float_p, _c_float_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int,
         ctypes.c_int, ctypes.c_int, ctypes.c_float, ctypes.c_void_p]),
 }
+
+
+def _v16(name):
+    """The 16-bit twin's signature: its fp32 entry point's, with vol_type after the volume (after vol and packed for the
+    blended-rigid and deformable renders)."""
+    restype, argtypes = _SIGNATURES[name]
+    at = 2 if name.startswith(("b200drr_polyrigid", "b200drr_deform")) else 1
+    return restype, argtypes[:at] + [ctypes.c_int] + argtypes[at:]
+
+
+_SIGNATURES.update({f"{name}_v16": _v16(name) for name in (
+    "b200drr_siddon_fwd", "b200drr_siddon_fwd_sens", "b200drr_siddon_fwd_sorted", "b200drr_siddon_fwd_sens_sorted",
+    "b200drr_siddon_fwd_grid", "b200drr_siddon_fwd_sens_grid", "b200drr_siddon_fwd_brick", "b200drr_siddon_fwd_brick_subset",
+    "b200drr_siddon_fwd_pose", "b200drr_siddon_fwd_sens_pose", "b200drr_siddon_fwd_sens_structures", "b200drr_pack_corners",
+    "b200drr_trilinear_fwd", "b200drr_trilinear_fwd_grid", "b200drr_trilinear_fwd_sens", "b200drr_trilinear_fwd_packed",
+    "b200drr_trilinear_fwd_sens_packed", "b200drr_trilinear_fwd_sens_pose", "b200drr_polyrigid_fwd", "b200drr_polyrigid_bwd",
+    "b200drr_polyrigid_jac", "b200drr_deform_fwd", "b200drr_deform_bwd", "b200drr_deform_jvp")})
 
 # entry points of rejected experiments (include/b200drr_experimental.h): bound only when the experimental build is loaded
 _EXPERIMENTAL_SIGNATURES = {

@@ -2,6 +2,7 @@
 #include <cuda_runtime.h>
 
 #include <algorithm>
+#include <type_traits>
 
 #include "../../include/b200drr.h"
 #ifdef B200DRR_EXPERIMENTS
@@ -15,6 +16,8 @@ namespace {
 
 inline bool bad_dims(int D0, int D1, int D2) { return D0 <= 0 || D1 <= 0 || D2 <= 0; }
 inline bool bad_rays(int B, int64_t N) { return B <= 0 || B > 65535 || N <= 0; }
+inline bool bad_grid(int B, int H, int W) { return bad_rays(B, (int64_t)H * W) || H <= 0 || W <= 0; }  // B detectors of H x W rays
+inline bool too_big(int D0, int D1, int D2) { return (int64_t)D0 * D1 * D2 >= (int64_t)INT32_MAX; }
 inline VolDims mk(int D0, int D1, int D2)
 {
     VolDims d;
@@ -59,7 +62,16 @@ int with_vox16(int vol_type, F&& f)
     if (vol_type == B200DRR_VOL_BF16) return f(VoxBF16{});
     return B200DRR_EINVAL;
 }
-inline bool too_big(int D0, int D1, int D2) { return (int64_t)D0 * D1 * D2 >= (int64_t)INT32_MAX; }
+inline bool bad_vol16(int vol_type) { return vol_type != B200DRR_VOL_F16 && vol_type != B200DRR_VOL_BF16; }
+
+// the brick kernels' refusals after the argument checks, in this order: a shape the TMA map cannot take or a volume (or volume
+// gradient) off 16 bytes is B200DRR_EUNSUPPORTED, a workspace under `need` bytes or off 256 bytes B200DRR_EINVAL; 0 = go on
+int brick_bad(const void* vol, VolDims d, int H, int W, int elem_bytes, const void* workspace, int64_t workspace_bytes, size_t need)
+{
+    if (!siddon_brick_supported(d, H, W, elem_bytes) || ((uintptr_t)vol & 15u) != 0) return B200DRR_EUNSUPPORTED;
+    if (workspace_bytes < (int64_t)need || ((uintptr_t)workspace & 255u) != 0) return B200DRR_EINVAL;
+    return 0;
+}
 }  // namespace
 
 extern "C" {
@@ -90,26 +102,6 @@ int b200drr_device_cc(void)
     if (cudaDeviceGetAttribute(&ma, cudaDevAttrComputeCapabilityMajor, dev) != cudaSuccess) return 0;
     if (cudaDeviceGetAttribute(&mi, cudaDevAttrComputeCapabilityMinor, dev) != cudaSuccess) return 0;
     return ma * 10 + mi;
-}
-
-int b200drr_siddon_fwd(const float* vol, int D0, int D1, int D2, const float* src, const float* tgt,
-                       const float* raylen, float* out, int B, int64_t N, float voxel_shift, float eps, int reduce,
-                       int align_corners, void* stream)
-{
-    if (!vol || !src || !tgt || !raylen || !out || bad_dims(D0, D1, D2) || bad_rays(B, N) || reduce < 0 || reduce > 1)
-        return B200DRR_EINVAL;
-    return ret(launch_siddon_fwd(vol, mk(D0, D1, D2), src, tgt, raylen, out, B, N, voxel_shift, eps, reduce,
-                                 align_corners != 0, (cudaStream_t)stream));
-}
-
-int b200drr_siddon_fwd_grid(const float* vol, int D0, int D1, int D2, const float* src, const float* tgt,
-                            const float* raylen, float* out, int B, int H, int W, float voxel_shift, float eps,
-                            int variant, void* stream)
-{
-    if (!vol || !src || !tgt || !raylen || !out || bad_dims(D0, D1, D2) || bad_rays(B, (int64_t)H * W) || H <= 0 || W <= 0)
-        return B200DRR_EINVAL;
-    return ret(launch_siddon_fwd_grid(vol, mk(D0, D1, D2), src, tgt, raylen, out, B, H, W, voxel_shift, eps, variant,
-                                      (cudaStream_t)stream));
 }
 
 int b200drr_siddon_fwd_f64(const double* vol, int D0, int D1, int D2, const double* src, const double* tgt, const double* raylen,
@@ -179,44 +171,10 @@ int b200drr_segments_bwd(int kind, int is_f64, const void* vol, int D0, int D1, 
                                         B, N, voxel_shift, eps, n_points, alpha_range, stop_grad != 0, align_corners != 0, stream);
 }
 
-int b200drr_siddon_fwd_sorted(const float* vol, int D0, int D1, int D2, const float* src, const float* tgt, const float* raylen,
-                              float* out, int B, int64_t N, float voxel_shift, float eps, void* stream)
-{
-    if (!vol || !src || !tgt || !raylen || !out || bad_dims(D0, D1, D2) || bad_rays(B, N)) return B200DRR_EINVAL;
-    if ((int64_t)D0 * D1 * D2 >= (int64_t)INT32_MAX) return B200DRR_EUNSUPPORTED;
-    return ret(launch_siddon_fwd_sorted(vol, mk(D0, D1, D2), src, tgt, raylen, out, B, N, voxel_shift, eps, (cudaStream_t)stream));
-}
-
-int b200drr_siddon_fwd_sens_sorted(const float* vol, int D0, int D1, int D2, const float* src, const float* tgt,
-                                   const float* raylen, float* out, float* sens, int B, int64_t N, float voxel_shift, float eps,
-                                   void* stream)
-{
-    if (!vol || !src || !tgt || !raylen || !out || !sens || bad_dims(D0, D1, D2) || bad_rays(B, N)) return B200DRR_EINVAL;
-    if ((int64_t)D0 * D1 * D2 >= (int64_t)INT32_MAX) return B200DRR_EUNSUPPORTED;
-    return ret(launch_siddon_fwd_sens_sorted(vol, mk(D0, D1, D2), src, tgt, raylen, out, sens, B, N, voxel_shift, eps,
-                                             (cudaStream_t)stream));
-}
-
 int64_t b200drr_siddon_brick_workspace_bytes(int B, int H, int W)
 {
     if (B <= 0 || H <= 0 || W <= 0) return 0;
     return (int64_t)siddon_brick_workspace_bytes(B, H, W);
-}
-
-int b200drr_siddon_fwd_brick(const float* vol, int D0, int D1, int D2, const float* src, const float* tgt,
-                             const float* raylen, const float* G, const float* Wd, const float* rows, const float* cols,
-                             float* out, void* workspace, int64_t workspace_bytes, int B, int H, int W, float voxel_shift,
-                             float eps, int variant, void* stream)
-{
-    const bool pose_in = G != nullptr;
-    if (!vol || !src || !out || !workspace || bad_dims(D0, D1, D2) || bad_rays(B, (int64_t)H * W) || H <= 0 || W <= 0)
-        return B200DRR_EINVAL;
-    if (pose_in ? (!Wd || !rows || !cols) : (!tgt || !raylen)) return B200DRR_EINVAL;
-    if (!siddon_brick_supported(mk(D0, D1, D2), H, W) || ((uintptr_t)vol & 15u) != 0) return B200DRR_EUNSUPPORTED;
-    if (workspace_bytes < (int64_t)siddon_brick_workspace_bytes(B, H, W) || ((uintptr_t)workspace & 255u) != 0)
-        return B200DRR_EINVAL;
-    return ret(launch_siddon_fwd_brick(vol, mk(D0, D1, D2), src, tgt, raylen, G, Wd, rows, cols, out, workspace,
-                                       (size_t)workspace_bytes, B, H, W, voxel_shift, eps, variant, (cudaStream_t)stream));
 }
 
 int b200drr_siddon_bwd_vol_brick(const float* gout, int D0, int D1, int D2, const float* src, const float* tgt, const float* raylen,
@@ -225,7 +183,7 @@ int b200drr_siddon_bwd_vol_brick(const float* gout, int D0, int D1, int D2, cons
                                  void* stream)
 {
     const bool pose_in = G != nullptr;
-    if (!gout || !src || !g_vol || !workspace || bad_dims(D0, D1, D2) || bad_rays(B, (int64_t)H * W) || H <= 0 || W <= 0)
+    if (!gout || !src || !g_vol || !workspace || bad_dims(D0, D1, D2) || bad_grid(B, H, W))
         return B200DRR_EINVAL;
     if (pose_in ? (!Wd || !rows || !cols) : (!tgt || !raylen)) return B200DRR_EINVAL;
     if (!siddon_brick_supported(mk(D0, D1, D2), H, W) || ((uintptr_t)g_vol & 15u) != 0) return B200DRR_EUNSUPPORTED;
@@ -233,22 +191,6 @@ int b200drr_siddon_bwd_vol_brick(const float* gout, int D0, int D1, int D2, cons
         return B200DRR_EINVAL;
     return ret(launch_siddon_bwd_vol_brick(gout, mk(D0, D1, D2), src, tgt, raylen, G, Wd, rows, cols, g_vol, workspace,
                                            (size_t)workspace_bytes, B, H, W, voxel_shift, eps, (cudaStream_t)stream));
-}
-
-int b200drr_siddon_fwd_brick_subset(const float* vol, int D0, int D1, int D2, const float* src, const float* tgt,
-                                    const float* raylen, const int32_t* pix_index, const float* corners, float* out,
-                                    void* workspace, int64_t workspace_bytes, int B, int H, int W, int64_t Nsub,
-                                    float voxel_shift, float eps, int variant, void* stream)
-{
-    if (!vol || !src || !tgt || !raylen || !pix_index || !corners || !out || !workspace || bad_dims(D0, D1, D2) ||
-        bad_rays(B, Nsub) || H <= 0 || W <= 0 || Nsub > (int64_t)H * W)
-        return B200DRR_EINVAL;
-    if (!siddon_brick_supported(mk(D0, D1, D2), H, W) || ((uintptr_t)vol & 15u) != 0) return B200DRR_EUNSUPPORTED;
-    if (workspace_bytes < (int64_t)siddon_brick_workspace_bytes(B, 1, (int)Nsub) || ((uintptr_t)workspace & 255u) != 0)
-        return B200DRR_EINVAL;
-    return ret(launch_siddon_fwd_brick(vol, mk(D0, D1, D2), src, tgt, raylen, nullptr, nullptr, nullptr, nullptr, out, workspace,
-                                       (size_t)workspace_bytes, B, H, W, voxel_shift, eps, variant, (cudaStream_t)stream,
-                                       pix_index, corners, Nsub));
 }
 
 int b200drr_siddon_bwd(const float* vol, int D0, int D1, int D2, const float* src, const float* tgt,
@@ -267,21 +209,10 @@ int b200drr_siddon_bwd_grid(const float* vol, int D0, int D1, int D2, const floa
                             float* g_vol, int B, int H, int W, float voxel_shift, float eps, int stop_grad, int variant,
                             void* stream)
 {
-    if (!vol || !src || !tgt || !raylen || !gout || bad_dims(D0, D1, D2) || bad_rays(B, (int64_t)H * W) || H <= 0 || W <= 0)
+    if (!vol || !src || !tgt || !raylen || !gout || bad_dims(D0, D1, D2) || bad_grid(B, H, W))
         return B200DRR_EINVAL;
     return ret(launch_siddon_bwd_grid(vol, mk(D0, D1, D2), src, tgt, raylen, gout, g_src, g_tgt, g_raylen, g_vol, B, H, W,
                                       voxel_shift, eps, stop_grad != 0, variant, (cudaStream_t)stream));
-}
-
-int b200drr_trilinear_fwd(const float* vol, int D0, int D1, int D2, const float* src, const float* tgt,
-                          const float* raylen, float* out, int B, int64_t N, float voxel_shift, float eps,
-                          int n_points, const float* alpha_range, int reduce, int align_corners, void* stream)
-{
-    if (!vol || !src || !tgt || !raylen || !out || !alpha_range || bad_dims(D0, D1, D2) || bad_rays(B, N) ||
-        n_points < 2 || reduce < 0 || reduce > 1)
-        return B200DRR_EINVAL;
-    return ret(launch_trilinear_fwd(vol, mk(D0, D1, D2), src, tgt, raylen, out, B, N, voxel_shift, eps, n_points,
-                                    alpha_range, reduce, align_corners != 0, (cudaStream_t)stream));
 }
 
 int b200drr_trilinear_bwd(const float* vol, int D0, int D1, int D2, const float* src, const float* tgt,
@@ -297,40 +228,16 @@ int b200drr_trilinear_bwd(const float* vol, int D0, int D1, int D2, const float*
                                     (cudaStream_t)stream));
 }
 
-int b200drr_trilinear_fwd_grid(const float* vol, int D0, int D1, int D2, const float* src, const float* tgt,
-                               const float* raylen, float* out, int B, int H, int W, float voxel_shift, float eps,
-                               int n_points, const float* alpha_range, int variant, void* stream)
-{
-    if (!vol || !src || !tgt || !raylen || !out || !alpha_range || bad_dims(D0, D1, D2) || bad_rays(B, (int64_t)H * W) ||
-        H <= 0 || W <= 0 || n_points < 2)
-        return B200DRR_EINVAL;
-    return ret(launch_trilinear_fwd_grid(vol, mk(D0, D1, D2), src, tgt, raylen, out, B, H, W, voxel_shift, eps, n_points,
-                                         alpha_range, variant, (cudaStream_t)stream));
-}
-
 int b200drr_trilinear_bwd_grid(const float* vol, int D0, int D1, int D2, const float* src, const float* tgt,
                                const float* raylen, const float* gout, float* g_src, float* g_tgt, float* g_raylen,
                                float* g_vol, float* g_alpha_range, int B, int H, int W, float voxel_shift, float eps,
                                int n_points, const float* alpha_range, int variant, void* stream)
 {
-    if (!vol || !src || !tgt || !raylen || !gout || !alpha_range || bad_dims(D0, D1, D2) || bad_rays(B, (int64_t)H * W) ||
-        H <= 0 || W <= 0 || n_points < 2)
+    if (!vol || !src || !tgt || !raylen || !gout || !alpha_range || bad_dims(D0, D1, D2) || bad_grid(B, H, W) || n_points < 2)
         return B200DRR_EINVAL;
     return ret(launch_trilinear_bwd_grid(vol, mk(D0, D1, D2), src, tgt, raylen, gout, g_src, g_tgt, g_raylen, g_vol,
                                          g_alpha_range, B, H, W, voxel_shift, eps, n_points, alpha_range, variant,
                                          (cudaStream_t)stream));
-}
-
-int b200drr_siddon_fwd_pose(const float* vol, int D0, int D1, int D2, const float* src, const float* G, const float* Wd,
-                            const float* rows, const float* cols, float* out, int B, int H, int W, float voxel_shift,
-                            float eps, void* stream)
-{
-    if (!vol || !src || !G || !Wd || !rows || !cols || !out || bad_dims(D0, D1, D2) || bad_rays(B, (int64_t)H * W) ||
-        H <= 0 || W <= 0)
-        return B200DRR_EINVAL;
-    if ((int64_t)D0 * D1 * D2 >= (int64_t)INT32_MAX) return B200DRR_EUNSUPPORTED;
-    return ret(launch_siddon_fwd_pose(vol, mk(D0, D1, D2), src, G, Wd, rows, cols, out, B, H, W, voxel_shift, eps,
-                                      (cudaStream_t)stream));
 }
 
 int b200drr_siddon_bwd_pose(const float* vol, int D0, int D1, int D2, const float* src, const float* G, const float* Wd,
@@ -339,45 +246,11 @@ int b200drr_siddon_bwd_pose(const float* vol, int D0, int D1, int D2, const floa
                             int stop_grad, void* stream)
 {
     if (!vol || !src || !G || !Wd || !rows || !cols || !gout || !g_src || !g_G || !g_Wd || !ws_tgt || !ws_len ||
-        bad_dims(D0, D1, D2) || bad_rays(B, (int64_t)H * W) || H <= 0 || W <= 0)
+        bad_dims(D0, D1, D2) || bad_grid(B, H, W))
         return B200DRR_EINVAL;
-    if ((int64_t)D0 * D1 * D2 >= (int64_t)INT32_MAX) return B200DRR_EUNSUPPORTED;
+    if (too_big(D0, D1, D2)) return B200DRR_EUNSUPPORTED;
     return ret(launch_siddon_bwd_pose(vol, mk(D0, D1, D2), src, G, Wd, rows, cols, gout, g_src, g_G, g_Wd, g_vol, ws_tgt,
                                       ws_len, B, H, W, voxel_shift, eps, stop_grad != 0, (cudaStream_t)stream));
-}
-
-int b200drr_siddon_fwd_sens(const float* vol, int D0, int D1, int D2, const float* src, const float* tgt,
-                            const float* raylen, float* out, float* sens, int B, int64_t N, float voxel_shift, float eps,
-                            void* stream)
-{
-    if (!vol || !src || !tgt || !raylen || !out || !sens || bad_dims(D0, D1, D2) || bad_rays(B, N)) return B200DRR_EINVAL;
-    if ((int64_t)D0 * D1 * D2 >= (int64_t)INT32_MAX) return B200DRR_EUNSUPPORTED;
-    return ret(launch_siddon_fwd_sens(vol, mk(D0, D1, D2), src, tgt, raylen, out, sens, B, N, voxel_shift, eps,
-                                      (cudaStream_t)stream));
-}
-
-int b200drr_siddon_fwd_sens_grid(const float* vol, int D0, int D1, int D2, const float* src, const float* tgt,
-                                 const float* raylen, float* out, float* sens, int B, int H, int W, float voxel_shift,
-                                 float eps, int variant, void* stream)
-{
-    if (!vol || !src || !tgt || !raylen || !out || !sens || bad_dims(D0, D1, D2) || bad_rays(B, (int64_t)H * W) || H <= 0 ||
-        W <= 0)
-        return B200DRR_EINVAL;
-    if ((int64_t)D0 * D1 * D2 >= (int64_t)INT32_MAX) return B200DRR_EUNSUPPORTED;
-    return ret(launch_siddon_fwd_sens_grid(vol, mk(D0, D1, D2), src, tgt, raylen, out, sens, B, H, W, voxel_shift, eps,
-                                           variant, (cudaStream_t)stream));
-}
-
-int b200drr_siddon_fwd_sens_pose(const float* vol, int D0, int D1, int D2, const float* src, const float* G, const float* Wd,
-                                 const float* rows, const float* cols, float* out, float* sens, int B, int H, int W,
-                                 float voxel_shift, float eps, void* stream)
-{
-    if (!vol || !src || !G || !Wd || !rows || !cols || !out || !sens || bad_dims(D0, D1, D2) ||
-        bad_rays(B, (int64_t)H * W) || H <= 0 || W <= 0)
-        return B200DRR_EINVAL;
-    if ((int64_t)D0 * D1 * D2 >= (int64_t)INT32_MAX) return B200DRR_EUNSUPPORTED;
-    return ret(launch_siddon_fwd_sens_pose(vol, mk(D0, D1, D2), src, G, Wd, rows, cols, out, sens, B, H, W, voxel_shift, eps,
-                                           (cudaStream_t)stream));
 }
 
 int b200drr_label_boxes(const uint8_t* labels, int D0, int D1, int D2, int32_t* boxes, void* stream)
@@ -385,20 +258,6 @@ int b200drr_label_boxes(const uint8_t* labels, int D0, int D1, int D2, int32_t* 
     if (!labels || !boxes || bad_dims(D0, D1, D2)) return B200DRR_EINVAL;
     if (too_big(D0, D1, D2)) return B200DRR_EUNSUPPORTED;
     return ret(launch_label_boxes(labels, mk(D0, D1, D2), boxes, (cudaStream_t)stream));
-}
-
-int b200drr_siddon_fwd_sens_structures(const float* vol, const uint8_t* labels, int D0, int D1, int D2, const float* src,
-                                       const float* G, const float* Wd, const float* rows, const float* cols,
-                                       const int32_t* slot_of_label, const int32_t* box, float* out, float* sens, int B, int S,
-                                       int H, int W, float voxel_shift, float eps, void* stream)
-{
-    if (!vol || !labels || !src || !G || !Wd || !rows || !cols || !slot_of_label || !box || !out || bad_dims(D0, D1, D2) ||
-        S <= 0 || S > 256 || B <= 0 || bad_rays((int)std::min<int64_t>((int64_t)B * S, INT32_MAX), (int64_t)H * W) || H <= 0 ||
-        W <= 0)
-        return B200DRR_EINVAL;
-    if (too_big(D0, D1, D2)) return B200DRR_EUNSUPPORTED;
-    return ret(launch_siddon_fwd_sens_structures(vol, labels, mk(D0, D1, D2), src, G, Wd, rows, cols, slot_of_label, box, out, sens,
-                                                 B, S, H, W, voxel_shift, eps, (cudaStream_t)stream));
 }
 
 int b200drr_siddon_bwd_sens(const float* sens, const float* gout, float* g_src, float* g_tgt, float* g_raylen, int B,
@@ -411,34 +270,10 @@ int b200drr_siddon_bwd_sens(const float* sens, const float* gout, float* g_src, 
 int b200drr_siddon_bwd_sens_pose(const float* sens, const float* gout, const float* Wd, const float* rows, const float* cols,
                                  float* g_src, float* g_G, float* g_Wd, int B, int H, int W, int stop_grad, void* stream)
 {
-    if (!sens || !gout || !Wd || !rows || !cols || !g_src || !g_G || !g_Wd || H <= 0 || W <= 0 ||
-        bad_rays(B, (int64_t)H * W))
+    if (!sens || !gout || !Wd || !rows || !cols || !g_src || !g_G || !g_Wd || bad_grid(B, H, W))
         return B200DRR_EINVAL;
     return ret(launch_siddon_bwd_sens_pose(sens, gout, Wd, rows, cols, g_src, g_G, g_Wd, B, H, W, stop_grad != 0,
                                            (cudaStream_t)stream));
-}
-
-int b200drr_trilinear_fwd_sens(const float* vol, int D0, int D1, int D2, const float* src, const float* tgt,
-                               const float* raylen, float* out, float* sens, int B, int64_t N, int H, int W,
-                               float voxel_shift, float eps, int n_points, const float* alpha_range, int align_corners,
-                               void* stream)
-{
-    if (!vol || !src || !tgt || !raylen || !out || !sens || !alpha_range || bad_dims(D0, D1, D2) || bad_rays(B, N) ||
-        n_points < 2 || H < 0 || W < 0 || (H > 0 && ((int64_t)H * W != N || align_corners)))
-        return B200DRR_EINVAL;
-    return ret(launch_trilinear_fwd_sens(vol, mk(D0, D1, D2), src, tgt, raylen, out, sens, B, N, H, W, voxel_shift, eps,
-                                         n_points, alpha_range, align_corners != 0, (cudaStream_t)stream));
-}
-
-int b200drr_trilinear_fwd_sens_packed(const float* packed, int D0, int D1, int D2, const float* src, const float* tgt,
-                                      const float* raylen, float* out, float* sens, int B, int H, int W, float voxel_shift,
-                                      float eps, int n_points, const float* alpha_range, int slab, void* stream)
-{
-    if (!packed || !src || !tgt || !raylen || !out || !sens || !alpha_range || bad_dims(D0, D1, D2) ||
-        bad_rays(B, (int64_t)H * W) || H <= 0 || W <= 0 || n_points < 2 || slab < 0)
-        return B200DRR_EINVAL;
-    return ret(launch_trilinear_fwd_sens_packed(packed, mk(D0, D1, D2), src, tgt, raylen, out, sens, B, H, W, voxel_shift, eps,
-                                                n_points, alpha_range, slab, (cudaStream_t)stream));
 }
 
 int b200drr_trilinear_bwd_sens(const float* sens, const float* gout, float* g_src, float* g_tgt, float* g_raylen,
@@ -453,27 +288,16 @@ int b200drr_trilinear_alpha_range_pose(int D0, int D1, int D2, const float* src,
                                        float voxel_shift, float eps, void* stream)
 {
     if (!src || !G || !Wd || !rows || !cols || !range || !arg || !scratch16 || bad_dims(D0, D1, D2) ||
-        bad_rays(B, (int64_t)H * W) || H <= 0 || W <= 0)
+        bad_grid(B, H, W))
         return B200DRR_EINVAL;
     return ret(launch_trilinear_alpha_range_pose(mk(D0, D1, D2), src, G, Wd, rows, cols, range, arg, scratch16, B, H, W, voxel_shift,
                                                  eps, (cudaStream_t)stream));
 }
 
-int b200drr_trilinear_fwd_sens_pose(const float* packed, int D0, int D1, int D2, const float* src, const float* G, const float* Wd,
-                                    const float* rows, const float* cols, float* out, float* sens, int B, int H, int W,
-                                    float voxel_shift, float eps, int n_points, const float* alpha_range, int slab, void* stream)
-{
-    if (!packed || !src || !G || !Wd || !rows || !cols || !out || !sens || !alpha_range || bad_dims(D0, D1, D2) ||
-        bad_rays(B, (int64_t)H * W) || H <= 0 || W <= 0 || n_points < 2 || slab < 0)
-        return B200DRR_EINVAL;
-    return ret(launch_trilinear_fwd_sens_pose(packed, mk(D0, D1, D2), src, G, Wd, rows, cols, out, sens, B, H, W, voxel_shift, eps,
-                                              n_points, alpha_range, slab, (cudaStream_t)stream));
-}
-
 int b200drr_trilinear_bwd_sens_pose(const float* sens, const float* gout, const float* Wd, const float* rows, const float* cols,
                                     float* g_src, float* g_G, float* g_Wd, float* g_alpha_range, int B, int H, int W, void* stream)
 {
-    if (!sens || !gout || !Wd || !rows || !cols || !g_src || !g_G || !g_Wd || bad_rays(B, (int64_t)H * W) || H <= 0 || W <= 0)
+    if (!sens || !gout || !Wd || !rows || !cols || !g_src || !g_G || !g_Wd || bad_grid(B, H, W))
         return B200DRR_EINVAL;
     return ret(launch_trilinear_bwd_sens_pose(sens, gout, Wd, rows, cols, g_src, g_G, g_Wd, g_alpha_range, B, H, W,
                                               (cudaStream_t)stream));
@@ -483,7 +307,7 @@ int b200drr_siddon_jac_sens_pose(const float* sens, const float* dsrc, const flo
                                  const float* rows, const float* cols, float* J, int B, int H, int W, int P, int stop_grad,
                                  void* stream)
 {
-    if (!sens || !dsrc || !dG || !dWd || !Wd || !rows || !cols || !J || H <= 0 || W <= 0 || bad_rays(B, (int64_t)H * W) || P < 1 ||
+    if (!sens || !dsrc || !dG || !dWd || !Wd || !rows || !cols || !J || bad_grid(B, H, W) || P < 1 ||
         P > 16)
         return B200DRR_EINVAL;
     return ret(launch_siddon_jac_sens_pose(sens, dsrc, dG, dWd, Wd, rows, cols, J, B, H, W, P, stop_grad != 0, (cudaStream_t)stream));
@@ -493,8 +317,7 @@ int b200drr_trilinear_jac_sens_pose(const float* sens, const float* dsrc, const 
                                     const float* rows, const float* cols, const float* drange, float* J, int B, int H, int W, int P,
                                     void* stream)
 {
-    if (!sens || !dsrc || !dG || !dWd || !Wd || !rows || !cols || !drange || !J || H <= 0 || W <= 0 ||
-        bad_rays(B, (int64_t)H * W) || P < 1 || P > 16)
+    if (!sens || !dsrc || !dG || !dWd || !Wd || !rows || !cols || !drange || !J || bad_grid(B, H, W) || P < 1 || P > 16)
         return B200DRR_EINVAL;
     return ret(launch_trilinear_jac_sens_pose(sens, dsrc, dG, dWd, Wd, rows, cols, drange, J, B, H, W, P, (cudaStream_t)stream));
 }
@@ -538,7 +361,7 @@ int b200drr_siddon_fwd_mask(const float* vol, const float* mask, int D0, int D1,
 {
     if (!vol || !mask || !src || !tgt || !raylen || !out || bad_dims(D0, D1, D2) || bad_rays(B, N) || C <= 0)
         return B200DRR_EINVAL;
-    if ((int64_t)D0 * D1 * D2 >= (int64_t)INT32_MAX) return B200DRR_EUNSUPPORTED;
+    if (too_big(D0, D1, D2)) return B200DRR_EUNSUPPORTED;
     return ret(launch_siddon_fwd_mask(vol, mask, mk(D0, D1, D2), src, tgt, raylen, out, B, N, C, voxel_shift, eps,
                                       (cudaStream_t)stream));
 }
@@ -559,10 +382,9 @@ int b200drr_siddon_fwd_mask_grid(const float* vol, const float* mask, int D0, in
                                  const float* raylen, float* out, int B, int H, int W, int C, float voxel_shift, float eps,
                                  void* stream)
 {
-    if (!vol || !mask || !src || !tgt || !raylen || !out || bad_dims(D0, D1, D2) || H <= 0 || W <= 0 ||
-        bad_rays(B, (int64_t)H * W) || C <= 0)
+    if (!vol || !mask || !src || !tgt || !raylen || !out || bad_dims(D0, D1, D2) || bad_grid(B, H, W) || C <= 0)
         return B200DRR_EINVAL;
-    if ((int64_t)D0 * D1 * D2 >= (int64_t)INT32_MAX) return B200DRR_EUNSUPPORTED;
+    if (too_big(D0, D1, D2)) return B200DRR_EUNSUPPORTED;
     return ret(launch_siddon_fwd_mask(vol, mask, mk(D0, D1, D2), src, tgt, raylen, out, B, (int64_t)H * W, C, voxel_shift, eps,
                                       (cudaStream_t)stream, W));
 }
@@ -572,8 +394,7 @@ int b200drr_trilinear_fwd_mask_grid(const float* vol, const float* mask, int D0,
                                     float voxel_shift, float eps, int n_points, const float* alpha_range, int align_corners,
                                     void* stream)
 {
-    if (!vol || !mask || !src || !tgt || !raylen || !out || !alpha_range || bad_dims(D0, D1, D2) || H <= 0 || W <= 0 ||
-        bad_rays(B, (int64_t)H * W) || C <= 0 || n_points < 2)
+    if (!vol || !mask || !src || !tgt || !raylen || !out || !alpha_range || bad_dims(D0, D1, D2) || bad_grid(B, H, W) || C <= 0 || n_points < 2)
         return B200DRR_EINVAL;
     return ret(launch_trilinear_fwd_mask(vol, mask, mk(D0, D1, D2), src, tgt, raylen, out, B, (int64_t)H * W, C, voxel_shift, eps,
                                          n_points, alpha_range, align_corners != 0, (cudaStream_t)stream, W));
@@ -620,8 +441,7 @@ int b200drr_siddon_bwd_mask_grid(const float* vol, const float* mask, int D0, in
                                  const float* raylen, const float* gout, float* g_src, float* g_tgt, float* g_raylen, float* g_vol,
                                  int B, int H, int W, int C, float voxel_shift, float eps, int stop_grad, void* stream)
 {
-    if (!vol || !mask || !src || !tgt || !raylen || !gout || bad_dims(D0, D1, D2) || H <= 0 || W <= 0 ||
-        bad_rays(B, (int64_t)H * W) || C <= 0)
+    if (!vol || !mask || !src || !tgt || !raylen || !gout || bad_dims(D0, D1, D2) || bad_grid(B, H, W) || C <= 0)
         return B200DRR_EINVAL;
     return ret(launch_siddon_bwd_mask(vol, mask, mk(D0, D1, D2), src, tgt, raylen, gout, g_src, g_tgt, g_raylen, g_vol, B,
                                       (int64_t)H * W, C, voxel_shift, eps, stop_grad != 0, (cudaStream_t)stream, W));
@@ -632,8 +452,7 @@ int b200drr_trilinear_bwd_mask_grid(const float* vol, const float* mask, int D0,
                                     float* g_vol, float* g_alpha_range, int B, int H, int W, int C, float voxel_shift, float eps,
                                     int n_points, const float* alpha_range, int align_corners, void* stream)
 {
-    if (!vol || !mask || !src || !tgt || !raylen || !gout || !alpha_range || bad_dims(D0, D1, D2) || H <= 0 || W <= 0 ||
-        bad_rays(B, (int64_t)H * W) || C <= 0 || n_points < 2)
+    if (!vol || !mask || !src || !tgt || !raylen || !gout || !alpha_range || bad_dims(D0, D1, D2) || bad_grid(B, H, W) || C <= 0 || n_points < 2)
         return B200DRR_EINVAL;
     return ret(launch_trilinear_bwd_mask(vol, mask, mk(D0, D1, D2), src, tgt, raylen, gout, g_src, g_tgt, g_raylen, g_vol,
                                          g_alpha_range, B, (int64_t)H * W, C, voxel_shift, eps, n_points, alpha_range,
@@ -664,85 +483,356 @@ int b200drr_trilinear_bwd_mask(const float* vol, const float* mask, int D0, int 
                                          (cudaStream_t)stream));
 }
 
-// ---- 16-bit volumes: twins of the Siddon forward entry points (include/b200drr.h, DESIGN.md 4.5) -------------------------------
+}  // extern "C"
+
+// ---- entry points with a 16-bit twin (include/b200drr.h, DESIGN.md 4.5) -----------------------------------------------------------
+// One body per fp32 entry point and its `_v16` twin, on the voxel type V: float for the fp32 entry point, VoxF16 / VoxBF16 for the
+// twin, which reaches it through with_vox16.  The twins have no tuning variants, and the plain Siddon / Trilinear forward twins
+// take only reduce = 0 and align_corners = 0.
+namespace {
+template <class V>
+constexpr bool kF32 = std::is_same<V, float>::value;
+
+template <class V>
+int siddon_fwd(const void* vol, int D0, int D1, int D2, const float* src, const float* tgt, const float* raylen, float* out, int B,
+               int64_t N, float voxel_shift, float eps, int reduce, int align_corners, void* stream)
+{
+    const bool bad_options = kF32<V> ? reduce < 0 || reduce > 1 : reduce != 0 || align_corners != 0;
+    if (!vol || !src || !tgt || !raylen || !out || bad_dims(D0, D1, D2) || bad_rays(B, N) || bad_options) return B200DRR_EINVAL;
+    if constexpr (kF32<V>)
+        return ret(launch_siddon_fwd((const V*)vol, mk(D0, D1, D2), src, tgt, raylen, out, B, N, voxel_shift, eps, reduce,
+                                     align_corners != 0, (cudaStream_t)stream));
+    else
+        return ret(launch_siddon_fwd_fast((const V*)vol, mk(D0, D1, D2), src, tgt, raylen, out, B, N, voxel_shift, eps,
+                                          (cudaStream_t)stream));
+}
+
+template <class V>
+int siddon_fwd_sens(const void* vol, int D0, int D1, int D2, const float* src, const float* tgt, const float* raylen, float* out,
+                    float* sens, int B, int64_t N, float voxel_shift, float eps, void* stream)
+{
+    if (!vol || !src || !tgt || !raylen || !out || !sens || bad_dims(D0, D1, D2) || bad_rays(B, N)) return B200DRR_EINVAL;
+    if (too_big(D0, D1, D2)) return B200DRR_EUNSUPPORTED;
+    return ret(launch_siddon_fwd_sens((const V*)vol, mk(D0, D1, D2), src, tgt, raylen, out, sens, B, N, voxel_shift, eps,
+                                      (cudaStream_t)stream));
+}
+
+template <class V>
+int siddon_fwd_sorted(const void* vol, int D0, int D1, int D2, const float* src, const float* tgt, const float* raylen, float* out,
+                      int B, int64_t N, float voxel_shift, float eps, void* stream)
+{
+    if (!vol || !src || !tgt || !raylen || !out || bad_dims(D0, D1, D2) || bad_rays(B, N)) return B200DRR_EINVAL;
+    if (too_big(D0, D1, D2)) return B200DRR_EUNSUPPORTED;
+    return ret(launch_siddon_fwd_sorted((const V*)vol, mk(D0, D1, D2), src, tgt, raylen, out, B, N, voxel_shift, eps,
+                                        (cudaStream_t)stream));
+}
+
+template <class V>
+int siddon_fwd_sens_sorted(const void* vol, int D0, int D1, int D2, const float* src, const float* tgt, const float* raylen,
+                           float* out, float* sens, int B, int64_t N, float voxel_shift, float eps, void* stream)
+{
+    if (!vol || !src || !tgt || !raylen || !out || !sens || bad_dims(D0, D1, D2) || bad_rays(B, N)) return B200DRR_EINVAL;
+    if (too_big(D0, D1, D2)) return B200DRR_EUNSUPPORTED;
+    return ret(launch_siddon_fwd_sens_sorted((const V*)vol, mk(D0, D1, D2), src, tgt, raylen, out, sens, B, N, voxel_shift, eps,
+                                             (cudaStream_t)stream));
+}
+
+template <class V>
+int siddon_fwd_grid(const void* vol, int D0, int D1, int D2, const float* src, const float* tgt, const float* raylen, float* out,
+                    int B, int H, int W, float voxel_shift, float eps, int variant, void* stream)
+{
+    if (!vol || !src || !tgt || !raylen || !out || bad_dims(D0, D1, D2) || bad_grid(B, H, W)) return B200DRR_EINVAL;
+    if constexpr (kF32<V>) {
+        return ret(launch_siddon_fwd_grid((const V*)vol, mk(D0, D1, D2), src, tgt, raylen, out, B, H, W, voxel_shift, eps, variant,
+                                          (cudaStream_t)stream));
+    } else {
+        if (variant != 0) return B200DRR_EUNSUPPORTED;
+        return ret(launch_siddon_fwd_grid_default((const V*)vol, mk(D0, D1, D2), src, tgt, raylen, out, B, H, W, voxel_shift, eps,
+                                                  (cudaStream_t)stream));
+    }
+}
+
+template <class V>
+int siddon_fwd_sens_grid(const void* vol, int D0, int D1, int D2, const float* src, const float* tgt, const float* raylen,
+                         float* out, float* sens, int B, int H, int W, float voxel_shift, float eps, int variant, void* stream)
+{
+    if (!vol || !src || !tgt || !raylen || !out || !sens || bad_dims(D0, D1, D2) || bad_grid(B, H, W)) return B200DRR_EINVAL;
+    if (too_big(D0, D1, D2) || (!kF32<V> && variant != 0)) return B200DRR_EUNSUPPORTED;
+    if constexpr (kF32<V>)
+        return ret(launch_siddon_fwd_sens_grid((const V*)vol, mk(D0, D1, D2), src, tgt, raylen, out, sens, B, H, W, voxel_shift, eps,
+                                               variant, (cudaStream_t)stream));
+    else
+        return ret(launch_siddon_fwd_sens_grid_default((const V*)vol, mk(D0, D1, D2), src, tgt, raylen, out, sens, B, H, W,
+                                                       voxel_shift, eps, (cudaStream_t)stream));
+}
+
+template <class V>
+int siddon_fwd_brick(const void* vol, int D0, int D1, int D2, const float* src, const float* tgt, const float* raylen, const float* G,
+                     const float* Wd, const float* rows, const float* cols, float* out, void* workspace, int64_t workspace_bytes, int B,
+                     int H, int W, float voxel_shift, float eps, int variant, void* stream)
+{
+    const bool pose_in = G != nullptr;
+    if (!vol || !src || !out || !workspace || bad_dims(D0, D1, D2) || bad_grid(B, H, W)) return B200DRR_EINVAL;
+    if (pose_in ? (!Wd || !rows || !cols) : (!tgt || !raylen)) return B200DRR_EINVAL;
+    if (!kF32<V> && variant != 0) return B200DRR_EUNSUPPORTED;
+    if (const int bad =
+            brick_bad(vol, mk(D0, D1, D2), H, W, sizeof(V), workspace, workspace_bytes, siddon_brick_workspace_bytes(B, H, W)))
+        return bad;
+    return ret(launch_siddon_fwd_brick((const V*)vol, mk(D0, D1, D2), src, tgt, raylen, G, Wd, rows, cols, out, workspace,
+                                       (size_t)workspace_bytes, B, H, W, voxel_shift, eps, variant, (cudaStream_t)stream));
+}
+
+template <class V>
+int siddon_fwd_brick_subset(const void* vol, int D0, int D1, int D2, const float* src, const float* tgt, const float* raylen,
+                            const int32_t* pix_index, const float* corners, float* out, void* workspace, int64_t workspace_bytes, int B,
+                            int H, int W, int64_t Nsub, float voxel_shift, float eps, int variant, void* stream)
+{
+    if (!vol || !src || !tgt || !raylen || !pix_index || !corners || !out || !workspace || bad_dims(D0, D1, D2) ||
+        bad_rays(B, Nsub) || H <= 0 || W <= 0 || Nsub > (int64_t)H * W)
+        return B200DRR_EINVAL;
+    if (!kF32<V> && variant != 0) return B200DRR_EUNSUPPORTED;
+    if (const int bad = brick_bad(vol, mk(D0, D1, D2), H, W, sizeof(V), workspace, workspace_bytes,
+                                  siddon_brick_workspace_bytes(B, 1, (int)Nsub)))
+        return bad;
+    return ret(launch_siddon_fwd_brick((const V*)vol, mk(D0, D1, D2), src, tgt, raylen, nullptr, nullptr, nullptr, nullptr, out,
+                                       workspace, (size_t)workspace_bytes, B, H, W, voxel_shift, eps, variant, (cudaStream_t)stream,
+                                       pix_index, corners, Nsub));
+}
+
+template <class V>
+int siddon_fwd_pose(const void* vol, int D0, int D1, int D2, const float* src, const float* G, const float* Wd, const float* rows,
+                    const float* cols, float* out, int B, int H, int W, float voxel_shift, float eps, void* stream)
+{
+    if (!vol || !src || !G || !Wd || !rows || !cols || !out || bad_dims(D0, D1, D2) || bad_grid(B, H, W)) return B200DRR_EINVAL;
+    if (too_big(D0, D1, D2)) return B200DRR_EUNSUPPORTED;
+    return ret(launch_siddon_fwd_pose((const V*)vol, mk(D0, D1, D2), src, G, Wd, rows, cols, out, B, H, W, voxel_shift, eps,
+                                      (cudaStream_t)stream));
+}
+
+template <class V>
+int siddon_fwd_sens_pose(const void* vol, int D0, int D1, int D2, const float* src, const float* G, const float* Wd,
+                         const float* rows, const float* cols, float* out, float* sens, int B, int H, int W, float voxel_shift,
+                         float eps, void* stream)
+{
+    if (!vol || !src || !G || !Wd || !rows || !cols || !out || !sens || bad_dims(D0, D1, D2) || bad_grid(B, H, W))
+        return B200DRR_EINVAL;
+    if (too_big(D0, D1, D2)) return B200DRR_EUNSUPPORTED;
+    return ret(launch_siddon_fwd_sens_pose((const V*)vol, mk(D0, D1, D2), src, G, Wd, rows, cols, out, sens, B, H, W, voxel_shift,
+                                           eps, (cudaStream_t)stream));
+}
+
+template <class V>
+int siddon_fwd_sens_structures(const void* vol, const uint8_t* labels, int D0, int D1, int D2, const float* src, const float* G,
+                               const float* Wd, const float* rows, const float* cols, const int32_t* slot_of_label,
+                               const int32_t* box, float* out, float* sens, int B, int S, int H, int W, float voxel_shift,
+                               float eps, void* stream)
+{
+    if (!vol || !labels || !src || !G || !Wd || !rows || !cols || !slot_of_label || !box || !out || bad_dims(D0, D1, D2) ||
+        S <= 0 || S > 256 || B <= 0 || bad_rays((int)std::min<int64_t>((int64_t)B * S, INT32_MAX), (int64_t)H * W) || H <= 0 ||
+        W <= 0)
+        return B200DRR_EINVAL;
+    if (too_big(D0, D1, D2)) return B200DRR_EUNSUPPORTED;
+    return ret(launch_siddon_fwd_sens_structures((const V*)vol, labels, mk(D0, D1, D2), src, G, Wd, rows, cols, slot_of_label, box,
+                                                 out, sens, B, S, H, W, voxel_shift, eps, (cudaStream_t)stream));
+}
+
+template <class V>
+int pack_corners(const void* vol, int D0, int D1, int D2, void* packed, void* stream)
+{
+    if (!vol || !packed || bad_dims(D0, D1, D2) || (!kF32<V> && ((uintptr_t)packed & 15u) != 0)) return B200DRR_EINVAL;
+    if constexpr (kF32<V>)
+        return ret(launch_pack_corners((const V*)vol, mk(D0, D1, D2), (float*)packed, (cudaStream_t)stream));
+    else
+        return ret(launch_pack_corners16((const V*)vol, mk(D0, D1, D2), (Cell16<V>*)packed, (cudaStream_t)stream));
+}
+
+template <class V>
+int trilinear_fwd(const void* vol, int D0, int D1, int D2, const float* src, const float* tgt, const float* raylen, float* out,
+                  int B, int64_t N, float voxel_shift, float eps, int n_points, const float* alpha_range, int reduce,
+                  int align_corners, void* stream)
+{
+    const bool bad_options = kF32<V> ? reduce < 0 || reduce > 1 : reduce != 0 || align_corners != 0;
+    if (!vol || !src || !tgt || !raylen || !out || !alpha_range || bad_dims(D0, D1, D2) || bad_rays(B, N) || n_points < 2 ||
+        bad_options)
+        return B200DRR_EINVAL;
+    return ret(launch_trilinear_fwd((const V*)vol, mk(D0, D1, D2), src, tgt, raylen, out, B, N, voxel_shift, eps, n_points,
+                                    alpha_range, reduce, align_corners != 0, (cudaStream_t)stream));
+}
+
+template <class V>
+int trilinear_fwd_grid(const void* vol, int D0, int D1, int D2, const float* src, const float* tgt, const float* raylen, float* out,
+                       int B, int H, int W, float voxel_shift, float eps, int n_points, const float* alpha_range, int variant,
+                       void* stream)
+{
+    if (!vol || !src || !tgt || !raylen || !out || !alpha_range || bad_dims(D0, D1, D2) || bad_grid(B, H, W) || n_points < 2)
+        return B200DRR_EINVAL;
+    return ret(launch_trilinear_fwd_grid((const V*)vol, mk(D0, D1, D2), src, tgt, raylen, out, B, H, W, voxel_shift, eps, n_points,
+                                         alpha_range, variant, (cudaStream_t)stream));
+}
+
+template <class V>
+int trilinear_fwd_sens(const void* vol, int D0, int D1, int D2, const float* src, const float* tgt, const float* raylen, float* out,
+                       float* sens, int B, int64_t N, int H, int W, float voxel_shift, float eps, int n_points,
+                       const float* alpha_range, int align_corners, void* stream)
+{
+    if (!vol || !src || !tgt || !raylen || !out || !sens || !alpha_range || bad_dims(D0, D1, D2) || bad_rays(B, N) ||
+        n_points < 2 || H < 0 || W < 0 || (H > 0 && ((int64_t)H * W != N || align_corners)) || (!kF32<V> && align_corners != 0))
+        return B200DRR_EINVAL;
+    return ret(launch_trilinear_fwd_sens((const V*)vol, mk(D0, D1, D2), src, tgt, raylen, out, sens, B, N, H, W, voxel_shift, eps,
+                                         n_points, alpha_range, align_corners != 0, (cudaStream_t)stream));
+}
+
+// the packed copy of a 16-bit volume holds cells of its own type (Cell16<V>)
+template <class V>
+int trilinear_fwd_packed(const void* packed, int D0, int D1, int D2, const float* src, const float* tgt, const float* raylen,
+                         float* out, int B, int H, int W, float voxel_shift, float eps, int n_points, const float* alpha_range,
+                         int slab, void* stream)
+{
+    if (!packed || slab < 0 || !src || !tgt || !raylen || !out || !alpha_range || bad_dims(D0, D1, D2) || bad_grid(B, H, W) ||
+        n_points < 2)
+        return B200DRR_EINVAL;
+    if constexpr (kF32<V>)
+        return ret(launch_trilinear_fwd_packed((const float*)packed, mk(D0, D1, D2), src, tgt, raylen, out, B, H, W, voxel_shift, eps,
+                                               n_points, alpha_range, slab, (cudaStream_t)stream));
+    else
+        return ret(launch_trilinear_fwd_packed_t((const Cell16<V>*)packed, mk(D0, D1, D2), src, tgt, raylen, out, B, H, W,
+                                                 voxel_shift, eps, n_points, alpha_range, slab, (cudaStream_t)stream));
+}
+
+template <class V>
+int trilinear_fwd_sens_packed(const void* packed, int D0, int D1, int D2, const float* src, const float* tgt, const float* raylen,
+                              float* out, float* sens, int B, int H, int W, float voxel_shift, float eps, int n_points,
+                              const float* alpha_range, int slab, void* stream)
+{
+    if (!packed || !src || !tgt || !raylen || !out || !sens || !alpha_range || bad_dims(D0, D1, D2) || bad_grid(B, H, W) ||
+        n_points < 2 || slab < 0)
+        return B200DRR_EINVAL;
+    if constexpr (kF32<V>)
+        return ret(launch_trilinear_fwd_sens_packed((const float*)packed, mk(D0, D1, D2), src, tgt, raylen, out, sens, B, H, W,
+                                                    voxel_shift, eps, n_points, alpha_range, slab, (cudaStream_t)stream));
+    else
+        return ret(launch_trilinear_fwd_sens_packed16((const Cell16<V>*)packed, mk(D0, D1, D2), src, tgt, raylen, nullptr, nullptr,
+                                                      nullptr, nullptr, out, sens, B, H, W, voxel_shift, eps, n_points, alpha_range,
+                                                      slab, (cudaStream_t)stream));
+}
+
+template <class V>
+int trilinear_fwd_sens_pose(const void* packed, int D0, int D1, int D2, const float* src, const float* G, const float* Wd,
+                            const float* rows, const float* cols, float* out, float* sens, int B, int H, int W, float voxel_shift,
+                            float eps, int n_points, const float* alpha_range, int slab, void* stream)
+{
+    if (!packed || !src || !G || !Wd || !rows || !cols || !out || !sens || !alpha_range || bad_dims(D0, D1, D2) ||
+        bad_grid(B, H, W) || n_points < 2 || slab < 0)
+        return B200DRR_EINVAL;
+    if constexpr (kF32<V>)
+        return ret(launch_trilinear_fwd_sens_pose((const float*)packed, mk(D0, D1, D2), src, G, Wd, rows, cols, out, sens, B, H, W,
+                                                  voxel_shift, eps, n_points, alpha_range, slab, (cudaStream_t)stream));
+    else
+        return ret(launch_trilinear_fwd_sens_packed16((const Cell16<V>*)packed, mk(D0, D1, D2), src, nullptr, nullptr, G, Wd, rows,
+                                                      cols, out, sens, B, H, W, voxel_shift, eps, n_points, alpha_range, slab,
+                                                      (cudaStream_t)stream));
+}
+}  // namespace
+
+extern "C" {
+
+int b200drr_siddon_fwd(const float* vol, int D0, int D1, int D2, const float* src, const float* tgt, const float* raylen, float* out,
+                       int B, int64_t N, float voxel_shift, float eps, int reduce, int align_corners, void* stream)
+{
+    return siddon_fwd<float>(vol, D0, D1, D2, src, tgt, raylen, out, B, N, voxel_shift, eps, reduce, align_corners, stream);
+}
+
 int b200drr_siddon_fwd_v16(const void* vol, int vol_type, int D0, int D1, int D2, const float* src, const float* tgt,
                            const float* raylen, float* out, int B, int64_t N, float voxel_shift, float eps, int reduce,
                            int align_corners, void* stream)
 {
-    if (!vol || !src || !tgt || !raylen || !out || bad_dims(D0, D1, D2) || bad_rays(B, N) || reduce != 0 || align_corners != 0)
-        return B200DRR_EINVAL;
     return with_vox16(vol_type, [&](auto v) {
-        using V = decltype(v);
-        return ret(launch_siddon_fwd_fast((const V*)vol, mk(D0, D1, D2), src, tgt, raylen, out, B, N, voxel_shift, eps,
-                                          (cudaStream_t)stream));
+        return siddon_fwd<decltype(v)>(vol, D0, D1, D2, src, tgt, raylen, out, B, N, voxel_shift, eps, reduce, align_corners, stream);
     });
+}
+
+int b200drr_siddon_fwd_sens(const float* vol, int D0, int D1, int D2, const float* src, const float* tgt, const float* raylen,
+                            float* out, float* sens, int B, int64_t N, float voxel_shift, float eps, void* stream)
+{
+    return siddon_fwd_sens<float>(vol, D0, D1, D2, src, tgt, raylen, out, sens, B, N, voxel_shift, eps, stream);
 }
 
 int b200drr_siddon_fwd_sens_v16(const void* vol, int vol_type, int D0, int D1, int D2, const float* src, const float* tgt,
                                 const float* raylen, float* out, float* sens, int B, int64_t N, float voxel_shift, float eps,
                                 void* stream)
 {
-    if (!vol || !src || !tgt || !raylen || !out || !sens || bad_dims(D0, D1, D2) || bad_rays(B, N)) return B200DRR_EINVAL;
     return with_vox16(vol_type, [&](auto v) {
-        using V = decltype(v);
-        if (too_big(D0, D1, D2)) return (int)B200DRR_EUNSUPPORTED;
-        return ret(launch_siddon_fwd_sens((const V*)vol, mk(D0, D1, D2), src, tgt, raylen, out, sens, B, N, voxel_shift, eps,
-                                          (cudaStream_t)stream));
+        return siddon_fwd_sens<decltype(v)>(vol, D0, D1, D2, src, tgt, raylen, out, sens, B, N, voxel_shift, eps, stream);
     });
+}
+
+int b200drr_siddon_fwd_sorted(const float* vol, int D0, int D1, int D2, const float* src, const float* tgt, const float* raylen,
+                              float* out, int B, int64_t N, float voxel_shift, float eps, void* stream)
+{
+    return siddon_fwd_sorted<float>(vol, D0, D1, D2, src, tgt, raylen, out, B, N, voxel_shift, eps, stream);
 }
 
 int b200drr_siddon_fwd_sorted_v16(const void* vol, int vol_type, int D0, int D1, int D2, const float* src, const float* tgt,
                                   const float* raylen, float* out, int B, int64_t N, float voxel_shift, float eps, void* stream)
 {
-    if (!vol || !src || !tgt || !raylen || !out || bad_dims(D0, D1, D2) || bad_rays(B, N)) return B200DRR_EINVAL;
     return with_vox16(vol_type, [&](auto v) {
-        using V = decltype(v);
-        if (too_big(D0, D1, D2)) return (int)B200DRR_EUNSUPPORTED;
-        return ret(launch_siddon_fwd_sorted((const V*)vol, mk(D0, D1, D2), src, tgt, raylen, out, B, N, voxel_shift, eps,
-                                            (cudaStream_t)stream));
+        return siddon_fwd_sorted<decltype(v)>(vol, D0, D1, D2, src, tgt, raylen, out, B, N, voxel_shift, eps, stream);
     });
+}
+
+int b200drr_siddon_fwd_sens_sorted(const float* vol, int D0, int D1, int D2, const float* src, const float* tgt,
+                                   const float* raylen, float* out, float* sens, int B, int64_t N, float voxel_shift, float eps,
+                                   void* stream)
+{
+    return siddon_fwd_sens_sorted<float>(vol, D0, D1, D2, src, tgt, raylen, out, sens, B, N, voxel_shift, eps, stream);
 }
 
 int b200drr_siddon_fwd_sens_sorted_v16(const void* vol, int vol_type, int D0, int D1, int D2, const float* src, const float* tgt,
                                        const float* raylen, float* out, float* sens, int B, int64_t N, float voxel_shift, float eps,
                                        void* stream)
 {
-    if (!vol || !src || !tgt || !raylen || !out || !sens || bad_dims(D0, D1, D2) || bad_rays(B, N)) return B200DRR_EINVAL;
     return with_vox16(vol_type, [&](auto v) {
-        using V = decltype(v);
-        if (too_big(D0, D1, D2)) return (int)B200DRR_EUNSUPPORTED;
-        return ret(launch_siddon_fwd_sens_sorted((const V*)vol, mk(D0, D1, D2), src, tgt, raylen, out, sens, B, N, voxel_shift, eps,
-                                                 (cudaStream_t)stream));
+        return siddon_fwd_sens_sorted<decltype(v)>(vol, D0, D1, D2, src, tgt, raylen, out, sens, B, N, voxel_shift, eps, stream);
     });
+}
+
+int b200drr_siddon_fwd_grid(const float* vol, int D0, int D1, int D2, const float* src, const float* tgt, const float* raylen,
+                            float* out, int B, int H, int W, float voxel_shift, float eps, int variant, void* stream)
+{
+    return siddon_fwd_grid<float>(vol, D0, D1, D2, src, tgt, raylen, out, B, H, W, voxel_shift, eps, variant, stream);
 }
 
 int b200drr_siddon_fwd_grid_v16(const void* vol, int vol_type, int D0, int D1, int D2, const float* src, const float* tgt,
                                 const float* raylen, float* out, int B, int H, int W, float voxel_shift, float eps, int variant,
                                 void* stream)
 {
-    if (!vol || !src || !tgt || !raylen || !out || bad_dims(D0, D1, D2) || bad_rays(B, (int64_t)H * W) || H <= 0 || W <= 0)
-        return B200DRR_EINVAL;
     return with_vox16(vol_type, [&](auto v) {
-        using V = decltype(v);
-        if (variant != 0) return (int)B200DRR_EUNSUPPORTED;  // the tuning variants are fp32-only
-        return ret(launch_siddon_fwd_grid_default((const V*)vol, mk(D0, D1, D2), src, tgt, raylen, out, B, H, W, voxel_shift, eps,
-                                                  (cudaStream_t)stream));
+        return siddon_fwd_grid<decltype(v)>(vol, D0, D1, D2, src, tgt, raylen, out, B, H, W, voxel_shift, eps, variant, stream);
     });
+}
+
+int b200drr_siddon_fwd_sens_grid(const float* vol, int D0, int D1, int D2, const float* src, const float* tgt, const float* raylen,
+                                 float* out, float* sens, int B, int H, int W, float voxel_shift, float eps, int variant, void* stream)
+{
+    return siddon_fwd_sens_grid<float>(vol, D0, D1, D2, src, tgt, raylen, out, sens, B, H, W, voxel_shift, eps, variant, stream);
 }
 
 int b200drr_siddon_fwd_sens_grid_v16(const void* vol, int vol_type, int D0, int D1, int D2, const float* src, const float* tgt,
                                      const float* raylen, float* out, float* sens, int B, int H, int W, float voxel_shift, float eps,
                                      int variant, void* stream)
 {
-    if (!vol || !src || !tgt || !raylen || !out || !sens || bad_dims(D0, D1, D2) || bad_rays(B, (int64_t)H * W) || H <= 0 ||
-        W <= 0)
-        return B200DRR_EINVAL;
     return with_vox16(vol_type, [&](auto v) {
-        using V = decltype(v);
-        if (variant != 0 || too_big(D0, D1, D2)) return (int)B200DRR_EUNSUPPORTED;
-        return ret(launch_siddon_fwd_sens_grid_default((const V*)vol, mk(D0, D1, D2), src, tgt, raylen, out, sens, B, H, W,
-                                                       voxel_shift, eps, (cudaStream_t)stream));
+        return siddon_fwd_sens_grid<decltype(v)>(vol, D0, D1, D2, src, tgt, raylen, out, sens, B, H, W, voxel_shift, eps, variant,
+                                                 stream);
     });
+}
+
+int b200drr_siddon_fwd_brick(const float* vol, int D0, int D1, int D2, const float* src, const float* tgt, const float* raylen,
+                             const float* G, const float* Wd, const float* rows, const float* cols, float* out, void* workspace,
+                             int64_t workspace_bytes, int B, int H, int W, float voxel_shift, float eps, int variant, void* stream)
+{
+    return siddon_fwd_brick<float>(vol, D0, D1, D2, src, tgt, raylen, G, Wd, rows, cols, out, workspace, workspace_bytes, B, H, W,
+                                   voxel_shift, eps, variant, stream);
 }
 
 int b200drr_siddon_fwd_brick_v16(const void* vol, int vol_type, int D0, int D1, int D2, const float* src, const float* tgt,
@@ -750,19 +840,19 @@ int b200drr_siddon_fwd_brick_v16(const void* vol, int vol_type, int D0, int D1, 
                                  float* out, void* workspace, int64_t workspace_bytes, int B, int H, int W, float voxel_shift,
                                  float eps, int variant, void* stream)
 {
-    const bool pose_in = G != nullptr;
-    if (!vol || !src || !out || !workspace || bad_dims(D0, D1, D2) || bad_rays(B, (int64_t)H * W) || H <= 0 || W <= 0)
-        return B200DRR_EINVAL;
-    if (pose_in ? (!Wd || !rows || !cols) : (!tgt || !raylen)) return B200DRR_EINVAL;
     return with_vox16(vol_type, [&](auto v) {
-        using V = decltype(v);
-        if (variant != 0) return (int)B200DRR_EUNSUPPORTED;  // the tuning variants are fp32-only
-        if (!siddon_brick_supported(mk(D0, D1, D2), H, W, 2) || ((uintptr_t)vol & 15u) != 0) return (int)B200DRR_EUNSUPPORTED;
-        if (workspace_bytes < (int64_t)siddon_brick_workspace_bytes(B, H, W) || ((uintptr_t)workspace & 255u) != 0)
-            return (int)B200DRR_EINVAL;
-        return ret(launch_siddon_fwd_brick((const V*)vol, mk(D0, D1, D2), src, tgt, raylen, G, Wd, rows, cols, out, workspace,
-                                           (size_t)workspace_bytes, B, H, W, voxel_shift, eps, variant, (cudaStream_t)stream));
+        return siddon_fwd_brick<decltype(v)>(vol, D0, D1, D2, src, tgt, raylen, G, Wd, rows, cols, out, workspace, workspace_bytes, B,
+                                             H, W, voxel_shift, eps, variant, stream);
     });
+}
+
+int b200drr_siddon_fwd_brick_subset(const float* vol, int D0, int D1, int D2, const float* src, const float* tgt,
+                                    const float* raylen, const int32_t* pix_index, const float* corners, float* out,
+                                    void* workspace, int64_t workspace_bytes, int B, int H, int W, int64_t Nsub,
+                                    float voxel_shift, float eps, int variant, void* stream)
+{
+    return siddon_fwd_brick_subset<float>(vol, D0, D1, D2, src, tgt, raylen, pix_index, corners, out, workspace, workspace_bytes, B,
+                                          H, W, Nsub, voxel_shift, eps, variant, stream);
 }
 
 int b200drr_siddon_fwd_brick_subset_v16(const void* vol, int vol_type, int D0, int D1, int D2, const float* src, const float* tgt,
@@ -770,49 +860,52 @@ int b200drr_siddon_fwd_brick_subset_v16(const void* vol, int vol_type, int D0, i
                                         void* workspace, int64_t workspace_bytes, int B, int H, int W, int64_t Nsub,
                                         float voxel_shift, float eps, int variant, void* stream)
 {
-    if (!vol || !src || !tgt || !raylen || !pix_index || !corners || !out || !workspace || bad_dims(D0, D1, D2) ||
-        bad_rays(B, Nsub) || H <= 0 || W <= 0 || Nsub > (int64_t)H * W)
-        return B200DRR_EINVAL;
     return with_vox16(vol_type, [&](auto v) {
-        using V = decltype(v);
-        if (variant != 0) return (int)B200DRR_EUNSUPPORTED;  // the tuning variants are fp32-only
-        if (!siddon_brick_supported(mk(D0, D1, D2), H, W, 2) || ((uintptr_t)vol & 15u) != 0) return (int)B200DRR_EUNSUPPORTED;
-        if (workspace_bytes < (int64_t)siddon_brick_workspace_bytes(B, 1, (int)Nsub) || ((uintptr_t)workspace & 255u) != 0)
-            return (int)B200DRR_EINVAL;
-        return ret(launch_siddon_fwd_brick((const V*)vol, mk(D0, D1, D2), src, tgt, raylen, nullptr, nullptr, nullptr, nullptr, out,
-                                           workspace, (size_t)workspace_bytes, B, H, W, voxel_shift, eps, variant,
-                                           (cudaStream_t)stream, pix_index, corners, Nsub));
+        return siddon_fwd_brick_subset<decltype(v)>(vol, D0, D1, D2, src, tgt, raylen, pix_index, corners, out, workspace,
+                                                    workspace_bytes, B, H, W, Nsub, voxel_shift, eps, variant, stream);
     });
+}
+
+int b200drr_siddon_fwd_pose(const float* vol, int D0, int D1, int D2, const float* src, const float* G, const float* Wd,
+                            const float* rows, const float* cols, float* out, int B, int H, int W, float voxel_shift,
+                            float eps, void* stream)
+{
+    return siddon_fwd_pose<float>(vol, D0, D1, D2, src, G, Wd, rows, cols, out, B, H, W, voxel_shift, eps, stream);
 }
 
 int b200drr_siddon_fwd_pose_v16(const void* vol, int vol_type, int D0, int D1, int D2, const float* src, const float* G,
                                 const float* Wd, const float* rows, const float* cols, float* out, int B, int H, int W,
                                 float voxel_shift, float eps, void* stream)
 {
-    if (!vol || !src || !G || !Wd || !rows || !cols || !out || bad_dims(D0, D1, D2) || bad_rays(B, (int64_t)H * W) || H <= 0 ||
-        W <= 0)
-        return B200DRR_EINVAL;
     return with_vox16(vol_type, [&](auto v) {
-        using V = decltype(v);
-        if (too_big(D0, D1, D2)) return (int)B200DRR_EUNSUPPORTED;
-        return ret(launch_siddon_fwd_pose((const V*)vol, mk(D0, D1, D2), src, G, Wd, rows, cols, out, B, H, W, voxel_shift, eps,
-                                          (cudaStream_t)stream));
+        return siddon_fwd_pose<decltype(v)>(vol, D0, D1, D2, src, G, Wd, rows, cols, out, B, H, W, voxel_shift, eps, stream);
     });
+}
+
+int b200drr_siddon_fwd_sens_pose(const float* vol, int D0, int D1, int D2, const float* src, const float* G, const float* Wd,
+                                 const float* rows, const float* cols, float* out, float* sens, int B, int H, int W,
+                                 float voxel_shift, float eps, void* stream)
+{
+    return siddon_fwd_sens_pose<float>(vol, D0, D1, D2, src, G, Wd, rows, cols, out, sens, B, H, W, voxel_shift, eps, stream);
 }
 
 int b200drr_siddon_fwd_sens_pose_v16(const void* vol, int vol_type, int D0, int D1, int D2, const float* src, const float* G,
                                      const float* Wd, const float* rows, const float* cols, float* out, float* sens, int B, int H,
                                      int W, float voxel_shift, float eps, void* stream)
 {
-    if (!vol || !src || !G || !Wd || !rows || !cols || !out || !sens || bad_dims(D0, D1, D2) || bad_rays(B, (int64_t)H * W) ||
-        H <= 0 || W <= 0)
-        return B200DRR_EINVAL;
     return with_vox16(vol_type, [&](auto v) {
-        using V = decltype(v);
-        if (too_big(D0, D1, D2)) return (int)B200DRR_EUNSUPPORTED;
-        return ret(launch_siddon_fwd_sens_pose((const V*)vol, mk(D0, D1, D2), src, G, Wd, rows, cols, out, sens, B, H, W,
-                                               voxel_shift, eps, (cudaStream_t)stream));
+        return siddon_fwd_sens_pose<decltype(v)>(vol, D0, D1, D2, src, G, Wd, rows, cols, out, sens, B, H, W, voxel_shift, eps,
+                                                 stream);
     });
+}
+
+int b200drr_siddon_fwd_sens_structures(const float* vol, const uint8_t* labels, int D0, int D1, int D2, const float* src,
+                                       const float* G, const float* Wd, const float* rows, const float* cols,
+                                       const int32_t* slot_of_label, const int32_t* box, float* out, float* sens, int B, int S,
+                                       int H, int W, float voxel_shift, float eps, void* stream)
+{
+    return siddon_fwd_sens_structures<float>(vol, labels, D0, D1, D2, src, G, Wd, rows, cols, slot_of_label, box, out, sens, B, S, H,
+                                             W, voxel_shift, eps, stream);
 }
 
 int b200drr_siddon_fwd_sens_structures_v16(const void* vol, int vol_type, const uint8_t* labels, int D0, int D1, int D2,
@@ -820,83 +913,100 @@ int b200drr_siddon_fwd_sens_structures_v16(const void* vol, int vol_type, const 
                                            const int32_t* slot_of_label, const int32_t* box, float* out, float* sens, int B,
                                            int S, int H, int W, float voxel_shift, float eps, void* stream)
 {
-    if (!vol || !labels || !src || !G || !Wd || !rows || !cols || !slot_of_label || !box || !out || bad_dims(D0, D1, D2) ||
-        S <= 0 || S > 256 || B <= 0 || bad_rays((int)std::min<int64_t>((int64_t)B * S, INT32_MAX), (int64_t)H * W) || H <= 0 ||
-        W <= 0)
-        return B200DRR_EINVAL;
     return with_vox16(vol_type, [&](auto v) {
-        using V = decltype(v);
-        if (too_big(D0, D1, D2)) return (int)B200DRR_EUNSUPPORTED;
-        return ret(launch_siddon_fwd_sens_structures((const V*)vol, labels, mk(D0, D1, D2), src, G, Wd, rows, cols, slot_of_label,
-                                                     box, out, sens, B, S, H, W, voxel_shift, eps, (cudaStream_t)stream));
+        return siddon_fwd_sens_structures<decltype(v)>(vol, labels, D0, D1, D2, src, G, Wd, rows, cols, slot_of_label, box, out,
+                                                       sens, B, S, H, W, voxel_shift, eps, stream);
     });
 }
 
-// ---- 16-bit volumes: twins of the Trilinear entry points --------------------------------------------------------------------------
+int b200drr_pack_corners(const float* vol, int D0, int D1, int D2, float* packed, void* stream)
+{
+    return pack_corners<float>(vol, D0, D1, D2, packed, stream);
+}
+
 int b200drr_pack_corners_v16(const void* vol, int vol_type, int D0, int D1, int D2, void* packed, void* stream)
 {
-    if (!vol || !packed || bad_dims(D0, D1, D2)) return B200DRR_EINVAL;
-    return with_vox16(vol_type, [&](auto v) {
-        using V = decltype(v);
-        if (((uintptr_t)packed & 15u) != 0) return (int)B200DRR_EINVAL;
-        return ret(launch_pack_corners16((const V*)vol, mk(D0, D1, D2), (Cell16<V>*)packed, (cudaStream_t)stream));
-    });
+    return with_vox16(vol_type, [&](auto v) { return pack_corners<decltype(v)>(vol, D0, D1, D2, packed, stream); });
+}
+
+int b200drr_trilinear_fwd(const float* vol, int D0, int D1, int D2, const float* src, const float* tgt, const float* raylen,
+                          float* out, int B, int64_t N, float voxel_shift, float eps, int n_points, const float* alpha_range,
+                          int reduce, int align_corners, void* stream)
+{
+    return trilinear_fwd<float>(vol, D0, D1, D2, src, tgt, raylen, out, B, N, voxel_shift, eps, n_points, alpha_range, reduce,
+                                align_corners, stream);
 }
 
 int b200drr_trilinear_fwd_v16(const void* vol, int vol_type, int D0, int D1, int D2, const float* src, const float* tgt,
                               const float* raylen, float* out, int B, int64_t N, float voxel_shift, float eps, int n_points,
                               const float* alpha_range, int reduce, int align_corners, void* stream)
 {
-    if (!vol || !src || !tgt || !raylen || !out || !alpha_range || bad_dims(D0, D1, D2) || bad_rays(B, N) || n_points < 2 ||
-        reduce != 0 || align_corners != 0)
-        return B200DRR_EINVAL;
     return with_vox16(vol_type, [&](auto v) {
-        using V = decltype(v);
-        return ret(launch_trilinear_fwd((const V*)vol, mk(D0, D1, D2), src, tgt, raylen, out, B, N, voxel_shift, eps, n_points,
-                                        alpha_range, 0, 0, (cudaStream_t)stream));
+        return trilinear_fwd<decltype(v)>(vol, D0, D1, D2, src, tgt, raylen, out, B, N, voxel_shift, eps, n_points, alpha_range,
+                                          reduce, align_corners, stream);
     });
+}
+
+int b200drr_trilinear_fwd_grid(const float* vol, int D0, int D1, int D2, const float* src, const float* tgt, const float* raylen,
+                               float* out, int B, int H, int W, float voxel_shift, float eps, int n_points,
+                               const float* alpha_range, int variant, void* stream)
+{
+    return trilinear_fwd_grid<float>(vol, D0, D1, D2, src, tgt, raylen, out, B, H, W, voxel_shift, eps, n_points, alpha_range,
+                                     variant, stream);
 }
 
 int b200drr_trilinear_fwd_grid_v16(const void* vol, int vol_type, int D0, int D1, int D2, const float* src, const float* tgt,
                                    const float* raylen, float* out, int B, int H, int W, float voxel_shift, float eps, int n_points,
                                    const float* alpha_range, int variant, void* stream)
 {
-    if (!vol || !src || !tgt || !raylen || !out || !alpha_range || bad_dims(D0, D1, D2) || bad_rays(B, (int64_t)H * W) ||
-        H <= 0 || W <= 0 || n_points < 2)
-        return B200DRR_EINVAL;
     return with_vox16(vol_type, [&](auto v) {
-        using V = decltype(v);
-        return ret(launch_trilinear_fwd_grid((const V*)vol, mk(D0, D1, D2), src, tgt, raylen, out, B, H, W, voxel_shift, eps,
-                                             n_points, alpha_range, variant, (cudaStream_t)stream));
+        return trilinear_fwd_grid<decltype(v)>(vol, D0, D1, D2, src, tgt, raylen, out, B, H, W, voxel_shift, eps, n_points,
+                                               alpha_range, variant, stream);
     });
+}
+
+int b200drr_trilinear_fwd_sens(const float* vol, int D0, int D1, int D2, const float* src, const float* tgt, const float* raylen,
+                               float* out, float* sens, int B, int64_t N, int H, int W, float voxel_shift, float eps, int n_points,
+                               const float* alpha_range, int align_corners, void* stream)
+{
+    return trilinear_fwd_sens<float>(vol, D0, D1, D2, src, tgt, raylen, out, sens, B, N, H, W, voxel_shift, eps, n_points,
+                                     alpha_range, align_corners, stream);
 }
 
 int b200drr_trilinear_fwd_sens_v16(const void* vol, int vol_type, int D0, int D1, int D2, const float* src, const float* tgt,
                                    const float* raylen, float* out, float* sens, int B, int64_t N, int H, int W, float voxel_shift,
                                    float eps, int n_points, const float* alpha_range, int align_corners, void* stream)
 {
-    if (!vol || !src || !tgt || !raylen || !out || !sens || !alpha_range || bad_dims(D0, D1, D2) || bad_rays(B, N) ||
-        n_points < 2 || H < 0 || W < 0 || (H > 0 && (int64_t)H * W != N) || align_corners != 0)
-        return B200DRR_EINVAL;
     return with_vox16(vol_type, [&](auto v) {
-        using V = decltype(v);
-        return ret(launch_trilinear_fwd_sens((const V*)vol, mk(D0, D1, D2), src, tgt, raylen, out, sens, B, N, H, W, voxel_shift,
-                                             eps, n_points, alpha_range, 0, (cudaStream_t)stream));
+        return trilinear_fwd_sens<decltype(v)>(vol, D0, D1, D2, src, tgt, raylen, out, sens, B, N, H, W, voxel_shift, eps, n_points,
+                                               alpha_range, align_corners, stream);
     });
+}
+
+int b200drr_trilinear_fwd_packed(const float* packed, int D0, int D1, int D2, const float* src, const float* tgt,
+                                 const float* raylen, float* out, int B, int H, int W, float voxel_shift, float eps, int n_points,
+                                 const float* alpha_range, int slab, void* stream)
+{
+    return trilinear_fwd_packed<float>(packed, D0, D1, D2, src, tgt, raylen, out, B, H, W, voxel_shift, eps, n_points, alpha_range,
+                                       slab, stream);
 }
 
 int b200drr_trilinear_fwd_packed_v16(const void* packed, int vol_type, int D0, int D1, int D2, const float* src, const float* tgt,
                                      const float* raylen, float* out, int B, int H, int W, float voxel_shift, float eps, int n_points,
                                      const float* alpha_range, int slab, void* stream)
 {
-    if (!packed || slab < 0 || !src || !tgt || !raylen || !out || !alpha_range || bad_dims(D0, D1, D2) ||
-        bad_rays(B, (int64_t)H * W) || H <= 0 || W <= 0 || n_points < 2)
-        return B200DRR_EINVAL;
     return with_vox16(vol_type, [&](auto v) {
-        using V = decltype(v);
-        return ret(launch_trilinear_fwd_packed_t((const Cell16<V>*)packed, mk(D0, D1, D2), src, tgt, raylen, out, B, H, W,
-                                                 voxel_shift, eps, n_points, alpha_range, slab, (cudaStream_t)stream));
+        return trilinear_fwd_packed<decltype(v)>(packed, D0, D1, D2, src, tgt, raylen, out, B, H, W, voxel_shift, eps, n_points,
+                                                 alpha_range, slab, stream);
     });
+}
+
+int b200drr_trilinear_fwd_sens_packed(const float* packed, int D0, int D1, int D2, const float* src, const float* tgt,
+                                      const float* raylen, float* out, float* sens, int B, int H, int W, float voxel_shift,
+                                      float eps, int n_points, const float* alpha_range, int slab, void* stream)
+{
+    return trilinear_fwd_sens_packed<float>(packed, D0, D1, D2, src, tgt, raylen, out, sens, B, H, W, voxel_shift, eps, n_points,
+                                            alpha_range, slab, stream);
 }
 
 int b200drr_trilinear_fwd_sens_packed_v16(const void* packed, int vol_type, int D0, int D1, int D2, const float* src,
@@ -904,15 +1014,18 @@ int b200drr_trilinear_fwd_sens_packed_v16(const void* packed, int vol_type, int 
                                           float voxel_shift, float eps, int n_points, const float* alpha_range, int slab,
                                           void* stream)
 {
-    if (!packed || !src || !tgt || !raylen || !out || !sens || !alpha_range || bad_dims(D0, D1, D2) ||
-        bad_rays(B, (int64_t)H * W) || H <= 0 || W <= 0 || n_points < 2 || slab < 0)
-        return B200DRR_EINVAL;
     return with_vox16(vol_type, [&](auto v) {
-        using V = decltype(v);
-        return ret(launch_trilinear_fwd_sens_packed16((const Cell16<V>*)packed, mk(D0, D1, D2), src, tgt, raylen, nullptr, nullptr,
-                                                      nullptr, nullptr, out, sens, B, H, W, voxel_shift, eps, n_points, alpha_range,
-                                                      slab, (cudaStream_t)stream));
+        return trilinear_fwd_sens_packed<decltype(v)>(packed, D0, D1, D2, src, tgt, raylen, out, sens, B, H, W, voxel_shift, eps,
+                                                      n_points, alpha_range, slab, stream);
     });
+}
+
+int b200drr_trilinear_fwd_sens_pose(const float* packed, int D0, int D1, int D2, const float* src, const float* G, const float* Wd,
+                                    const float* rows, const float* cols, float* out, float* sens, int B, int H, int W,
+                                    float voxel_shift, float eps, int n_points, const float* alpha_range, int slab, void* stream)
+{
+    return trilinear_fwd_sens_pose<float>(packed, D0, D1, D2, src, G, Wd, rows, cols, out, sens, B, H, W, voxel_shift, eps,
+                                          n_points, alpha_range, slab, stream);
 }
 
 int b200drr_trilinear_fwd_sens_pose_v16(const void* packed, int vol_type, int D0, int D1, int D2, const float* src, const float* G,
@@ -920,14 +1033,9 @@ int b200drr_trilinear_fwd_sens_pose_v16(const void* packed, int vol_type, int D0
                                         int W, float voxel_shift, float eps, int n_points, const float* alpha_range, int slab,
                                         void* stream)
 {
-    if (!packed || !src || !G || !Wd || !rows || !cols || !out || !sens || !alpha_range || bad_dims(D0, D1, D2) ||
-        bad_rays(B, (int64_t)H * W) || H <= 0 || W <= 0 || n_points < 2 || slab < 0)
-        return B200DRR_EINVAL;
     return with_vox16(vol_type, [&](auto v) {
-        using V = decltype(v);
-        return ret(launch_trilinear_fwd_sens_packed16((const Cell16<V>*)packed, mk(D0, D1, D2), src, nullptr, nullptr, G, Wd, rows,
-                                                      cols, out, sens, B, H, W, voxel_shift, eps, n_points, alpha_range, slab,
-                                                      (cudaStream_t)stream));
+        return trilinear_fwd_sens_pose<decltype(v)>(packed, D0, D1, D2, src, G, Wd, rows, cols, out, sens, B, H, W, voxel_shift, eps,
+                                                    n_points, alpha_range, slab, stream);
     });
 }
 
@@ -945,6 +1053,46 @@ int polyrigid_bad(const void* vol, const void* packed, int D0, int D1, int D2, c
     if (K > 8 || too_big(D0, D1, D2) || (int64_t)g0 * g1 * g2 * polyrigid_channels(K) >= (int64_t)INT32_MAX)
         return B200DRR_EUNSUPPORTED;
     return 0;
+}
+
+// one body per fp32 entry point and its 16-bit twin; vol_type is 0 for an fp32 volume, as the launchers take it
+int polyrigid_fwd(const void* vol, const void* packed, int vol_type, int D0, int D1, int D2, const float* src, const float* tgt,
+                  const float* raylen, const float* M, int Bm, int K, const float* weights, int g0, int g1, int g2, float* out, int B,
+                  int64_t N, int H, int W, float voxel_shift, float eps, int n_points, const float* alpha_range, void* stream)
+{
+    if (!out) return B200DRR_EINVAL;
+    if (const int bad = polyrigid_bad(vol, packed, D0, D1, D2, src, tgt, raylen, M, Bm, K, weights, g0, g1, g2, B, N, H, W, n_points,
+                                      alpha_range))
+        return bad;
+    return ret(launch_polyrigid_fwd(vol, packed, vol_type, mk(D0, D1, D2), src, tgt, raylen, M, Bm, K, weights, g0, g1, g2, out, B, N,
+                                    W, voxel_shift, eps, n_points, alpha_range, (cudaStream_t)stream));
+}
+
+int polyrigid_bwd(const void* vol, const void* packed, int vol_type, int D0, int D1, int D2, const float* src, const float* tgt,
+                  const float* raylen, const float* M, int Bm, int K, const float* weights, int g0, int g1, int g2, const float* gout,
+                  float* g_src, float* g_tgt, float* g_raylen, float* g_M, float* g_alpha_range, float* scratch, int B, int64_t N,
+                  int H, int W, float voxel_shift, float eps, int n_points, const float* alpha_range, void* stream)
+{
+    if (!gout || !scratch) return B200DRR_EINVAL;
+    if (const int bad = polyrigid_bad(vol, packed, D0, D1, D2, src, tgt, raylen, M, Bm, K, weights, g0, g1, g2, B, N, H, W, n_points,
+                                      alpha_range))
+        return bad;
+    return ret(launch_polyrigid_bwd(vol, packed, vol_type, mk(D0, D1, D2), src, tgt, raylen, M, Bm, K, weights, g0, g1, g2, gout, g_src,
+                                    g_tgt, g_raylen, g_M, g_alpha_range, scratch, B, N, W, voxel_shift, eps, n_points, alpha_range,
+                                    (cudaStream_t)stream));
+}
+
+int polyrigid_jac(const void* vol, const void* packed, int vol_type, int D0, int D1, int D2, const float* src, const float* tgt,
+                  const float* raylen, const float* M, int Bm, int K, const float* weights, int g0, int g1, int g2, const float* T,
+                  float* img, float* J, int32_t* rects, int B, int H, int W, float voxel_shift, float eps, int n_points,
+                  const float* alpha_range, void* stream)
+{
+    if (!T || !img || !J || !rects || H <= 0 || W <= 0) return B200DRR_EINVAL;
+    if (const int bad = polyrigid_bad(vol, packed, D0, D1, D2, src, tgt, raylen, M, Bm, K, weights, g0, g1, g2, B, (int64_t)H * W, H,
+                                      W, n_points, alpha_range))
+        return bad;
+    return ret(launch_polyrigid_jac(vol, packed, vol_type, mk(D0, D1, D2), src, tgt, raylen, M, Bm, K, weights, g0, g1, g2, T, img, J,
+                                    rects, B, H, W, voxel_shift, eps, n_points, alpha_range, (cudaStream_t)stream));
 }
 }  // namespace
 
@@ -972,12 +1120,18 @@ int b200drr_polyrigid_fwd(const float* vol, const float* packed, int D0, int D1,
                           int B, int64_t N, int H, int W, float voxel_shift, float eps, int n_points, const float* alpha_range,
                           void* stream)
 {
-    if (!out) return B200DRR_EINVAL;
-    if (const int bad = polyrigid_bad(vol, packed, D0, D1, D2, src, tgt, raylen, M, Bm, K, weights, g0, g1, g2, B, N, H, W, n_points,
-                                      alpha_range))
-        return bad;
-    return ret(launch_polyrigid_fwd(vol, packed, 0, mk(D0, D1, D2), src, tgt, raylen, M, Bm, K, weights, g0, g1, g2, out, B, N, W,
-                                    voxel_shift, eps, n_points, alpha_range, (cudaStream_t)stream));
+    return polyrigid_fwd(vol, packed, 0, D0, D1, D2, src, tgt, raylen, M, Bm, K, weights, g0, g1, g2, out, B, N, H, W, voxel_shift, eps,
+                         n_points, alpha_range, stream);
+}
+
+int b200drr_polyrigid_fwd_v16(const void* vol, const void* packed, int vol_type, int D0, int D1, int D2, const float* src,
+                              const float* tgt, const float* raylen, const float* M, int Bm, int K, const float* weights, int g0,
+                              int g1, int g2, float* out, int B, int64_t N, int H, int W, float voxel_shift, float eps, int n_points,
+                              const float* alpha_range, void* stream)
+{
+    if (bad_vol16(vol_type)) return B200DRR_EINVAL;
+    return polyrigid_fwd(vol, packed, vol_type, D0, D1, D2, src, tgt, raylen, M, Bm, K, weights, g0, g1, g2, out, B, N, H, W,
+                         voxel_shift, eps, n_points, alpha_range, stream);
 }
 
 int b200drr_polyrigid_bwd(const float* vol, const float* packed, int D0, int D1, int D2, const float* src, const float* tgt,
@@ -986,26 +1140,8 @@ int b200drr_polyrigid_bwd(const float* vol, const float* packed, int D0, int D1,
                           float* scratch, int B, int64_t N, int H, int W, float voxel_shift, float eps, int n_points,
                           const float* alpha_range, void* stream)
 {
-    if (!gout || !scratch) return B200DRR_EINVAL;
-    if (const int bad = polyrigid_bad(vol, packed, D0, D1, D2, src, tgt, raylen, M, Bm, K, weights, g0, g1, g2, B, N, H, W, n_points,
-                                      alpha_range))
-        return bad;
-    return ret(launch_polyrigid_bwd(vol, packed, 0, mk(D0, D1, D2), src, tgt, raylen, M, Bm, K, weights, g0, g1, g2, gout, g_src, g_tgt,
-                                    g_raylen, g_M, g_alpha_range, scratch, B, N, W, voxel_shift, eps, n_points, alpha_range,
-                                    (cudaStream_t)stream));
-}
-
-int b200drr_polyrigid_fwd_v16(const void* vol, const void* packed, int vol_type, int D0, int D1, int D2, const float* src,
-                              const float* tgt, const float* raylen, const float* M, int Bm, int K, const float* weights, int g0,
-                              int g1, int g2, float* out, int B, int64_t N, int H, int W, float voxel_shift, float eps, int n_points,
-                              const float* alpha_range, void* stream)
-{
-    if (!out || (vol_type != B200DRR_VOL_F16 && vol_type != B200DRR_VOL_BF16)) return B200DRR_EINVAL;
-    if (const int bad = polyrigid_bad(vol, packed, D0, D1, D2, src, tgt, raylen, M, Bm, K, weights, g0, g1, g2, B, N, H, W, n_points,
-                                      alpha_range))
-        return bad;
-    return ret(launch_polyrigid_fwd(vol, packed, vol_type, mk(D0, D1, D2), src, tgt, raylen, M, Bm, K, weights, g0, g1, g2, out, B, N,
-                                    W, voxel_shift, eps, n_points, alpha_range, (cudaStream_t)stream));
+    return polyrigid_bwd(vol, packed, 0, D0, D1, D2, src, tgt, raylen, M, Bm, K, weights, g0, g1, g2, gout, g_src, g_tgt, g_raylen, g_M,
+                         g_alpha_range, scratch, B, N, H, W, voxel_shift, eps, n_points, alpha_range, stream);
 }
 
 int b200drr_polyrigid_bwd_v16(const void* vol, const void* packed, int vol_type, int D0, int D1, int D2, const float* src,
@@ -1014,13 +1150,9 @@ int b200drr_polyrigid_bwd_v16(const void* vol, const void* packed, int vol_type,
                               float* g_alpha_range, float* scratch, int B, int64_t N, int H, int W, float voxel_shift, float eps,
                               int n_points, const float* alpha_range, void* stream)
 {
-    if (!gout || !scratch || (vol_type != B200DRR_VOL_F16 && vol_type != B200DRR_VOL_BF16)) return B200DRR_EINVAL;
-    if (const int bad = polyrigid_bad(vol, packed, D0, D1, D2, src, tgt, raylen, M, Bm, K, weights, g0, g1, g2, B, N, H, W, n_points,
-                                      alpha_range))
-        return bad;
-    return ret(launch_polyrigid_bwd(vol, packed, vol_type, mk(D0, D1, D2), src, tgt, raylen, M, Bm, K, weights, g0, g1, g2, gout, g_src,
-                                    g_tgt, g_raylen, g_M, g_alpha_range, scratch, B, N, W, voxel_shift, eps, n_points, alpha_range,
-                                    (cudaStream_t)stream));
+    if (bad_vol16(vol_type)) return B200DRR_EINVAL;
+    return polyrigid_bwd(vol, packed, vol_type, D0, D1, D2, src, tgt, raylen, M, Bm, K, weights, g0, g1, g2, gout, g_src, g_tgt,
+                         g_raylen, g_M, g_alpha_range, scratch, B, N, H, W, voxel_shift, eps, n_points, alpha_range, stream);
 }
 
 int b200drr_polyrigid_jac(const float* vol, const float* packed, int D0, int D1, int D2, const float* src, const float* tgt,
@@ -1028,12 +1160,8 @@ int b200drr_polyrigid_jac(const float* vol, const float* packed, int D0, int D1,
                           const float* T, float* img, float* J, int32_t* rects, int B, int H, int W, float voxel_shift, float eps,
                           int n_points, const float* alpha_range, void* stream)
 {
-    if (!T || !img || !J || !rects || H <= 0 || W <= 0) return B200DRR_EINVAL;
-    if (const int bad = polyrigid_bad(vol, packed, D0, D1, D2, src, tgt, raylen, M, Bm, K, weights, g0, g1, g2, B, (int64_t)H * W, H,
-                                      W, n_points, alpha_range))
-        return bad;
-    return ret(launch_polyrigid_jac(vol, packed, 0, mk(D0, D1, D2), src, tgt, raylen, M, Bm, K, weights, g0, g1, g2, T, img, J, rects, B,
-                                    H, W, voxel_shift, eps, n_points, alpha_range, (cudaStream_t)stream));
+    return polyrigid_jac(vol, packed, 0, D0, D1, D2, src, tgt, raylen, M, Bm, K, weights, g0, g1, g2, T, img, J, rects, B, H, W,
+                         voxel_shift, eps, n_points, alpha_range, stream);
 }
 
 int b200drr_polyrigid_jac_v16(const void* vol, const void* packed, int vol_type, int D0, int D1, int D2, const float* src,
@@ -1041,13 +1169,9 @@ int b200drr_polyrigid_jac_v16(const void* vol, const void* packed, int vol_type,
                               int g1, int g2, const float* T, float* img, float* J, int32_t* rects, int B, int H, int W,
                               float voxel_shift, float eps, int n_points, const float* alpha_range, void* stream)
 {
-    if (!T || !img || !J || !rects || H <= 0 || W <= 0 || (vol_type != B200DRR_VOL_F16 && vol_type != B200DRR_VOL_BF16))
-        return B200DRR_EINVAL;
-    if (const int bad = polyrigid_bad(vol, packed, D0, D1, D2, src, tgt, raylen, M, Bm, K, weights, g0, g1, g2, B, (int64_t)H * W, H,
-                                      W, n_points, alpha_range))
-        return bad;
-    return ret(launch_polyrigid_jac(vol, packed, vol_type, mk(D0, D1, D2), src, tgt, raylen, M, Bm, K, weights, g0, g1, g2, T, img, J,
-                                    rects, B, H, W, voxel_shift, eps, n_points, alpha_range, (cudaStream_t)stream));
+    if (bad_vol16(vol_type)) return B200DRR_EINVAL;
+    return polyrigid_jac(vol, packed, vol_type, D0, D1, D2, src, tgt, raylen, M, Bm, K, weights, g0, g1, g2, T, img, J, rects, B, H, W,
+                         voxel_shift, eps, n_points, alpha_range, stream);
 }
 
 // ---- deformable (dense displacement field) trilinear render (deform.cu) ------------------------------------------------------------
@@ -1071,6 +1195,42 @@ int deform_bad(const void* vol, const void* packed, int D0, int D1, int D2, cons
     if ((vol == nullptr) == (packed == nullptr) || ((uintptr_t)packed & 15u) != 0) return B200DRR_EINVAL;
     return deform_geom_bad(D0, D1, D2, src, tgt, raylen, field, Bf, g0, g1, g2, B, N, H, W, n_points, alpha_range);
 }
+
+// one body per fp32 entry point and its 16-bit twin; vol_type is 0 for an fp32 volume, as the launchers take it
+int deform_fwd(const void* vol, const void* packed, int vol_type, int D0, int D1, int D2, const float* src, const float* tgt,
+               const float* raylen, const float* field, int Bf, int g0, int g1, int g2, float* out, int B, int64_t N, int H, int W,
+               float voxel_shift, float eps, int n_points, const float* alpha_range, void* stream)
+{
+    if (!out) return B200DRR_EINVAL;
+    if (const int bad = deform_bad(vol, packed, D0, D1, D2, src, tgt, raylen, field, Bf, g0, g1, g2, B, N, H, W, n_points, alpha_range))
+        return bad;
+    return ret(launch_deform_fwd(vol, packed, vol_type, mk(D0, D1, D2), src, tgt, raylen, field, Bf, g0, g1, g2, out, B, N, W, voxel_shift,
+                                 eps, n_points, alpha_range, (cudaStream_t)stream));
+}
+
+int deform_bwd(const void* vol, const void* packed, int vol_type, int D0, int D1, int D2, const float* src, const float* tgt,
+               const float* raylen, const float* field, int Bf, int g0, int g1, int g2, const float* gout, float* g_src, float* g_tgt,
+               float* g_raylen, float* g_field, float* g_alpha_range, float* scratch, int B, int64_t N, int H, int W, float voxel_shift,
+               float eps, int n_points, const float* alpha_range, void* stream)
+{
+    if (!gout || !scratch || ((uintptr_t)g_field & 15u) != 0) return B200DRR_EINVAL;
+    if (const int bad = deform_bad(vol, packed, D0, D1, D2, src, tgt, raylen, field, Bf, g0, g1, g2, B, N, H, W, n_points, alpha_range))
+        return bad;
+    return ret(launch_deform_bwd(vol, packed, vol_type, mk(D0, D1, D2), src, tgt, raylen, field, Bf, g0, g1, g2, gout, g_src, g_tgt,
+                                 g_raylen, g_field, g_alpha_range, scratch, B, N, W, voxel_shift, eps, n_points, alpha_range,
+                                 (cudaStream_t)stream));
+}
+
+int deform_jvp(const void* vol, const void* packed, int vol_type, int D0, int D1, int D2, const float* src, const float* tgt,
+               const float* raylen, const float* field, int Bf, int g0, int g1, int g2, const float* tangent, float* img, float* jv, int B,
+               int64_t N, int H, int W, float voxel_shift, float eps, int n_points, const float* alpha_range, void* stream)
+{
+    if (!tangent || !jv || ((uintptr_t)tangent & 15u) != 0) return B200DRR_EINVAL;
+    if (const int bad = deform_bad(vol, packed, D0, D1, D2, src, tgt, raylen, field, Bf, g0, g1, g2, B, N, H, W, n_points, alpha_range))
+        return bad;
+    return ret(launch_deform_jvp(vol, packed, vol_type, mk(D0, D1, D2), src, tgt, raylen, field, Bf, g0, g1, g2, tangent, img, jv, B, N,
+                                 W, voxel_shift, eps, n_points, alpha_range, (cudaStream_t)stream));
+}
 }  // namespace
 
 int64_t b200drr_deform_scratch_floats(int B, int64_t N, int H, int W)
@@ -1083,11 +1243,17 @@ int b200drr_deform_fwd(const float* vol, const float* packed, int D0, int D1, in
                        const float* raylen, const float* field, int Bf, int g0, int g1, int g2, float* out, int B, int64_t N, int H,
                        int W, float voxel_shift, float eps, int n_points, const float* alpha_range, void* stream)
 {
-    if (!out) return B200DRR_EINVAL;
-    if (const int bad = deform_bad(vol, packed, D0, D1, D2, src, tgt, raylen, field, Bf, g0, g1, g2, B, N, H, W, n_points, alpha_range))
-        return bad;
-    return ret(launch_deform_fwd(vol, packed, 0, mk(D0, D1, D2), src, tgt, raylen, field, Bf, g0, g1, g2, out, B, N, W, voxel_shift, eps,
-                                 n_points, alpha_range, (cudaStream_t)stream));
+    return deform_fwd(vol, packed, 0, D0, D1, D2, src, tgt, raylen, field, Bf, g0, g1, g2, out, B, N, H, W, voxel_shift, eps, n_points,
+                      alpha_range, stream);
+}
+
+int b200drr_deform_fwd_v16(const void* vol, const void* packed, int vol_type, int D0, int D1, int D2, const float* src, const float* tgt,
+                           const float* raylen, const float* field, int Bf, int g0, int g1, int g2, float* out, int B, int64_t N, int H,
+                           int W, float voxel_shift, float eps, int n_points, const float* alpha_range, void* stream)
+{
+    if (bad_vol16(vol_type)) return B200DRR_EINVAL;
+    return deform_fwd(vol, packed, vol_type, D0, D1, D2, src, tgt, raylen, field, Bf, g0, g1, g2, out, B, N, H, W, voxel_shift, eps,
+                      n_points, alpha_range, stream);
 }
 
 int b200drr_deform_bwd(const float* vol, const float* packed, int D0, int D1, int D2, const float* src, const float* tgt,
@@ -1095,22 +1261,8 @@ int b200drr_deform_bwd(const float* vol, const float* packed, int D0, int D1, in
                        float* g_tgt, float* g_raylen, float* g_field, float* g_alpha_range, float* scratch, int B, int64_t N, int H,
                        int W, float voxel_shift, float eps, int n_points, const float* alpha_range, void* stream)
 {
-    if (!gout || !scratch || ((uintptr_t)g_field & 15u) != 0) return B200DRR_EINVAL;
-    if (const int bad = deform_bad(vol, packed, D0, D1, D2, src, tgt, raylen, field, Bf, g0, g1, g2, B, N, H, W, n_points, alpha_range))
-        return bad;
-    return ret(launch_deform_bwd(vol, packed, 0, mk(D0, D1, D2), src, tgt, raylen, field, Bf, g0, g1, g2, gout, g_src, g_tgt, g_raylen,
-                                 g_field, g_alpha_range, scratch, B, N, W, voxel_shift, eps, n_points, alpha_range, (cudaStream_t)stream));
-}
-
-int b200drr_deform_fwd_v16(const void* vol, const void* packed, int vol_type, int D0, int D1, int D2, const float* src, const float* tgt,
-                           const float* raylen, const float* field, int Bf, int g0, int g1, int g2, float* out, int B, int64_t N, int H,
-                           int W, float voxel_shift, float eps, int n_points, const float* alpha_range, void* stream)
-{
-    if (!out || (vol_type != B200DRR_VOL_F16 && vol_type != B200DRR_VOL_BF16)) return B200DRR_EINVAL;
-    if (const int bad = deform_bad(vol, packed, D0, D1, D2, src, tgt, raylen, field, Bf, g0, g1, g2, B, N, H, W, n_points, alpha_range))
-        return bad;
-    return ret(launch_deform_fwd(vol, packed, vol_type, mk(D0, D1, D2), src, tgt, raylen, field, Bf, g0, g1, g2, out, B, N, W, voxel_shift,
-                                 eps, n_points, alpha_range, (cudaStream_t)stream));
+    return deform_bwd(vol, packed, 0, D0, D1, D2, src, tgt, raylen, field, Bf, g0, g1, g2, gout, g_src, g_tgt, g_raylen, g_field,
+                      g_alpha_range, scratch, B, N, H, W, voxel_shift, eps, n_points, alpha_range, stream);
 }
 
 int b200drr_deform_bwd_v16(const void* vol, const void* packed, int vol_type, int D0, int D1, int D2, const float* src, const float* tgt,
@@ -1118,13 +1270,9 @@ int b200drr_deform_bwd_v16(const void* vol, const void* packed, int vol_type, in
                            float* g_tgt, float* g_raylen, float* g_field, float* g_alpha_range, float* scratch, int B, int64_t N, int H,
                            int W, float voxel_shift, float eps, int n_points, const float* alpha_range, void* stream)
 {
-    if (!gout || !scratch || ((uintptr_t)g_field & 15u) != 0 || (vol_type != B200DRR_VOL_F16 && vol_type != B200DRR_VOL_BF16))
-        return B200DRR_EINVAL;
-    if (const int bad = deform_bad(vol, packed, D0, D1, D2, src, tgt, raylen, field, Bf, g0, g1, g2, B, N, H, W, n_points, alpha_range))
-        return bad;
-    return ret(launch_deform_bwd(vol, packed, vol_type, mk(D0, D1, D2), src, tgt, raylen, field, Bf, g0, g1, g2, gout, g_src, g_tgt,
-                                 g_raylen, g_field, g_alpha_range, scratch, B, N, W, voxel_shift, eps, n_points, alpha_range,
-                                 (cudaStream_t)stream));
+    if (bad_vol16(vol_type)) return B200DRR_EINVAL;
+    return deform_bwd(vol, packed, vol_type, D0, D1, D2, src, tgt, raylen, field, Bf, g0, g1, g2, gout, g_src, g_tgt, g_raylen, g_field,
+                      g_alpha_range, scratch, B, N, H, W, voxel_shift, eps, n_points, alpha_range, stream);
 }
 
 int b200drr_deform_jvp(const float* vol, const float* packed, int D0, int D1, int D2, const float* src, const float* tgt,
@@ -1132,11 +1280,8 @@ int b200drr_deform_jvp(const float* vol, const float* packed, int D0, int D1, in
                        float* jv, int B, int64_t N, int H, int W, float voxel_shift, float eps, int n_points, const float* alpha_range,
                        void* stream)
 {
-    if (!tangent || !jv || ((uintptr_t)tangent & 15u) != 0) return B200DRR_EINVAL;
-    if (const int bad = deform_bad(vol, packed, D0, D1, D2, src, tgt, raylen, field, Bf, g0, g1, g2, B, N, H, W, n_points, alpha_range))
-        return bad;
-    return ret(launch_deform_jvp(vol, packed, 0, mk(D0, D1, D2), src, tgt, raylen, field, Bf, g0, g1, g2, tangent, img, jv, B, N, W,
-                                 voxel_shift, eps, n_points, alpha_range, (cudaStream_t)stream));
+    return deform_jvp(vol, packed, 0, D0, D1, D2, src, tgt, raylen, field, Bf, g0, g1, g2, tangent, img, jv, B, N, H, W, voxel_shift,
+                      eps, n_points, alpha_range, stream);
 }
 
 int b200drr_deform_jvp_v16(const void* vol, const void* packed, int vol_type, int D0, int D1, int D2, const float* src, const float* tgt,
@@ -1144,12 +1289,9 @@ int b200drr_deform_jvp_v16(const void* vol, const void* packed, int vol_type, in
                            float* jv, int B, int64_t N, int H, int W, float voxel_shift, float eps, int n_points,
                            const float* alpha_range, void* stream)
 {
-    if (!tangent || !jv || ((uintptr_t)tangent & 15u) != 0 || (vol_type != B200DRR_VOL_F16 && vol_type != B200DRR_VOL_BF16))
-        return B200DRR_EINVAL;
-    if (const int bad = deform_bad(vol, packed, D0, D1, D2, src, tgt, raylen, field, Bf, g0, g1, g2, B, N, H, W, n_points, alpha_range))
-        return bad;
-    return ret(launch_deform_jvp(vol, packed, vol_type, mk(D0, D1, D2), src, tgt, raylen, field, Bf, g0, g1, g2, tangent, img, jv, B, N,
-                                 W, voxel_shift, eps, n_points, alpha_range, (cudaStream_t)stream));
+    if (bad_vol16(vol_type)) return B200DRR_EINVAL;
+    return deform_jvp(vol, packed, vol_type, D0, D1, D2, src, tgt, raylen, field, Bf, g0, g1, g2, tangent, img, jv, B, N, H, W,
+                      voxel_shift, eps, n_points, alpha_range, stream);
 }
 
 int b200drr_deform_bproj(int D0, int D1, int D2, const float* src, const float* tgt, const float* raylen, const float* field, int Bf,
@@ -1239,30 +1381,13 @@ int64_t b200drr_packed_volume_floats(int D0, int D1, int D2)
     return (int64_t)(D0 + 1) * (D1 + 1) * (D2 + 1) * 8;
 }
 
-int b200drr_pack_corners(const float* vol, int D0, int D1, int D2, float* packed, void* stream)
-{
-    if (!vol || !packed || bad_dims(D0, D1, D2)) return B200DRR_EINVAL;
-    return ret(launch_pack_corners(vol, mk(D0, D1, D2), packed, (cudaStream_t)stream));
-}
-
-int b200drr_trilinear_fwd_packed(const float* packed, int D0, int D1, int D2, const float* src, const float* tgt,
-                                 const float* raylen, float* out, int B, int H, int W, float voxel_shift, float eps,
-                                 int n_points, const float* alpha_range, int slab, void* stream)
-{
-    if (!packed || slab < 0 || !src || !tgt || !raylen || !out || !alpha_range || bad_dims(D0, D1, D2) ||
-        bad_rays(B, (int64_t)H * W) || H <= 0 || W <= 0 || n_points < 2)
-        return B200DRR_EINVAL;
-    return ret(launch_trilinear_fwd_packed(packed, mk(D0, D1, D2), src, tgt, raylen, out, B, H, W, voxel_shift, eps,
-                                           n_points, alpha_range, slab, (cudaStream_t)stream));
-}
-
 int b200drr_trilinear_bwd_packed(const float* packed, int D0, int D1, int D2, const float* src, const float* tgt,
                                  const float* raylen, const float* gout, float* g_src, float* g_tgt, float* g_raylen,
                                  float* g_alpha_range, int B, int H, int W, float voxel_shift, float eps, int n_points,
                                  const float* alpha_range, int slab, void* stream)
 {
     if (!packed || slab < 0 || !src || !tgt || !raylen || !gout || !alpha_range || bad_dims(D0, D1, D2) ||
-        bad_rays(B, (int64_t)H * W) || H <= 0 || W <= 0 || n_points < 2)
+        bad_grid(B, H, W) || n_points < 2)
         return B200DRR_EINVAL;
     return ret(launch_trilinear_bwd_packed(packed, mk(D0, D1, D2), src, tgt, raylen, gout, g_src, g_tgt, g_raylen,
                                            g_alpha_range, B, H, W, voxel_shift, eps, n_points, alpha_range, slab,

@@ -262,6 +262,10 @@ _SIGNATURES = {
         ctypes.c_int, ctypes.c_int, _c_float_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, _c_float_p, _c_float_p, _c_float_p,
         _c_float_p, _c_float_p, _c_float_p, _c_float_p, ctypes.c_int, ctypes.c_int64, ctypes.c_int, ctypes.c_int, ctypes.c_float,
         ctypes.c_float, ctypes.c_int, _c_float_p, ctypes.c_void_p]),
+    "b200drr_polyrigid_bproj": (ctypes.c_int, [
+        ctypes.c_int, ctypes.c_int, ctypes.c_int, _c_float_p, _c_float_p, _c_float_p, _c_float_p, ctypes.c_int, ctypes.c_int,
+        _c_float_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, _c_float_p, _c_float_p, ctypes.c_int, ctypes.c_int64, ctypes.c_int,
+        ctypes.c_int, ctypes.c_float, ctypes.c_float, ctypes.c_int, _c_float_p, ctypes.c_void_p]),
     "b200drr_polyrigid_jac": (ctypes.c_int, [
         _c_float_p, _c_float_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, _c_float_p, _c_float_p, _c_float_p, _c_float_p,
         ctypes.c_int, ctypes.c_int, _c_float_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, _c_float_p, _c_float_p, _c_float_p,

@@ -1041,18 +1041,27 @@ int b200drr_trilinear_fwd_sens_pose_v16(const void* packed, int vol_type, int D0
 
 // ---- blended-rigid (skinned) trilinear render (polyrigid.cu) ----------------------------------------------------------------------
 namespace {
-// the checks every polyrigid entry point shares; 0 = go on
-int polyrigid_bad(const void* vol, const void* packed, int D0, int D1, int D2, const float* src, const float* tgt, const float* raylen,
-                  const float* M, int Bm, int K, const float* weights, int g0, int g1, int g2, int B, int64_t N, int H, int W,
-                  int n_points, const float* alpha_range)
+// the geometry, lattice and map checks, without the volume
+int polyrigid_geom_bad(int D0, int D1, int D2, const float* src, const float* tgt, const float* raylen, const float* M, int Bm, int K,
+                       const float* weights, int g0, int g1, int g2, int B, int64_t N, int H, int W, int n_points,
+                       const float* alpha_range)
 {
-    if ((vol == nullptr) == (packed == nullptr) || !src || !tgt || !raylen || !M || !weights || !alpha_range || bad_dims(D0, D1, D2) ||
-        bad_dims(g0, g1, g2) || bad_rays(B, N) || K <= 0 || (Bm != 1 && Bm != B) || n_points < 2 || H < 0 || W < 0 ||
-        ((H > 0 || W > 0) && (int64_t)H * W != N) || (((uintptr_t)weights | (uintptr_t)packed) & 15u) != 0)
+    if (!src || !tgt || !raylen || !M || !weights || !alpha_range || bad_dims(D0, D1, D2) || bad_dims(g0, g1, g2) || bad_rays(B, N) ||
+        K <= 0 || (Bm != 1 && Bm != B) || n_points < 2 || H < 0 || W < 0 || ((H > 0 || W > 0) && (int64_t)H * W != N) ||
+        ((uintptr_t)weights & 15u) != 0)
         return B200DRR_EINVAL;
     if (K > 8 || too_big(D0, D1, D2) || (int64_t)g0 * g1 * g2 * polyrigid_channels(K) >= (int64_t)INT32_MAX)
         return B200DRR_EUNSUPPORTED;
     return 0;
+}
+
+// the checks every polyrigid entry point with a volume shares; 0 = go on
+int polyrigid_bad(const void* vol, const void* packed, int D0, int D1, int D2, const float* src, const float* tgt, const float* raylen,
+                  const float* M, int Bm, int K, const float* weights, int g0, int g1, int g2, int B, int64_t N, int H, int W,
+                  int n_points, const float* alpha_range)
+{
+    if ((vol == nullptr) == (packed == nullptr) || ((uintptr_t)packed & 15u) != 0) return B200DRR_EINVAL;
+    return polyrigid_geom_bad(D0, D1, D2, src, tgt, raylen, M, Bm, K, weights, g0, g1, g2, B, N, H, W, n_points, alpha_range);
 }
 
 // one body per fp32 entry point and its 16-bit twin; vol_type is 0 for an fp32 volume, as the launchers take it
@@ -1172,6 +1181,18 @@ int b200drr_polyrigid_jac_v16(const void* vol, const void* packed, int vol_type,
     if (bad_vol16(vol_type)) return B200DRR_EINVAL;
     return polyrigid_jac(vol, packed, vol_type, D0, D1, D2, src, tgt, raylen, M, Bm, K, weights, g0, g1, g2, T, img, J, rects, B, H, W,
                          voxel_shift, eps, n_points, alpha_range, stream);
+}
+
+int b200drr_polyrigid_bproj(int D0, int D1, int D2, const float* src, const float* tgt, const float* raylen, const float* M, int Bm,
+                            int K, const float* wpacked, int g0, int g1, int g2, const float* gout, float* g_vol, int B, int64_t N,
+                            int H, int W, float voxel_shift, float eps, int n_points, const float* alpha_range, void* stream)
+{
+    if (!gout || !g_vol) return B200DRR_EINVAL;
+    if (const int bad = polyrigid_geom_bad(D0, D1, D2, src, tgt, raylen, M, Bm, K, wpacked, g0, g1, g2, B, N, H, W, n_points,
+                                           alpha_range))
+        return bad;
+    return ret(launch_polyrigid_bproj(mk(D0, D1, D2), src, tgt, raylen, M, Bm, K, wpacked, g0, g1, g2, gout, g_vol, B, N, W,
+                                      voxel_shift, eps, n_points, alpha_range, (cudaStream_t)stream));
 }
 
 // ---- deformable (dense displacement field) trilinear render (deform.cu) ------------------------------------------------------------

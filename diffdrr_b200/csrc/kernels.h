@@ -298,6 +298,10 @@ cudaError_t launch_polyrigid_jac(const void* vol, const void* packed, int vol_ty
                                  const float* raylen, const float* M, int Bm, int K, const float* weights, int g0, int g1, int g2,
                                  const float* T, float* img, float* J, int* rects, int B, int H, int W, float shift, float eps,
                                  int n_points, const float* alpha_range, cudaStream_t stream);
+// the forward's transpose in the density: g_vol [D0][D1][D2], zeroed here, += sum over the rays of gout * d out / d V
+cudaError_t launch_polyrigid_bproj(VolDims dims, const float* src, const float* tgt, const float* raylen, const float* M, int Bm, int K,
+                                   const float* weights, int g0, int g1, int g2, const float* gout, float* g_vol, int B, int64_t N, int W,
+                                   float shift, float eps, int n_points, const float* alpha_range, cudaStream_t stream);
 // the fixed-order finish of the blended-rigid backward's per-CTA partial rows; deform.cu launches it too
 __global__ void __launch_bounds__(256) polyrigid_finish_kernel(const float* __restrict__ partial, int row, int KP, int B, int T, int Bm,
                                                                int K, float* __restrict__ g_M, float* __restrict__ g_src,

@@ -3,7 +3,9 @@
 // grid (W > 0) or 128 consecutive rays of any ray set (W == 0), as tiled_ray_index lays them out.  The pose's K affine maps sit in
 // shared memory.  The forward and backward write every output from exactly one thread and use no atomics: the backward kernel
 // writes one row of partial sums per CTA and polyrigid_finish_kernel adds the rows in a fixed order, so repeated calls give
-// identical bits.  The Jacobian's footprints use integer min / max atomics, which do not depend on order.
+// identical bits.  The Jacobian's footprints use integer min / max atomics, which do not depend on order.  The backprojection kernel
+// (the forward's transpose in the density) reads the maps from global memory, with no shared memory, and scatters into one volume
+// gradient with scalar reductions, shared and per-pose maps alike: it repeats to fp32 reordering.
 #include <climits>
 
 #include "kernels.h"
@@ -44,6 +46,27 @@ __global__ void __launch_bounds__(kPolyThreads, 6) polyrigid_fwd_kernel(Gather g
     const float amin = __ldg(alpha_range), amax = __ldg(alpha_range + 1);
     const float step = (amax - amin) / (float)(P - 1);
     out[r] = polyrigid_ray_fwd<KP>(gather, dims, lat, sM, ray, shift, P, amin, amax) * (__ldg(raylen + r) * step);
+}
+
+// g_vol [D0][D1][D2] += the transpose of polyrigid_fwd_kernel in the density, for upstream gradient gout (polyrigid_ray_bproj)
+template <int KP>
+__global__ void __launch_bounds__(kPolyThreads) polyrigid_bproj_kernel(VolDims dims, PolyLattice lat, const float* __restrict__ M,
+                                                                       int Bm, int K, const float* __restrict__ src,
+                                                                       const float* __restrict__ tgt, const float* __restrict__ raylen,
+                                                                       const float* __restrict__ gout, float* g_vol, int64_t N, int W,
+                                                                       float shift, float eps, int P, const float* __restrict__ alpha_range)
+{
+    const int b = blockIdx.y;
+    const int64_t n = tiled_ray_index(N, W);
+    if (n < 0) return;
+    const int64_t r = (int64_t)b * N + n;
+    const float amin = __ldg(alpha_range), amax = __ldg(alpha_range + 1);
+    const float step = (amax - amin) / (float)(P - 1);
+    const float c = __ldg(gout + r) * __ldg(raylen + r) * step;
+    if (c == 0.0f) return;  // every add would be a zero
+    const float* Mb = M + (Bm == 1 ? 0 : (int64_t)b * K * 12);
+    const Ray ray = load_ray(src, tgt, b, r, eps);
+    polyrigid_ray_bproj<KP>(dims, lat, Mb, K, ray, shift, P, amin, amax, c, g_vol);
 }
 
 template <int KP, class Gather>
@@ -364,6 +387,24 @@ cudaError_t launch_polyrigid_jac(const void* vol, const void* packed, int vol_ty
     return with_gather(vol, packed, vol_type, [&](auto gather) {
         return K <= 4 ? run_jac<4>(gather, c, T, img, J, rects, H) : run_jac<8>(gather, c, T, img, J, rects, H);
     });
+}
+
+cudaError_t launch_polyrigid_bproj(VolDims dims, const float* src, const float* tgt, const float* raylen, const float* M, int Bm, int K,
+                                   const float* weights, int g0, int g1, int g2, const float* gout, float* g_vol, int B, int64_t N, int W,
+                                   float shift, float eps, int n_points, const float* alpha_range, cudaStream_t stream)
+{
+    const size_t bytes = sizeof(float) * (size_t)dims.d[0] * dims.d[1] * dims.d[2];
+    const cudaError_t e = cudaMemsetAsync(g_vol, 0, bytes, stream);
+    if (e != cudaSuccess) return e;
+    const PolyLattice lat = make_lattice(weights, g0, g1, g2, dims);
+    const dim3 grid = tiled_ray_grid(B, N, W);
+    if (K <= 4)
+        polyrigid_bproj_kernel<4><<<grid, kPolyThreads, 0, stream>>>(dims, lat, M, Bm, K, src, tgt, raylen, gout, g_vol, N, W, shift, eps,
+                                                                     n_points, alpha_range);
+    else
+        polyrigid_bproj_kernel<8><<<grid, kPolyThreads, 0, stream>>>(dims, lat, M, Bm, K, src, tgt, raylen, gout, g_vol, N, W, shift, eps,
+                                                                     n_points, alpha_range);
+    return cudaGetLastError();
 }
 
 }  // namespace b200drr

@@ -6,7 +6,9 @@
 //   y_m = x_m + sum_k w_k(x_m) (M_k [x_m; 1] - x_m),      I = L step sum_m tri(V, y_m)
 // w_k is a coarse lattice sampled trilinearly (align_corners=False over the volume, zero outside the lattice), stored channel-last
 // with the channels padded to KP = 4 or 8 (zero weights, zero matrices), so a lattice corner is KP / 4 float4 reads.
-// With M = identity or w = 0 the displacement is exactly 0.0f and the march is trilinear_ray_fwd bit for bit.
+// With M = identity or w = 0 the displacement is exactly 0.0f and the march is trilinear_ray_fwd bit for bit.  The backprojection
+// (polyrigid_ray_bproj) is the forward's transpose in the density: 8 scalar reductions per in-volume sample into a volume gradient,
+// with no density read.
 #pragma once
 
 #include "ray_math.cuh"
@@ -192,6 +194,64 @@ B200_HD float polyrigid_ray_fwd(const Gather& gather, const VolDims& dims, const
         acc += val;
     }
     return acc;
+}
+
+// Transpose of polyrigid_ray_fwd in the density (DESIGN.md 6o): polyrigid_ray_fwd's samples through the same arithmetic, each adding
+//   g_vol[corner] += c tri_weight(corner, y_m)
+// to the in-bounds corners of the cell around y_m, for every y_m inside the padded volume.  The cell, the fractions and the weight
+// product are deform_ray_bproj's, so with w = 0 or identity maps every add is the Trilinear volume gradient's.  c = gout raylen step;
+// no density is read.  M: the pose's K maps [K][12], read from global memory (no shared copy); rows k >= K read as zeros, the
+// forward's zero-padded rows, so the blend's arithmetic is the forward's.
+template <int KP>
+B200_HD void polyrigid_ray_bproj(const VolDims& dims, const PolyLattice& lat, const float* M, int K, const Ray& ray, float shift, int P,
+                                 float amin, float amax, float c, float* g_vol)
+{
+    const PixLine pl = make_pixline(ray, dims, shift, 0);
+    const float range = amax - amin;
+    const float lstep = 1.0f / (float)(P - 1);
+    const float kb = shift - 0.5f;  // pix = x + kb
+    int m_lo, m_hi;
+    poly_sample_range(pl, lat, amin, range, P, m_lo, m_hi);
+    for (int m = m_lo; m <= m_hi; ++m) {
+        const float alpha = add_rn(mul_rn(linspace01(m, P, lstep), range), amin);
+        float pix[3], w[KP];
+#pragma unroll
+        for (int a = 0; a < 3; ++a) pix[a] = fmaf(alpha, pl.dp[a], pl.p0[a]);
+        if (poly_weights<KP, false>(lat, pix, w, nullptr)) {
+            const float x[3] = {pix[0] - kb, pix[1] - kb, pix[2] - kb};
+            float disp[3] = {0.0f, 0.0f, 0.0f};
+#pragma unroll
+            for (int k = 0; k < KP; ++k) {
+                float Mk[12], o[3];
+#pragma unroll
+                for (int e = 0; e < 12; ++e) Mk[e] = k < K ? ldg(M + 12 * k + e) : 0.0f;
+                poly_offset(Mk, x, o);
+#pragma unroll
+                for (int a = 0; a < 3; ++a) disp[a] = fmaf(w[k], o[a], disp[a]);
+            }
+#pragma unroll
+            for (int a = 0; a < 3; ++a) pix[a] += disp[a];
+        }
+        if (!inside_padded(pix, dims)) continue;
+        float f[3], e[3];
+        int i0[3];
+#pragma unroll
+        for (int a = 0; a < 3; ++a) {
+            const float fl = floorf(pix[a]);
+            f[a] = pix[a] - fl;
+            e[a] = 1.0f - f[a];
+            i0[a] = (int)fl;
+        }
+        const int64_t base = ((int64_t)i0[0] * dims.d[1] + i0[1]) * dims.d[2] + i0[2];
+#pragma unroll
+        for (int q = 0; q < 8; ++q) {
+            const int x = i0[0] + (q & 1), y = i0[1] + ((q >> 1) & 1), z = i0[2] + ((q >> 2) & 1);
+            if ((unsigned)x < (unsigned)dims.d[0] && (unsigned)y < (unsigned)dims.d[1] && (unsigned)z < (unsigned)dims.d[2]) {
+                const float wq = ((q & 1) ? f[0] : e[0]) * (((q >> 1) & 1) ? f[1] : e[1]) * (((q >> 2) & 1) ? f[2] : e[2]);
+                red_add(g_vol + base + corner_off(dims, q), c * wq);
+            }
+        }
+    }
 }
 
 // Closed-form backward of one ray (DESIGN.md 6h).  With G_m the interpolant's gradient at y_m and

@@ -48,6 +48,23 @@ def _check_density(vol, name, no_grad):
                                 "fallback")
 
 
+def _rendered_density(drr, density, name, no_grad):
+    """The density a warped render `name` marches -> (vol, the refusal _check_density takes): drr.density with `no_grad`, the
+    refusal of a drr.density that requires grad; or the volume passed as density=, which must have drr.density's shape and device,
+    and may require grad when it is fp32."""
+    vol = drr.density
+    if density is None:
+        return vol, no_grad
+    # the module keeps the geometry (affine, dims); the volume fitted through it is passed in
+    if not torch.is_tensor(density) or density.shape != vol.shape or density.device != vol.device:
+        got = f"{tuple(density.shape)} on {density.device}" if torch.is_tensor(density) else type(density).__name__
+        raise ValueError(f"density must be a tensor of drr.density's shape {tuple(vol.shape)} on its device {vol.device}, got {got}")
+    if density.dtype != torch.float32:
+        return density, (f"{name} produces no volume gradient to a {density.dtype} density: 16-bit volumes are static densities "
+                         "(optimise an fp32 volume for volume gradients)")
+    return density, None
+
+
 def check_supported(drr, args, parameterization, field, kwargs, density=None):
     """Refuse, before any launch, what the deformable render does not cover: -> B.  density: the volume rendered in place of
     drr.density (render_deformed's density=), or None."""
@@ -60,21 +77,9 @@ def check_supported(drr, args, parameterization, field, kwargs, density=None):
     g0, g1, g2 = field.shape[-3:]
     if 4 * g0 * g1 * g2 >= 2**31 - 1:
         raise NotImplementedError(f"render_deformed takes a lattice below 2^31 floats per pose (4 channels), got {(g0, g1, g2)}")
-    vol = drr.density
-    if density is not None:   # the module keeps the geometry (affine, dims); the volume fitted through it is passed in
-        if not torch.is_tensor(density) or density.shape != vol.shape or density.device != vol.device:
-            got = f"{tuple(density.shape)} on {density.device}" if torch.is_tensor(density) else type(density).__name__
-            raise ValueError(f"density must be a tensor of drr.density's shape {tuple(vol.shape)} on its device {vol.device}, got "
-                             f"{got}")
-        vol = density
-    if density is None:
-        no_grad = ("render_deformed produces no volume gradient to drr.density: the density must not require grad (pass the volume "
-                   "to fit as density= instead)")
-    elif vol.dtype != torch.float32:
-        no_grad = (f"render_deformed produces no volume gradient to a {vol.dtype} density: 16-bit volumes are static densities "
-                   "(optimise an fp32 volume for volume gradients)")
-    else:
-        no_grad = None
+    vol, no_grad = _rendered_density(drr, density, "render_deformed",
+                                     "render_deformed produces no volume gradient to drr.density: the density must not require grad "
+                                     "(pass the volume to fit as density= instead)")
     _check_density(vol, "render_deformed", no_grad)
     if field.device != vol.device:
         raise ValueError(f"field must be on the density's device {vol.device}, not {field.device}")

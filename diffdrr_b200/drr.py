@@ -206,7 +206,7 @@ class DRR(nn.Module):
 
     def render_polyrigid(self, *args, motions, weights, parameterization: str = None, convention: str = None,
                          degrees: bool = False, calibration: RigidTransform = None, n_points: int = 500, alphamin=None,
-                         alphamax=None, blend: str = "linear", steps: int = 10, **kwargs):
+                         alphamax=None, blend: str = "linear", steps: int = 10, density=None, **kwargs):
         """Blended-rigid (skinned) DRR (DESIGN.md 6h, 6m) -> (B, 1, H, W): the volume deformed by K rigid motions that smooth weights
         blend into one continuous map, marched with the Trilinear renderer's rays and samples.
 
@@ -220,14 +220,24 @@ class DRR(nn.Module):
         or (B, K, 4, 4) world motions x -> X x as in render_structures (a tensor or a RigidTransform; it may require grad).
         weights: (K, g0, g1, g2) fp32 lattice over the volume with values in [0, 1] and sum_k <= 1, e.g. from
         polyrigid.polyrigid_weights; K <= 8.  The camera pose `*args`, calibration, n_points and alphamin / alphamax mean what they
-        do in forward.  Gradients reach the camera pose, the calibration and the motions; the density and the weights get none.
-        Supported: Trilinear with default options, fp32 / fp16 / bf16 densities, the full detector, p_subsample and patch_size;
-        anything else raises before any launch.  No host synchronisation once the lattice has been seen."""
+        do in forward.
+
+        density: a volume rendered in place of self.density (the reconstruction idiom: the module keeps the geometry, the fitted
+        volume is passed in), of self.density's shape and on its device (ValueError otherwise), fp32 / fp16 / bf16.  An fp32
+        density may require grad: for a fixed camera and fixed motions the render is linear in the density, and its gradient is
+        the render's transpose, a backprojection along the blended samples (blend="linear": DESIGN.md 6o; blend="log_euclidean":
+        render_deformed's, DESIGN.md 6l).  So one volume can be fitted to projections taken while structures move against each
+        other (a knee flexion series, a spine between positions), alone or jointly with the motions and the camera.
+
+        Gradients reach the camera pose, the calibration, the motions and a `density=` volume that requires grad; self.density
+        (it must not require grad) and the weights get none.  Supported: Trilinear with default options, fp32 / fp16 / bf16
+        densities, the full detector, p_subsample and patch_size; anything else raises before any launch.  No host
+        synchronisation once the lattice has been seen."""
         from .polyrigid import render_polyrigid
 
         return render_polyrigid(self, *args, motions=motions, weights=weights, parameterization=parameterization,
                                 convention=convention, degrees=degrees, calibration=calibration, n_points=n_points,
-                                alphamin=alphamin, alphamax=alphamax, blend=blend, steps=steps, **kwargs)
+                                alphamin=alphamin, alphamax=alphamax, blend=blend, steps=steps, density=density, **kwargs)
 
     def polyrigid_jacobian(self, *args, motions, weights, parameterization: str = None, convention: str = None,
                            degrees: bool = False, calibration: RigidTransform = None, n_points: int = 500, alphamin=None,

@@ -5,6 +5,9 @@ The rays and samples are the Trilinear renderer's.  Every sample x (voxel-index 
 X_k the world motion of structure k (meaning as in render_structures), A = drr.affine, w_k a coarse weight lattice over the volume
 with sum_k w_k <= 1 (the rest of the weight stays on the identity).  M is formed here with torch ops, so autograd carries the
 kernel's g_M (include/b200drr.h: b200drr_polyrigid_bwd) on to whatever parameterises the motions.
+
+A density passed as `density=` may require grad (fp32): its gradient is the forward's transpose in the density, a backprojection
+along the blended samples (b200drr_polyrigid_bproj; DESIGN.md 6o), for reconstruction under articulated motion.
 """
 from __future__ import annotations
 
@@ -14,7 +17,7 @@ import torch
 from torch.autograd.function import once_differentiable
 
 from . import _lib
-from .deform import _check_density, _check_renderer, _launch_args, _marches
+from .deform import _check_density, _check_renderer, _launch_args, _marches, _rendered_density
 from .renderers import _ptr, _stream, _vol_entry  # noqa: F401  (_vol_entry: the tests call the entry points through this module)
 from .structures import _batch_size, _label_tuple, _motion_matrices, _rigid_inverse, _translation, twist_matrix
 
@@ -84,8 +87,9 @@ def _packed_weights(drr, weights):
     return packed
 
 
-def check_supported(drr, args, parameterization, motions, weights, kwargs):
-    """Refuse, before any launch, what the blended-rigid render does not cover: -> (motion matrices, B, K)."""
+def check_supported(drr, args, parameterization, motions, weights, kwargs, density=None):
+    """Refuse, before any launch, what the blended-rigid render does not cover: -> (motion matrices, B, K).  density: the volume
+    rendered in place of drr.density (render_polyrigid's density=), or None."""
     _check_renderer(drr, "render_polyrigid", "the blended motion", kwargs)
     if not torch.is_tensor(weights) or weights.dim() != 4 or weights.dtype != torch.float32:
         got = f"{weights.dtype} {tuple(weights.shape)}" if torch.is_tensor(weights) else type(weights).__name__
@@ -97,8 +101,9 @@ def check_supported(drr, args, parameterization, motions, weights, kwargs):
         raise NotImplementedError("render_polyrigid produces no gradient for the blend weights: they must not require grad")
     B = _batch_size(args, parameterization)
     X = _motion_matrices(motions, K, B)
-    vol = drr.density
-    _check_density(vol, "render_polyrigid", "render_polyrigid produces no volume gradient: the density must not require grad")
+    vol, no_grad = _rendered_density(drr, density, "render_polyrigid",
+                                     "render_polyrigid produces no volume gradient: the density must not require grad")
+    _check_density(vol, "render_polyrigid", no_grad)
     if X.device != vol.device or weights.device != vol.device:
         raise ValueError(f"motions and weights must be on the density's device {vol.device}, not {X.device} and {weights.device}")
     return X, B, K
@@ -132,19 +137,28 @@ class _PolyrigidFunction(torch.autograd.Function):
         B, N = tgt.shape[0], tgt.shape[1]
         dev = vol.device
         gout = gout.reshape(B, N).contiguous().float()
+        lib = _lib.load()
+        g_vol = None
+        if ctx.needs_input_grad[0]:   # the forward's transpose in the density: a backprojection, no density read
+            g_vol = torch.empty(vol.shape, dtype=torch.float32, device=dev)
+            with torch.cuda.device(dev):
+                _lib.check(lib.b200drr_polyrigid_bproj(*vol.shape, _ptr(src), _ptr(tgt), _ptr(raylen), _ptr(M), M.shape[0],
+                                                       M.shape[1], _ptr(wpacked), *lattice, _ptr(gout), _ptr(g_vol), B, N, H, W,
+                                                       voxel_shift, eps, n_points, _ptr(arange), _stream()), "b200drr_polyrigid_bproj")
+        if not any(ctx.needs_input_grad[2:7]):   # a reconstruction step: the density is the only input that wants a gradient
+            return g_vol, None, None, None, None, None, None, None, None, None, None, None, None
         g_src = torch.empty(B, 3, dtype=torch.float32, device=dev)
         g_tgt = torch.empty(B, N, 3, dtype=torch.float32, device=dev)
         g_raylen = torch.empty(B, N, dtype=torch.float32, device=dev)
         g_M = torch.empty_like(M)
         g_range = torch.empty(2, dtype=torch.float32, device=dev)
-        lib = _lib.load()
         scratch = torch.empty(int(lib.b200drr_polyrigid_scratch_floats(B, N, H, W, M.shape[1])), dtype=torch.float32, device=dev)
         fn, head, name, _, _ = _launch_args("b200drr_polyrigid_bwd", vol, packed, src, tgt, raylen, (H, W))
         with torch.cuda.device(dev):
             _lib.check(fn(*head, *vol.shape, _ptr(src), _ptr(tgt), _ptr(raylen), _ptr(M), M.shape[0], M.shape[1], _ptr(wpacked),
                           *lattice, _ptr(gout), _ptr(g_src), _ptr(g_tgt), _ptr(g_raylen), _ptr(g_M), _ptr(g_range), _ptr(scratch),
                           B, N, H, W, voxel_shift, eps, n_points, _ptr(arange), _stream()), name)
-        return (None, None, g_src.view(source_shape), g_tgt, g_raylen.view(img_shape), g_M, g_range, None, None, None, None, None,
+        return (g_vol, None, g_src.view(source_shape), g_tgt, g_raylen.view(img_shape), g_M, g_range, None, None, None, None, None,
                 None)
 
 
@@ -157,7 +171,7 @@ def voxel_maps(drr, X):
 
 
 def render_polyrigid(drr, *args, motions, weights, parameterization=None, convention=None, degrees=False, calibration=None,
-                     n_points=500, alphamin=None, alphamax=None, blend="linear", steps=10, **kwargs):
+                     n_points=500, alphamin=None, alphamax=None, blend="linear", steps=10, density=None, **kwargs):
     """See DRR.render_polyrigid."""
     if blend not in ("linear", "log_euclidean"):
         raise ValueError(f"blend must be 'linear' or 'log_euclidean', got {blend!r}")
@@ -165,13 +179,13 @@ def render_polyrigid(drr, *args, motions, weights, parameterization=None, conven
         from . import svf
 
         svf.check_steps(steps)
-    X, B, K = check_supported(drr, args, parameterization, motions, weights, kwargs)
-    vol, r = drr.density, drr.renderer
+    X, B, K = check_supported(drr, args, parameterization, motions, weights, kwargs, density=density)
+    vol, r = drr.density if density is None else density, drr.renderer
     wpacked = _packed_weights(drr, weights)
     if blend == "log_euclidean":   # the lattice check above is the linear blend's; the packed copy is not used
         return svf.render_log_euclidean(drr, args, X, B, weights, steps, parameterization, convention, degrees, calibration,
-                                        n_points, alphamin, alphamax)
-    source, marches = _marches(drr, args, B, parameterization, convention, degrees, calibration, alphamin, alphamax)
+                                        n_points, alphamin, alphamax, vol)
+    source, marches = _marches(drr, args, B, parameterization, convention, degrees, calibration, alphamin, alphamax, vol=vol)
     M = voxel_maps(drr, X)
     M = M if M.dim() == 4 else M[None]
     packed = r._packed_volume(vol)

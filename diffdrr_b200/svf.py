@@ -202,8 +202,9 @@ def polyrigid_velocity(drr, X, weights):
 
 
 def render_log_euclidean(drr, args, X, B, weights, steps, parameterization, convention, degrees, calibration, n_points, alphamin,
-                         alphamax):
-    """render_polyrigid(blend="log_euclidean") after its checks: exp of polyrigid_velocity, marched by render_deformed."""
+                         alphamax, vol):
+    """render_polyrigid(blend="log_euclidean") after its checks: exp of polyrigid_velocity, marched by render_deformed through the
+    density vol (drr.density, or render_polyrigid's density=, whose gradient is then b200drr_deform_bproj's)."""
     U = _SquaringFunction.apply(polyrigid_velocity(drr, X, weights), steps, tuple(drr.density.shape))
     return render_voxel_field(drr, args, B, U, parameterization, convention, degrees, calibration, n_points, alphamin, alphamax,
-                              drr.density)
+                              vol)

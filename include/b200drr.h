@@ -698,7 +698,8 @@ int b200drr_trilinear_fwd_sens_pose_v16(const void *packed, int vol_type, int D0
  *
  * b200drr_polyrigid_bwd: gradients of sum(gout * out), every output OVERWRITTEN and NULL where not wanted: g_src [B][3],
  * g_tgt [B][N][3], g_raylen [B][N], g_M [Bm][K][12], g_alpha_range [2] (the partials w.r.t. alpha_range, as
- * b200drr_trilinear_bwd's).  No volume and no weight gradient.  scratch: b200drr_polyrigid_scratch_floats(B, N, H, W, K) floats;
+ * b200drr_trilinear_bwd's).  No weight gradient; the volume gradient is b200drr_polyrigid_bproj's.
+ * scratch: b200drr_polyrigid_scratch_floats(B, N, H, W, K) floats;
  * the sums over rays are taken from it in a fixed order, so repeated calls return identical bits.  The library allocates
  * nothing.  The _v16 twins read a 16-bit volume (vol_type as above; `packed` from b200drr_pack_corners_v16) and equal the fp32
  * call on the up-cast volume.
@@ -724,6 +725,22 @@ int b200drr_polyrigid_bwd_v16(const void *vol, const void *packed, int vol_type,
                               int g1, int g2, const float *gout, float *g_src, float *g_tgt, float *g_raylen, float *g_M,
                               float *g_alpha_range, float *scratch, int B, int64_t N, int H, int W, float voxel_shift, float eps,
                               int n_points, const float *alpha_range, void *stream);
+
+/*
+ * Backprojection through the blended-rigid render (DESIGN.md 6o): the transpose of b200drr_polyrigid_fwd in the density, for
+ * reconstruction under known (or jointly fitted) articulated motion.  For a fixed camera and fixed maps the render is linear in V:
+ *     out = raylen * step * sum_m tri(V, y_m),      y_m = x_m + sum_k w_k(x_m) (M_k [x_m; 1] - x_m),
+ * so the gradient of sum(gout * out) with respect to V is
+ *     g_vol[corner] = sum over rays and samples of gout * raylen * step * tri_weight(corner, y_m),
+ * over every y_m inside the padded volume.  The samples, the maps, the packed lattice `wpacked` and the range are
+ * b200drr_polyrigid_fwd's; no density is read, so there is no volume argument and no _v16 twin.  gout [B][N]; g_vol [D0][D1][D2],
+ * OVERWRITTEN: the entry zeroes it on the stream, then every pose (shared or per-pose maps) adds into it with scalar atomics, so
+ * it repeats only to fp32 reordering.  A NULL gout or g_vol returns B200DRR_EINVAL, and the geometry, lattice and map checks are
+ * b200drr_polyrigid_fwd's (with the same return codes), all before touching CUDA.  The library allocates nothing.
+ */
+int b200drr_polyrigid_bproj(int D0, int D1, int D2, const float *src, const float *tgt, const float *raylen, const float *M, int Bm,
+                            int K, const float *wpacked, int g0, int g1, int g2, const float *gout, float *g_vol, int B, int64_t N,
+                            int H, int W, float voxel_shift, float eps, int n_points, const float *alpha_range, void *stream);
 
 /*
  * Per-pixel motion Jacobian of the blended-rigid render (DESIGN.md 6j), for Gauss-Newton / Levenberg-Marquardt on the motions.

@@ -190,4 +190,24 @@ for shape in ((rot.shape[0], 3, 7, 5, 9), (3, 7, 5, 9)):
     E = lm.step()
     torch.cuda.synchronize()
     print("svf_jvp", shape, "ok", float(du.abs().max()), E.tolist())
+# blended-rigid density backprojection (polyrigid.cu: polyrigid_bproj_kernel): the 23 x 23 detector (partial 16 x 8 tiles),
+# p_subsample (128-ray chunks) and patches, K = 3 and 6 (both channel paddings), per-pose and shared motions, a structure pulled
+# from outside the volume, the density alone and jointly with the motions
+for kw in (dict(), dict(p_subsample=0.37), dict(patch_size=8, height=24)):
+    kw = dict(kw)
+    drr = DRR(synthetic.make_subject(vol), **synthetic.detector_kwargs(kw.pop("height", 23)), renderer="trilinear", **kw).to(dev)
+    for K in (3, 6):
+        W = torch.rand(K, 7, 5, 9, device=dev) / K
+        for shape in ((rot.shape[0], K, 6), (K, 6)):
+            for joint in (False, True):
+                xi = (torch.rand(*shape, device=dev) - 0.5) * torch.tensor([0.1, 0.1, 0.1, 8.0, 8.0, 8.0], device=dev)
+                xi[..., 0, 3] += 300.0
+                xi.requires_grad_(joint)
+                V = drr.density.detach().clone().requires_grad_(True)
+                r, x = (t.detach().clone().requires_grad_(joint) for t in (rot, xyz))
+                img = drr.render_polyrigid(r, x, motions=se3_exp(xi), weights=W, n_points=64, density=V,
+                                           parameterization="euler_angles", convention="ZXY")
+                img.sum().backward()
+                torch.cuda.synchronize()
+                print("polyrigid_bproj", kw, K, shape, joint, "ok", float(img.sum()), float(V.grad.abs().max()))
 print("done")

@@ -286,6 +286,11 @@ _SIGNATURES = {
         _c_float_p, _c_float_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, _c_float_p, _c_float_p, _c_float_p, _c_float_p,
         ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, _c_float_p, _c_float_p, _c_float_p, ctypes.c_int, ctypes.c_int64,
         ctypes.c_int, ctypes.c_int, ctypes.c_float, ctypes.c_float, ctypes.c_int, _c_float_p, ctypes.c_void_p]),
+    "b200drr_deform_jac": (ctypes.c_int, [
+        _c_float_p, _c_float_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, _c_float_p, _c_float_p, _c_float_p, _c_float_p,
+        ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, _c_float_p, ctypes.c_int, ctypes.c_int, _c_float_p, _c_float_p,
+        ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_float, ctypes.c_float, ctypes.c_int, _c_float_p,
+        ctypes.c_void_p]),
     "b200drr_deform_bproj": (ctypes.c_int, [
         ctypes.c_int, ctypes.c_int, ctypes.c_int, _c_float_p, _c_float_p, _c_float_p, _c_float_p, ctypes.c_int, ctypes.c_int,
         ctypes.c_int, ctypes.c_int, _c_float_p, _c_float_p, ctypes.c_int, ctypes.c_int64, ctypes.c_int, ctypes.c_int, ctypes.c_float,
@@ -300,6 +305,9 @@ _SIGNATURES = {
     "b200drr_svf_square_jvp": (ctypes.c_int, [
         _c_float_p, _c_float_p, _c_float_p, _c_float_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int,
         ctypes.c_int, ctypes.c_int, ctypes.c_float, ctypes.c_void_p]),
+    "b200drr_svf_square_tangents": (ctypes.c_int, [
+        _c_float_p, _c_float_p, _c_float_p, _c_float_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int,
+        ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_float, ctypes.c_void_p]),
 }
 
 
@@ -317,7 +325,8 @@ _SIGNATURES.update({f"{name}_v16": _v16(name) for name in (
     "b200drr_siddon_fwd_pose", "b200drr_siddon_fwd_sens_pose", "b200drr_siddon_fwd_sens_structures", "b200drr_pack_corners",
     "b200drr_trilinear_fwd", "b200drr_trilinear_fwd_grid", "b200drr_trilinear_fwd_sens", "b200drr_trilinear_fwd_packed",
     "b200drr_trilinear_fwd_sens_packed", "b200drr_trilinear_fwd_sens_pose", "b200drr_polyrigid_fwd", "b200drr_polyrigid_bwd",
-    "b200drr_polyrigid_jac", "b200drr_deform_fwd", "b200drr_deform_bwd", "b200drr_deform_jvp")})
+    "b200drr_polyrigid_jac", "b200drr_deform_fwd", "b200drr_deform_bwd", "b200drr_deform_jvp",
+    "b200drr_deform_jac")})
 
 # entry points of rejected experiments (include/b200drr_experimental.h): bound only when the experimental build is loaded
 _EXPERIMENTAL_SIGNATURES = {

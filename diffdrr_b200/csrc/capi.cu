@@ -1252,6 +1252,22 @@ int deform_jvp(const void* vol, const void* packed, int vol_type, int D0, int D1
     return ret(launch_deform_jvp(vol, packed, vol_type, mk(D0, D1, D2), src, tgt, raylen, field, Bf, g0, g1, g2, tangent, img, jv, B, N,
                                  W, voxel_shift, eps, n_points, alpha_range, (cudaStream_t)stream));
 }
+
+int deform_jac(const void* vol, const void* packed, int vol_type, int D0, int D1, int D2, const float* src, const float* tgt,
+               const float* raylen, const float* field, int Bf, int g0, int g1, int g2, const float* tangents, int P, int K, float* img,
+               float* J, int32_t* rects, int B, int H, int W, float voxel_shift, float eps, int n_points, const float* alpha_range,
+               void* stream)
+{
+    if (!tangents || !img || !J || !rects || H <= 0 || W <= 0 || P < 1 || P > 48 || P != 6 * K ||
+        ((uintptr_t)tangents & 15u) != 0 || (const float*)img == tangents || (const float*)J == tangents)
+        return B200DRR_EINVAL;
+    if (K > 8 || (int64_t)g0 * g1 * g2 * 4 * P >= (int64_t)INT32_MAX) return B200DRR_EUNSUPPORTED;
+    if (const int bad = deform_bad(vol, packed, D0, D1, D2, src, tgt, raylen, field, Bf, g0, g1, g2, B, (int64_t)H * W, H, W, n_points,
+                                   alpha_range))
+        return bad;
+    return ret(launch_deform_jac(vol, packed, vol_type, mk(D0, D1, D2), src, tgt, raylen, field, Bf, g0, g1, g2, tangents, K, img, J,
+                                 rects, B, H, W, voxel_shift, eps, n_points, alpha_range, (cudaStream_t)stream));
+}
 }  // namespace
 
 int64_t b200drr_deform_scratch_floats(int B, int64_t N, int H, int W)
@@ -1315,6 +1331,25 @@ int b200drr_deform_jvp_v16(const void* vol, const void* packed, int vol_type, in
                       voxel_shift, eps, n_points, alpha_range, stream);
 }
 
+int b200drr_deform_jac(const float* vol, const float* packed, int D0, int D1, int D2, const float* src, const float* tgt,
+                       const float* raylen, const float* field, int Bf, int g0, int g1, int g2, const float* tangents, int P, int K,
+                       float* img, float* J, int32_t* rects, int B, int H, int W, float voxel_shift, float eps, int n_points,
+                       const float* alpha_range, void* stream)
+{
+    return deform_jac(vol, packed, 0, D0, D1, D2, src, tgt, raylen, field, Bf, g0, g1, g2, tangents, P, K, img, J, rects, B, H, W,
+                      voxel_shift, eps, n_points, alpha_range, stream);
+}
+
+int b200drr_deform_jac_v16(const void* vol, const void* packed, int vol_type, int D0, int D1, int D2, const float* src, const float* tgt,
+                           const float* raylen, const float* field, int Bf, int g0, int g1, int g2, const float* tangents, int P, int K,
+                           float* img, float* J, int32_t* rects, int B, int H, int W, float voxel_shift, float eps, int n_points,
+                           const float* alpha_range, void* stream)
+{
+    if (bad_vol16(vol_type)) return B200DRR_EINVAL;
+    return deform_jac(vol, packed, vol_type, D0, D1, D2, src, tgt, raylen, field, Bf, g0, g1, g2, tangents, P, K, img, J, rects, B, H, W,
+                      voxel_shift, eps, n_points, alpha_range, stream);
+}
+
 int b200drr_deform_bproj(int D0, int D1, int D2, const float* src, const float* tgt, const float* raylen, const float* field, int Bf,
                          int g0, int g1, int g2, const float* gout, float* g_vol, int B, int64_t N, int H, int W, float voxel_shift,
                          float eps, int n_points, const float* alpha_range, void* stream)
@@ -1362,6 +1397,16 @@ int b200drr_svf_square_jvp(const float* field, const float* tangent, float* tout
     if (const int bad = svf_bad(field, tout, Bf, g0, g1, g2, D0, D1, D2, scale)) return bad;
     if (tout == field || tout == tangent || out == field || out == tangent || out == tout) return B200DRR_EINVAL;
     return ret(launch_svf_square_jvp(field, tangent, tout, out, Bf, g0, g1, g2, mk(D0, D1, D2), scale, (cudaStream_t)stream));
+}
+
+int b200drr_svf_square_tangents(const float* field, const float* tangents, float* tout, float* out, int Bf, int P, int g0, int g1, int g2,
+                                int D0, int D1, int D2, float scale, void* stream)
+{
+    if (!tangents || P < 1 || P > 48 || (((uintptr_t)tangents | (uintptr_t)out) & 15u) != 0) return B200DRR_EINVAL;
+    if (const int bad = svf_bad(field, tout, Bf, g0, g1, g2, D0, D1, D2, scale)) return bad;
+    if (tout == field || tout == tangents || out == field || out == tangents || out == tout) return B200DRR_EINVAL;
+    if ((int64_t)g0 * g1 * g2 * 4 * P >= (int64_t)INT32_MAX) return B200DRR_EUNSUPPORTED;
+    return ret(launch_svf_square_tangents(field, tangents, tout, out, Bf, P, g0, g1, g2, mk(D0, D1, D2), scale, (cudaStream_t)stream));
 }
 
 #ifdef B200DRR_EXPERIMENTS

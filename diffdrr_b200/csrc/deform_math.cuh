@@ -10,6 +10,7 @@
 // The backward scatters d I / d u into a lattice gradient with one vector reduction per lattice node and flush (deform_red4): the
 // field gradient repeats only to fp32 reordering of those adds.  Every other output is a per-ray value.  The tangent march
 // (deform_ray_jvp) is the scatter's transpose: the image's derivative along a field direction, one value per ray.  The
+// Jacobian march (deform_ray_jac) takes the transpose of that scatter for 6K tangents at once.  The
 // backprojection (deform_ray_bproj) is the forward's transpose in the density: 8 scalar reductions per in-volume sample into a
 // volume gradient, with no density read.
 #pragma once
@@ -212,6 +213,97 @@ B200_HD float deform_ray_jvp(const Gather& gather, const VolDims& dims, const Po
     }
     img = acc;
     return jv;
+}
+
+// Contracts the register accumulator of deform_ray_jac with the tangents at the in-lattice corners of the cell with lower node `cell`:
+// Jp[p] += sum_c <acc[c], t_p(c)> for p < 6K, tan = this pose's tangents [g0][g1][g2][6K] float4 (lane 3 ignored), and sets bit k of
+// touched when one of structure k's six tangents is nonzero at such a corner.  cell[0] < -1: nothing held.
+template <int KP>
+B200_HD int deform_jac_flush(const PolyLattice& lat, const float4* tan, int K, const int cell[3], const float acc[8][3],
+                             float Jp[KP * 6], unsigned& touched)
+{
+    if (cell[0] < -1) return 0;
+    const int P = 6 * K;
+#pragma unroll
+    for (int c = 0; c < 8; ++c) {
+        const int x = cell[0] + (c & 1), y = cell[1] + ((c >> 1) & 1), z = cell[2] + ((c >> 2) & 1);
+        if (!((unsigned)x < (unsigned)lat.g[0] && (unsigned)y < (unsigned)lat.g[1] && (unsigned)z < (unsigned)lat.g[2])) continue;
+        const float4* t = tan + (int64_t)((x * lat.g[1] + y) * lat.g[2] + z) * P;
+#pragma unroll
+        for (int p = 0; p < KP * 6; ++p) {
+            if (p >= P) break;
+            const float4 v = ldg4(t + p);
+            Jp[p] = fmaf(acc[c][0], v.x, fmaf(acc[c][1], v.y, fmaf(acc[c][2], v.z, Jp[p])));
+            if (v.x != 0.0f || v.y != 0.0f || v.z != 0.0f) touched |= 1u << (p / 6);
+        }
+    }
+    return 1;
+}
+
+// Per-pixel Jacobian of one ray along the 6K field tangents of K structures' motions (DESIGN.md 6p): deform_ray_jvp's samples,
+// through the same arithmetic, for all 6K tangents at once,
+//   Jp[p] = sum_m G_m . t_p(x_m),      G_m = grad tri(V)(y_m),
+// over exactly the samples where deform_ray_jvp adds.  t_p is not interpolated per sample: as deform_ray_bwd's field scatter,
+// acc[c] += w_c(x_m) G_m is summed in 8 x 3 registers while consecutive samples stay in one lattice cell, and contracted with the
+// tangents at the cell's corners when the cell changes and at the end (deform_jac_flush), so sum_n gout_n L step Jp_n is <g_field
+// of deform_ray_bwd, t_p> to fp32 reordering.  touched: bit k set when a contraction met a nonzero tangent of structure k.
+// -> deform_ray_fwd's sum bit for bit.  Multiply it and Jp by raylen * step outside.  flushes: the contractions made.
+template <int KP, class Gather>
+B200_HD float deform_ray_jac(const Gather& gather, const VolDims& dims, const PolyLattice& lat, const float4* tan, int K, const Ray& ray,
+                             float shift, int P, float amin, float amax, float Jp[KP * 6], unsigned& touched, int& flushes)
+{
+    const PixLine pl = make_pixline(ray, dims, shift, 0);
+    const float range = amax - amin;
+    const float lstep = 1.0f / (float)(P - 1);
+    int m_lo, m_hi;
+    poly_sample_range(pl, lat, amin, range, P, m_lo, m_hi);
+    float img = 0.0f, acc[8][3];
+    int cell[3] = {-2, 0, 0};
+#pragma unroll
+    for (int c = 0; c < 8; ++c)
+#pragma unroll
+        for (int a = 0; a < 3; ++a) acc[c][a] = 0.0f;
+#pragma unroll
+    for (int p = 0; p < KP * 6; ++p) Jp[p] = 0.0f;
+    touched = 0u;
+    flushes = 0;
+    for (int m = m_lo; m <= m_hi; ++m) {
+        const float alpha = add_rn(mul_rn(linspace01(m, P, lstep), range), amin);
+        float pix[3], u[4], f[3];
+        int i0[3];
+#pragma unroll
+        for (int a = 0; a < 3; ++a) pix[a] = fmaf(alpha, pl.dp[a], pl.p0[a]);
+        const bool moved = poly_weights<4, false>(lat, pix, u, nullptr);
+        if (moved) {
+            deform_cell(lat, pix, i0, f);
+#pragma unroll
+            for (int a = 0; a < 3; ++a) pix[a] += u[a];
+        }
+        if (!inside_padded(pix, dims)) continue;
+        const Corner8 c8 = gather(dims, pix);
+        img += lerp8(c8);
+        if (!moved) continue;
+        float val, G[3];
+        tri_value_grad(c8.v, c8.f, val, G);
+        if (i0[0] != cell[0] || i0[1] != cell[1] || i0[2] != cell[2]) {
+            flushes += deform_jac_flush<KP>(lat, tan, K, cell, acc, Jp, touched);
+#pragma unroll
+            for (int a = 0; a < 3; ++a) cell[a] = i0[a];
+#pragma unroll
+            for (int c = 0; c < 8; ++c)
+#pragma unroll
+                for (int a = 0; a < 3; ++a) acc[c][a] = 0.0f;
+        }
+        const float e[3] = {1.0f - f[0], 1.0f - f[1], 1.0f - f[2]};
+#pragma unroll
+        for (int c = 0; c < 8; ++c) {
+            const float w = ((c & 1) ? f[0] : e[0]) * ((c & 2) ? f[1] : e[1]) * ((c & 4) ? f[2] : e[2]);
+#pragma unroll
+            for (int a = 0; a < 3; ++a) acc[c][a] = fmaf(w, G[a], acc[c][a]);
+        }
+    }
+    flushes += deform_jac_flush<KP>(lat, tan, K, cell, acc, Jp, touched);
+    return img;
 }
 
 // Transpose of deform_ray_fwd in the density (DESIGN.md 6l): deform_ray_fwd's samples, through the same arithmetic, each adding

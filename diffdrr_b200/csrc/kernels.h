@@ -307,6 +307,9 @@ __global__ void __launch_bounds__(256) polyrigid_finish_kernel(const float* __re
                                                                int K, float* __restrict__ g_M, float* __restrict__ g_src,
                                                                float* __restrict__ g_alpha_range);
 
+// every rectangle of polyrigid_jac's footprint format empty, {W, -1, H, -1}; deform.cu launches it too
+__global__ void __launch_bounds__(256) polyrigid_rects_empty_kernel(int* __restrict__ rects, int n, int H, int W);
+
 // deformable (dense displacement field) trilinear render (deform.cu).  Arguments as the polyrigid ones; field: [Bf][g0][g1][g2][4]
 // voxel-index displacements, lane 3 zero; g_field: the same layout, zeroed here before the scatter.
 int64_t deform_scratch_floats(int B, int64_t N, int W);
@@ -322,6 +325,12 @@ cudaError_t launch_deform_jvp(const void* vol, const void* packed, int vol_type,
                               const float* raylen, const float* field, int Bf, int g0, int g1, int g2, const float* tangent, float* img,
                               float* jv, int B, int64_t N, int W, float shift, float eps, int n_points, const float* alpha_range,
                               cudaStream_t stream);
+// per-pixel Jacobian along P = 6K field tangents [Bf][g0][g1][g2][P][4] on a full H x W grid: img [B][H*W] (the forward's),
+// J [B][K][H*W][6], rects [B][K][4] (set empty first)
+cudaError_t launch_deform_jac(const void* vol, const void* packed, int vol_type, VolDims dims, const float* src, const float* tgt,
+                              const float* raylen, const float* field, int Bf, int g0, int g1, int g2, const float* tangents, int K,
+                              float* img, float* J, int* rects, int B, int H, int W, float shift, float eps, int n_points,
+                              const float* alpha_range, cudaStream_t stream);
 // the forward's transpose in the density: g_vol [D0][D1][D2], zeroed here, += sum over the rays of gout * d out / d V
 cudaError_t launch_deform_bproj(VolDims dims, const float* src, const float* tgt, const float* raylen, const float* field, int Bf, int g0,
                                 int g1, int g2, const float* gout, float* g_vol, int B, int64_t N, int W, float shift, float eps,
@@ -336,5 +345,8 @@ cudaError_t launch_svf_square_bwd(const float* field, const float* gout, float* 
 // tout = the step's tangent along `tangent` (same layout); out (may be null) = the step itself, launch_svf_square's out bit for bit
 cudaError_t launch_svf_square_jvp(const float* field, const float* tangent, float* tout, float* out, int Bf, int g0, int g1, int g2,
                                   VolDims dims, float scale, cudaStream_t stream);
+// the step's tangents along P tangents at once, node-major [Bf][g0][g1][g2][P][4] in tangents and tout; out (may be null) as above
+cudaError_t launch_svf_square_tangents(const float* field, const float* tangents, float* tout, float* out, int Bf, int P, int g0, int g1,
+                                       int g2, VolDims dims, float scale, cudaStream_t stream);
 
 }  // namespace b200drr

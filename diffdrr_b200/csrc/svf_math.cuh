@@ -142,4 +142,47 @@ B200_HD float4 svf_square_node_jvp(const PolyLattice& lat_u, const PolyLattice& 
     return r;
 }
 
+// svf_square_node_jvp for P tangents at once (DESIGN.md 6p).  tan: this pose's tangents, node-major [g0][g1][g2][P] float4; tout
+// receives node x's P results [P] float4.  y, its cell and J_U depend only on u, so they are formed once per node; the per-tangent
+// arithmetic is svf_square_node_jvp's in the same order, so slice p equals that function on tangent p bit for bit.  out_u as there.
+B200_HD void svf_square_node_tangents(const PolyLattice& lat_u, const float4* tan, int P, const int node[3], float s, float4* tout,
+                                      float4* out_u)
+{
+    const int64_t x = svf_node(lat_u, node[0], node[1], node[2]);
+    const float4 u = ldg4(lat_u.w + x);
+    float q[3], U[3], J[3][3];
+    svf_target(lat_u, node, u, s, q);
+    const SvfCell c = svf_cell(lat_u, q);
+    svf_lookup<true>(lat_u, c, U, J);
+    if (out_u) *out_u = svf_square_node(lat_u, node, s);
+    int64_t corner[8];
+#pragma unroll
+    for (int k = 0; k < 8; ++k)
+        corner[k] = svf_node(lat_u, (k & 1) ? c.i1[0] : c.i0[0], (k & 2) ? c.i1[1] : c.i0[1], (k & 4) ? c.i1[2] : c.i0[2]) * P;
+    const float ss = s * s;
+    for (int p = 0; p < P; ++p) {
+        const float4 tx = ldg4(tan + x * P + p);
+        float v[3][8], T[3], G[3];
+#pragma unroll
+        for (int k = 0; k < 8; ++k) {
+            const float4 t = ldg4(tan + corner[k] + p);
+            v[0][k] = t.x;
+            v[1][k] = t.y;
+            v[2][k] = t.z;
+        }
+#pragma unroll
+        for (int i = 0; i < 3; ++i) tri_value_grad(v[i], c.f, T[i], G);
+        const float t[3] = {tx.x, tx.y, tx.z};
+        float o[3];
+#pragma unroll
+        for (int i = 0; i < 3; ++i) o[i] = fmaf(ss, fmaf(J[i][0], t[0], fmaf(J[i][1], t[1], J[i][2] * t[2])), s * (t[i] + T[i]));
+        float4 r;
+        r.x = o[0];
+        r.y = o[1];
+        r.z = o[2];
+        r.w = 0.0f;
+        tout[p] = r;
+    }
+}
+
 }  // namespace b200drr

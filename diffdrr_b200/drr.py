@@ -241,19 +241,26 @@ class DRR(nn.Module):
 
     def polyrigid_jacobian(self, *args, motions, weights, parameterization: str = None, convention: str = None,
                            degrees: bool = False, calibration: RigidTransform = None, n_points: int = 500, alphamin=None,
-                           alphamax=None, return_footprints: bool = False, **kwargs):
+                           alphamax=None, return_footprints: bool = False, blend: str = "linear", steps: int = 10, **kwargs):
         """(img, J): the render_polyrigid image (B, 1, H, W), bit for bit, and its per-pixel Jacobian J (B, K, H, W, 6) with
         respect to the increment xi_k = (omega, v) of each motion (DESIGN.md 6j), from one march.  xi_k is a left increment about
         the pivot c_k in world coordinates, X_k(xi) = T(c_k) exp(xi^) T(-c_k) X_k, c_k the weight-weighted centroid of channel k of
         the lattice (polyrigid.polyrigid_pivots).  Columns: the rotation's three, then the translation's three.  return_footprints
         adds rects (B, K, 4) int32 {w0, w1, h0, h1}: J[:, k] is zero outside rectangle k.  Arguments as in render_polyrigid; the
         same set is supported except p_subsample and patch_size, and anything else raises before any launch.  Detached results;
-        no host sync once the lattice has been seen."""
+        no host sync once the lattice has been seen.
+
+        blend="log_euclidean" (DESIGN.md 6p): the Jacobian of render_polyrigid(blend="log_euclidean", steps=steps), whose image it
+        returns bit for bit.  The 6K velocity tangents are pushed through the `steps` squarings together and contracted in one
+        march; rectangle k then bounds the pixels the exponential's spread of structure k's tangents reaches, wider than the
+        support of w_k.  It holds two tangent fields of Bm * g0 * g1 * g2 * 6K * 16 bytes (201 MB at 64^3 with K = 8 and shared
+        motions)."""
         from .polyrigid import polyrigid_jacobian
 
         return polyrigid_jacobian(self, *args, motions=motions, weights=weights, parameterization=parameterization,
                                   convention=convention, degrees=degrees, calibration=calibration, n_points=n_points,
-                                  alphamin=alphamin, alphamax=alphamax, return_footprints=return_footprints, **kwargs)
+                                  alphamin=alphamin, alphamax=alphamax, return_footprints=return_footprints, blend=blend,
+                                  steps=steps, **kwargs)
 
     def render_deformed(self, *args, field, parameterization: str = None, convention: str = None, degrees: bool = False,
                         calibration: RigidTransform = None, n_points: int = 500, alphamin=None, alphamax=None, density=None,

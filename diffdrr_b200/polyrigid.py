@@ -229,13 +229,22 @@ def polyrigid_tangents(drr, X, pivots):
 
 
 def polyrigid_jacobian(drr, *args, motions, weights, parameterization=None, convention=None, degrees=False, calibration=None,
-                       n_points=500, alphamin=None, alphamax=None, return_footprints=False, **kwargs):
+                       n_points=500, alphamin=None, alphamax=None, return_footprints=False, blend="linear", steps=10, **kwargs):
     """See DRR.polyrigid_jacobian."""
+    if blend not in ("linear", "log_euclidean"):
+        raise ValueError(f"blend must be 'linear' or 'log_euclidean', got {blend!r}")
+    if blend == "log_euclidean":
+        from . import svf
+
+        svf.check_steps(steps)
     det = drr.detector
     if det.n_subsample is not None or drr.patch_size is not None:
         raise NotImplementedError("polyrigid_jacobian covers the full detector only, not p_subsample or patch_size: the Jacobian "
                                   "kernel marches full H x W grids")
     X, B, K = check_supported(drr, args, parameterization, motions, weights, kwargs)
+    if blend == "log_euclidean":
+        return _log_euclidean_jacobian(drr, args, X, B, K, weights, steps, parameterization, convention, degrees, calibration,
+                                       n_points, alphamin, alphamax, return_footprints)
     vol, r = drr.density, drr.renderer
     H, W = det.height, det.width
     with torch.no_grad():
@@ -255,6 +264,38 @@ def polyrigid_jacobian(drr, *args, motions, weights, parameterization=None, conv
             _lib.check(fn(*head, *vol.shape, _ptr(src), _ptr(tgt), _ptr(raylen), _ptr(M), M.shape[0], K, _ptr(wpacked),
                           *weights.shape[1:], _ptr(T), _ptr(img), _ptr(J), _ptr(rects), B, H, W, float(r.voxel_shift), float(r.eps),
                           int(n_points), _ptr(arange), _stream()), name)
+    img = drr.reshape_transform(img.view(B, 1, H * W), batch_size=B)
+    J = J.view(B, K, H, W, 6)
+    return (img, J, rects) if return_footprints else (img, J)
+
+
+def _log_euclidean_jacobian(drr, args, X, B, K, weights, steps, parameterization, convention, degrees, calibration, n_points, alphamin,
+                            alphamax, return_footprints):
+    """polyrigid_jacobian(blend="log_euclidean") after its checks (DESIGN.md 6p): the velocity and its 6K tangents, the squarings
+    of the velocity (svf.square_chain, as render_polyrigid takes them) and of the tangents over its levels
+    (svf.square_chain_tangents), then one b200drr_deform_jac march of exp(v) contracting the 6K tangents of exp(v)."""
+    from . import svf
+
+    vol, r = drr.density, drr.renderer
+    H, W = drr.detector.height, drr.detector.width
+    dims = tuple(vol.shape)
+    with torch.no_grad():
+        _packed_weights(drr, weights)   # render_polyrigid's lattice check
+        levels, U = svf.square_chain(svf.polyrigid_velocity(drr, X, weights), steps, dims)
+        T = svf.square_chain_tangents(levels, svf.velocity_tangents(drr, X, weights, polyrigid_pivots(drr, weights)), dims)
+        del levels
+        source, [(target, raylen, arange, grid)] = _marches(drr, args, B, parameterization, convention, degrees, calibration,
+                                                            alphamin, alphamax)
+        packed = r._packed_volume(vol)
+        volc = vol.contiguous()
+        fn, head, name, (src, tgt, raylen), _ = _launch_args("b200drr_deform_jac", volc, packed, source, target, raylen, grid)
+        img = torch.empty(B, H * W, dtype=torch.float32, device=vol.device)
+        J = torch.empty(B, K, H * W, 6, dtype=torch.float32, device=vol.device)
+        rects = torch.empty(B, K, 4, dtype=torch.int32, device=vol.device)
+        with torch.cuda.device(vol.device):
+            _lib.check(fn(*head, *vol.shape, _ptr(src), _ptr(tgt), _ptr(raylen), _ptr(U), U.shape[0], *U.shape[1:4], _ptr(T), 6 * K, K,
+                          _ptr(img), _ptr(J), _ptr(rects), B, H, W, float(r.voxel_shift), float(r.eps), int(n_points), _ptr(arange),
+                          _stream()), name)
     img = drr.reshape_transform(img.view(B, 1, H * W), batch_size=B)
     J = J.view(B, K, H, W, 6)
     return (img, J, rects) if return_footprints else (img, J)

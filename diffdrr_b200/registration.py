@@ -351,18 +351,29 @@ class PolyrigidLevenbergMarquardt(_MotionLevenbergMarquardt):
     (one march: the image, the per-pixel columns of every motion and their footprints), the trial render render_polyrigid's, and
     the pivot c_k the weight-weighted centroid of channel k's lattice (polyrigid.polyrigid_pivots).  The sampling range is
     Trilinear's batch-global one unless alphamin / alphamax fix it; its dependence on the motions is nil (the rays do not move),
-    so the model is the image's full derivative.  Full detectors only.  No host sync once the lattice has been seen."""
+    so the model is the image's full derivative.  Full detectors only.  No host sync once the lattice has been seen.
+
+    blend / steps are render_polyrigid's: with blend="log_euclidean" the Jacobian is that of the exponential's render (DESIGN.md
+    6p: the 6K motion tangents through the `steps` squarings and one march) and the trial render render_polyrigid(blend=
+    "log_euclidean", steps=steps).  A blend other than the two or a bad steps raises ValueError here."""
 
     def __init__(self, drr, rot: torch.Tensor, xyz: torch.Tensor, motions: torch.Tensor, weights: torch.Tensor, target: torch.Tensor,
                  parameterization: str = "euler_angles", convention: str | None = None, degrees: bool = False, calibration=None,
-                 n_points: int = 500, alphamin=None, alphamax=None, loss=None, damping: float = 1e-3, eps: float = 1e-5):
+                 n_points: int = 500, alphamin=None, alphamax=None, loss=None, damping: float = 1e-3, eps: float = 1e-5,
+                 blend: str = "linear", steps: int = 10):
         from .polyrigid import check_supported, polyrigid_pivots
 
+        if blend not in ("linear", "log_euclidean"):
+            raise ValueError(f"blend must be 'linear' or 'log_euclidean', got {blend!r}")
+        if blend == "log_euclidean":
+            from .svf import check_steps
+
+            check_steps(steps)
         super().__init__(drr, rot, xyz, motions, target, parameterization, loss, damping, eps,
                          lambda: check_supported(drr, (rot, xyz), parameterization, motions, weights, {}), full_detector=True)
         self.weights = weights
         self.kw = dict(parameterization=parameterization, convention=convention, degrees=degrees, calibration=calibration,
-                       n_points=n_points, alphamin=alphamin, alphamax=alphamax)
+                       n_points=n_points, alphamin=alphamin, alphamax=alphamax, blend=blend, steps=steps)
         self.pivots = polyrigid_pivots(drr, weights)
 
     def _jacobian(self, X):

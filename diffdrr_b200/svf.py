@@ -201,6 +201,54 @@ def polyrigid_velocity(drr, X, weights):
     return torch.nn.functional.pad(v.view(L.shape[0], *g, 3), (0, 1)).contiguous()
 
 
+def square_chain_tangents(levels, T, dims):
+    """P tangents T (Bm, g0, g1, g2, P, 4), voxel units, node-major, pushed through the squarings over square_chain's levels (read
+    as they are, so the primal is not recomputed), one b200drr_svf_square_tangents per step -> the P tangents of exp(U) in the
+    same layout.  Slice p is square_chain_jvp(levels, T[..., p, :], dims)[1] bit for bit.  Two tangent fields live at a time.  No
+    autograd."""
+    steps = len(levels)
+    T = _aligned(T)
+    Bm, P = T.shape[0], T.shape[4]
+    lib = _lib.load()
+    with torch.cuda.device(T.device):
+        spare = torch.empty_like(T)
+        for k in range(steps):
+            _lib.check(lib.b200drr_svf_square_tangents(_ptr(levels[k]), _ptr(T), _ptr(spare), None, Bm, P, *T.shape[1:4], *dims,
+                                                       _scale(k, steps), _stream()), "b200drr_svf_square_tangents")
+            T, spare = spare, T
+    return T
+
+
+def se3_log_tangents(Y, dY):
+    """The derivative of se3_log_matrix at Y (..., 4, 4) along dY (the same shape), float64, by forward-mode AD through its closed
+    form (torch.func.jvp): finite at the identity, where registration starts, and no host sync."""
+    return torch.func.jvp(se3_log_matrix, (Y.double(),), (dY.double(),))[1]
+
+
+def velocity_tangents(drr, X, weights, pivots):
+    """The derivatives of polyrigid_velocity along the 6K motion increments (DESIGN.md 6p) -> (Bm, g0, g1, g2, 6K, 4) fp32, voxel
+    units, node-major, lane 3 zero: tangent p = 6k + i at node x is w_k(x) (dL_k / d xi_ki) [x; 1] with
+    dL_k / d xi_ki = A^-1 Dlog|_{X_k^-1}[-X_k^-1 T(c_k) E_i T(-c_k)] A, the left increment X_k(xi) = T(c_k) exp(xi^) T(-c_k) X_k about
+    the pivot c_k of polyrigid_tangents (its inner matrix).  X (K, 4, 4) or (B, K, 4, 4); pivots (K, 3) float64.  Dlog in float64."""
+    from .structures import _translation, twist_matrix
+
+    A = drr._affine.reshape(4, 4).double()
+    Ainv = torch.linalg.inv_ex(A).inverse
+    Xinv = _rigid_inverse(X.detach().double())
+    Xinv = Xinv if Xinv.dim() == 4 else Xinv[None]                                          # (Bm, K, 4, 4)
+    E = twist_matrix(torch.eye(6, dtype=torch.float64, device=Xinv.device))                 # (6, 4, 4)
+    dXinv = -(Xinv @ _translation(pivots))[:, :, None] @ E @ _translation(-pivots)[None, :, None]   # (Bm, K, 6, 4, 4)
+    dL = Ainv @ se3_log_tangents(Xinv[:, :, None].expand_as(dXinv).contiguous(), dXinv) @ A
+    dL = dL[..., :3, :].float()                                                             # (Bm, K, 6, 3, 4)
+    Bm, K = dL.shape[:2]
+    g = tuple(weights.shape[1:])
+    D = drr.density.shape
+    axes = [((torch.arange(g[a], dtype=torch.float64, device=dL.device) + 0.5) * (D[a] / g[a]) - 0.5).float() for a in range(3)]
+    xh = torch.nn.functional.pad(torch.stack(torch.meshgrid(*axes, indexing="ij"), -1).reshape(-1, 3), (0, 1), value=1.0)
+    t = torch.einsum("bkirc,nc->bnkir", dL, xh) * weights.reshape(K, -1).T[None, :, :, None, None]
+    return torch.nn.functional.pad(t.reshape(Bm, *g, 6 * K, 3), (0, 1)).contiguous()
+
+
 def render_log_euclidean(drr, args, X, B, weights, steps, parameterization, convention, degrees, calibration, n_points, alphamin,
                          alphamax, vol):
     """render_polyrigid(blend="log_euclidean") after its checks: exp of polyrigid_velocity, marched by render_deformed through the

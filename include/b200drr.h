@@ -820,6 +820,34 @@ int b200drr_deform_jvp_v16(const void *vol, const void *packed, int vol_type, in
                            const float *alpha_range, void *stream);
 
 /*
+ * Per-pixel Jacobian of the deformable render along P = 6K field tangents (DESIGN.md 6p), for Levenberg-Marquardt on the K motions
+ * of a log-Euclidean blended-rigid render (the field is the exponential of their blended velocity, the tangents its derivatives
+ * along the 6K motion increments).  Arguments as b200drr_deform_fwd's, on a full row-major H x W grid only (N = H * W, H, W > 0),
+ * plus tangents [Bf][g0][g1][g2][P][4] fp32, node-major (with P = 1 the field's layout; voxel-index units, lane 3 ignored, the
+ * field's Bf, 16-byte aligned, fewer than 2^31 floats per pose).  Per pose b, structure k, pixel n and i < 6, p = 6k + i:
+ *     J[b][k][n][i] = raylen * step * sum_m grad tri(V)(y_m) . t_p(x_m),
+ * summed over b200drr_deform_jvp's samples: jv of that entry point along tangent p, to fp32 reordering.  t_p is not interpolated
+ * per sample: the march sums w_c(x_m) grad tri(V)(y_m) per lattice corner c while the samples stay in one cell and contracts the
+ * sums with t_p(c) when the cell changes, so sum_n gout_n J[b][.][n][.] is <g_field of b200drr_deform_bwd, t_p> to fp32 reordering.
+ * Outputs, all OVERWRITTEN: img [B][H*W], b200drr_deform_fwd's out bit for bit; J [B][K][H*W][6]; rects [B][K][4] int32
+ * {w0, w1, h0, h1} (inclusive; empty as {W, -1, H, -1}), the bounding rectangle of the pixels whose ray contracted a nonzero
+ * tangent of one of structure k's six: J[b][k] is exactly zero outside it (the contract of b200drr_ncc_normal_structures with
+ * S = K).  The entry sets the rects empty on the stream, then grows them with integer atomic min / max: every output repeats bit
+ * for bit.  A null pointer, H * W = 0, P outside 1..48, P != 6 K, a misaligned tangents array, J or img aliasing the tangents or
+ * a bad vol_type returns B200DRR_EINVAL; K > 8 or a tangents array of 2^31 floats or more per pose B200DRR_EUNSUPPORTED; the field
+ * and ray checks are b200drr_deform_fwd's; all before touching CUDA.  The library allocates nothing.  The _v16 twin reads a 16-bit
+ * volume and equals the fp32 call on the up-cast volume.
+ */
+int b200drr_deform_jac(const float *vol, const float *packed, int D0, int D1, int D2, const float *src, const float *tgt,
+                       const float *raylen, const float *field, int Bf, int g0, int g1, int g2, const float *tangents, int P, int K,
+                       float *img, float *J, int32_t *rects, int B, int H, int W, float voxel_shift, float eps, int n_points,
+                       const float *alpha_range, void *stream);
+int b200drr_deform_jac_v16(const void *vol, const void *packed, int vol_type, int D0, int D1, int D2, const float *src, const float *tgt,
+                           const float *raylen, const float *field, int Bf, int g0, int g1, int g2, const float *tangents, int P, int K,
+                           float *img, float *J, int32_t *rects, int B, int H, int W, float voxel_shift, float eps, int n_points,
+                           const float *alpha_range, void *stream);
+
+/*
  * Backprojection through the deformable render (DESIGN.md 6l): the transpose of b200drr_deform_fwd in the density, for
  * reconstruction through known (or jointly fitted) displacement fields.  For a fixed camera and field the render is linear in V:
  *     out = raylen * step * sum_m tri(V, y_m),      y_m = x_m + u(x_m),
@@ -870,6 +898,18 @@ int b200drr_svf_square_bwd(const float *field, const float *gout, float *gin, in
  */
 int b200drr_svf_square_jvp(const float *field, const float *tangent, float *tout, float *out /* nullable */, int Bf, int g0, int g1,
                            int g2, int D0, int D1, int D2, float scale, void *stream);
+
+/*
+ * b200drr_svf_square_jvp for P tangents at once (DESIGN.md 6p): tangents and tout [Bf][g0][g1][g2][P][4] fp32, node-major (the P
+ * tangents of a node are contiguous; with P = 1 the field's layout).  Slice p of tout equals b200drr_svf_square_jvp on slice p of
+ * tangents bit for bit: y, its cell and J_U are formed once per node and the per-tangent arithmetic is that entry point's, in the
+ * same order.  out (NULL skips it) receives b200drr_svf_square's out bit for bit.  tout and out are OVERWRITTEN, lane 3 zero.
+ * tangents, tout and out 16-byte aligned, tout and out aliasing neither input nor each other.  The refusals are
+ * b200drr_svf_square_jvp's, plus P outside 1..48 (B200DRR_EINVAL) and a tangents array of 2^31 floats or more per pose
+ * (B200DRR_EUNSUPPORTED), all before touching CUDA.  The library allocates nothing.
+ */
+int b200drr_svf_square_tangents(const float *field, const float *tangents, float *tout, float *out /* nullable */, int Bf, int P,
+                                int g0, int g1, int g2, int D0, int D1, int D2, float scale, void *stream);
 
 #ifdef __cplusplus
 }

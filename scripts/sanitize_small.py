@@ -210,4 +210,19 @@ for kw in (dict(), dict(p_subsample=0.37), dict(patch_size=8, height=24)):
                 img.sum().backward()
                 torch.cuda.synchronize()
                 print("polyrigid_bproj", kw, K, shape, joint, "ok", float(img.sum()), float(V.grad.abs().max()))
+# log-Euclidean motion Jacobian (svf.cu: svf_square_tangents_kernel; deform.cu: deform_jac_kernel): the 23 x 23 detector (partial
+# 16 x 8 tiles), a 7 x 5 x 9 lattice (partial CTA), K = 3 and 6 (both register paddings), per-pose and shared motions, a structure
+# pulled from outside the volume, fp32 and bf16 densities
+for dtype in (torch.float32, torch.bfloat16):
+    drr = DRR(synthetic.make_subject(vol), **synthetic.detector_kwargs(23), renderer="trilinear").to(dev)
+    drr.density = drr.density.to(dtype)
+    for K in (3, 6):
+        W = torch.rand(K, 7, 5, 9, device=dev) / K
+        for shape in ((rot.shape[0], K, 6), (K, 6)):
+            xi = (torch.rand(*shape, device=dev) - 0.5) * torch.tensor([0.1, 0.1, 0.1, 8.0, 8.0, 8.0], device=dev)
+            xi[..., 0, 3] += 300.0
+            img, J, rects = drr.polyrigid_jacobian(rot, xyz, motions=se3_exp(xi), weights=W, n_points=64, return_footprints=True,
+                                                   blend="log_euclidean", steps=4, parameterization="euler_angles", convention="ZXY")
+            torch.cuda.synchronize()
+            print("log_euclidean_jac", dtype, K, shape, "ok", float(img.sum()), float(J.abs().max()), rects.tolist())
 print("done")

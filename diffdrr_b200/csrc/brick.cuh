@@ -718,12 +718,16 @@ B200_HD VolFrame unpack_sens_frame(const SensFrameRec& r, const float inv[3], fl
 // so M goes into the key (bin = M * 10 + one of 10 length bins, longest first within each M): warps are M-uniform except at
 // the group boundaries.  M comes from the ray table's 1/d (largest |d| = smallest |1/d|, ties to the lower axis as in
 // siddon_ray_sens_box); a rounding near 45 degrees only costs a divergent warp, the walk itself decides on d.
+// A length bin is U voxels of the chord's L1 length wide, the length of one walk group of U steps: a pair visits about one voxel
+// per unit of L1 length, so the pairs of a bin mostly run the same number of groups, and a 32-item chunk, which runs until its
+// longest pair is done, pads few of its lanes (CPU emulation of the bench's lists, DESIGN.md 4.2b).
 constexpr int kSensLenBins = 10;
-B200_HD int sens_bin(const float inv[3], float a_in, float a_out, float sumabs_d, float inv_width)
+template <int U>
+B200_HD int sens_bin(const float inv[3], float a_in, float a_out, float sumabs_d)
 {
     const float i0 = fabsf(inv[0]), i1 = fabsf(inv[1]), i2 = fabsf(inv[2]);
     const int M = (i0 <= i1 && i0 <= i2) ? 0 : (i1 <= i2 ? 1 : 2);
-    const int b = step_bin(a_in, a_out, sumabs_d, inv_width);
+    const int b = step_bin(a_in, a_out, sumabs_d, 1.0f / (float)U);
     return M * kSensLenBins + (b < kSensLenBins - 1 ? b : kSensLenBins - 1);
 }
 

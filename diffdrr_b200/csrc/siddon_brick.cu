@@ -296,7 +296,6 @@ __global__ void __launch_bounds__(THREADS, CTAS)
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int n_bricks = bg.nb0 * bg.nb1 * bg.nb2;
     const float inv_bin_width = (float)kBrickBins / (float)(BX + BY + BZ + 8);
-    const float inv_sens_width = (float)kSensLenBins / (float)(BX + BY + BZ + 8);
 
     if (tid == 0) {
 #pragma unroll
@@ -637,7 +636,7 @@ __global__ void __launch_bounds__(THREADS, CTAS)
                                 const float clo3[3] = {clo.x, clo.y, clo.z}, chi3[3] = {chi.x, chi.y, chi.z};
                                 float a_in, a_out;
                                 if (brick_maybe_hit(inv, clo3, chi3, a_in, a_out)) {
-                                    const int bin = SENS ? sens_bin(inv, a_in, a_out, q.w, inv_sens_width)
+                                    const int bin = SENS ? sens_bin<U>(inv, a_in, a_out, q.w)
                                                          : step_bin(a_in, a_out, q.w, inv_bin_width);
                                     items[j] = pack_item(bin, bl, n);
                                     atomicAdd(&s_hist[bin], 1);
